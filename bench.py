@@ -1,12 +1,19 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native NeRF-LOAM hot path (BASELINE.json metric):
+"""bench.py -- headline benchmark of the H100-native NeRF-LOAM hot path (BASELINE.json metric):
 neural-SDF samples/s per mapping iteration on a synthetic 100k-ray KITTI-shape scan.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one full mapping iteration of bundle_adjust_frames' loop body on every ray of one scan per GPU:
 pose -> rays -> octree traversal -> inverse-CDF sampling -> embedding gather + trilinear -> 16-256-256-1 MLP
 -> SDF/free-space loss -> backward (decoder, embeddings, pose) -> Adam on all three.  Prints ONE JSON line.
+
+--dump-outputs DIR: right after the K timed steps, the same step runs once more from the benchmark's seeded starting state
+(map, embeddings, decoder, pose, fresh Adam state) and what it computed -- per-sample SDF and voxel ids, loss statistics,
+updated decoder, pose and embedding table (a fixed, seeded sample of its rows when it is large) -- is written as
+DIR/<name>.npy.  Its inputs are identical from run to run, so two builds run with the same arguments can be compared output
+for output.  (The timed steps themselves drift apart between runs: their gradient sums use fp32 atomics, and Adam turns
+last-bit differences of near-zero gradients into steps of the full learning rate.)
 """
 import argparse
 import json
@@ -26,8 +33,11 @@ LR = (0.01, 0.005, 0.001)                     # kitti.yaml learning_rate_emb / _
 BYTES_PER_SAMPLE_MAP = 1116                   # BASELINE.md: algorithmic HBM bytes / valid sample, MAP mode
 FLOPS_PER_SAMPLE_MAP_DEC = 419328             # BASELINE.md: MLP fwd + bwd-data + bwd-weight
 # tf32 tensor-core FLOPs actually issued per sample for that fp32-parity result: 3 terms (hi*hi, hi*lo, lo*hi) for layer 1/2
-# forward, backward layer 1 and gW0|gb0 (N = 32); 2 terms for backward layer 2 and gW1 (one operand is the exact 0/1 ReLU mask)
-ISSUED_TF32_FLOPS_PER_SAMPLE = 2 * (3 * 16 * 256 + 3 * 256 * 256 + 2 * 256 * 256 + 3 * 256 * 16 + 2 * 256 * 256 + 3 * 256 * 32)
+# forward and backward layer 1; 2 terms for backward layer 2 (one operand is the exact 0/1 ReLU mask).  The weight gradients
+# run on the fp32 CUDA cores.
+ISSUED_TF32_FLOPS_PER_SAMPLE = 2 * (3 * 16 * 256 + 3 * 256 * 256 + 2 * 256 * 256 + 3 * 256 * 16)
+N_SETTLE = 24                                 # untimed steps between warm-up and the clock (a fixed count: outputs reproducible)
+DUMP_EMB_ROWS = 1 << 19                       # embedding rows written by --dump-outputs (a seeded sample when the table is larger)
 WORKLOAD = "synthetic 100k-ray KITTI-shape scan (64x1563 beams, 82.7k returns), single-scan 0.3 m map, " \
            "mapping iteration on ALL rays, decoder+embeddings+pose updated, Adam included"
 
@@ -37,7 +47,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet (700 W), not measured")
 
 
 class ClockSampler:
@@ -98,19 +108,6 @@ def host_rays(pts, cos):
     return dirs.pin_memory(), gt.pin_memory(), torch.from_numpy(cos).float().contiguous().pin_memory()
 
 
-def _traffic_record(kernel_key):
-    """dram bytes per launch of the dominant kernel from the committed ncu capture of THIS build (profiles/r02_traffic.json, written by
-    scripts/summarise_profiles.py from an `ncu --set full` report); None when no capture is recorded."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if not os.path.exists(p):
-        return None, None
-    d = json.load(open(p))
-    rec = d.get(kernel_key)
-    if not rec:
-        return None, None
-    return rec.get("dram_bytes"), {"ncu_report": rec.get("report"), "read": rec.get("read"), "write": rec.get("write"), "samples": rec.get("samples")}
-
-
 def run_ours(args):
     import nerfloam_b200 as nl
     rank = int(os.environ.get("RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1)); local = int(os.environ.get("LOCAL_RANK", 0))
@@ -134,6 +131,7 @@ def run_ours(args):
     bufs = nl.engine.DecoderBuffers(dec, dev)
     emb = ms.emb
     state = {"opt": None}
+    start = (emb.clone(), [p.detach().clone() for p in bufs.params], pose6.clone())
     # multi-GPU: the embedding-gradient reduction fused with the table's Adam step over NVLink peer memory (csrc/peer.cu) and the
     # statistics exchange through symmetric memory, instead of NCCL all-reduces (NL_PEER=0: plain NCCL, the baseline)
     peer = pstats = None
@@ -197,31 +195,28 @@ def run_ours(args):
     W = max(args.warmup, 3)
     for _ in range(W):
         step(d_dirs, d_gt, d_cos)
-    # settle: clocks, allocator, NCCL channels and the two-stream pipeline reach steady state before the clock starts (untimed, >= 100 ms)
-    sync_all()
-    t_s = time.perf_counter()
-    n_settle = 0
-    while time.perf_counter() - t_s < 0.10:
-        for _ in range(8):
-            step(d_dirs, d_gt, d_cos)
-        torch.cuda.synchronize()
-        n_settle += 8
-    if world > 1:       # same number of settle steps on every rank (collectives inside)
-        import torch.distributed as dist
-        t_n = torch.tensor([n_settle], device=dev); dist.all_reduce(t_n, op=dist.ReduceOp.MAX)
-        for _ in range(int(t_n.item()) - n_settle):
-            step(d_dirs, d_gt, d_cos)
-        n_settle = int(t_n.item())
+    # settle: clocks, allocator, NCCL channels and the two-stream pipeline reach steady state before the clock starts (untimed)
+    n_settle = N_SETTLE
+    for _ in range(n_settle):
+        step(d_dirs, d_gt, d_cos)
     l0 = nl._capi.LAUNCHES
     ms_total = timed(lambda: step(d_dirs, d_gt, d_cos), args.steps, eng.join_side)   # deferred decoder work of the last iteration is inside
     launches = nl._capi.LAUNCHES - l0
     st = eng.read_stats()
     n_local = st.n_samples
-    # ---------------- the same loop over >= 250 ms with one event per step: median / max (what a 32 ms window cannot show) ----------------
-    n_long = max(args.steps, int(0.25 / max(ms_total / args.steps * 1e-3, 1e-6)) + 1)
-    if world > 1:
-        import torch.distributed as dist
-        t_n = torch.tensor([n_long], device=dev); dist.all_reduce(t_n, op=dist.ReduceOp.MAX); n_long = int(t_n.item())
+    if args.dump_outputs:           # one more step from the starting state (every rank: the step has collectives inside)
+        emb.copy_(start[0])
+        for p, p0 in zip(bufs.params, start[1]):
+            p.data.copy_(p0)
+        pose6.copy_(start[2])
+        state["opt"] = None
+        step(d_dirs, d_gt, d_cos)
+        eng.join_side()
+        sync_all()
+        if rank == 0:
+            dump_outputs(args.dump_outputs, eng, eng.read_stats(), bufs, pose6, emb)
+    # ---------------- the same loop with one event per step: median / max ----------------
+    n_long = args.steps
     sync_all()
     evs = [torch.cuda.Event(enable_timing=True) for _ in range(n_long + 1)]
     evs[0].record()
@@ -340,7 +335,6 @@ def run_ours(args):
     ach_tf = flops / (t_mlp * 1e-3) / 1e12
     gather_gbs = n_local * BYTES_PER_SAMPLE_MAP / ((t_gf + t_gb) * 1e-3) / 1e9
     tc = nl.engine.mlp_impl(256) == "tc"
-    traffic, traffic_src = _traffic_record("k_mlp_tc_train" if tc else "k_mlp")
     long_stats["value_from_median"] = n_total / (long_stats["ms_median"] * 1e-3)
     out = {
         "metric": "neural-SDF samples/sec per mapping iter", "value": value, "unit": "samples/s", "n_gpus": world, "steps": args.steps,
@@ -352,7 +346,7 @@ def run_ours(args):
                                   f": the batch is a window of {world} scans (all rays), split contiguously = one scan per rank; per step: statistics exchange, "
                                   "embedding-gradient reduction (fused with Adam over NVLink peer memory when multi_gpu_exchange.fused_reduce_adam), "
                                   "decoder-gradient all-reduce (NCCL, side stream)"),
-                   "l2": "per-step working set (samples x ~2.2 KB activations+features) ~1.9 GB >> 126 MB L2; no flush needed",
+                   "l2": "per-step working set (samples x ~4 KB activations+features) >> 50 MB L2; no flush needed",
                    "sampler_noise": "in-kernel counter RNG", "loss": loss_val,
                    "untimed_before_clock": f"{W} warm-up steps + {n_settle} settle steps (>= 100 ms)",
                    "kernel_error_bits_over_all_steps": ctl[nl._capi.CTL_ERROR], "skipped_steps": ctl[nl._capi.CTL_SKIPPED],
@@ -362,11 +356,10 @@ def run_ours(args):
         "gpu_launches": int(launches),
         "steady_state": long_stats,
         "roofline": {"bound": "tensor",
-                     "kernel": ("tc::k_mlp_tc_train<wgrad> + tc::k_dw1_tc + tc::k_dw0_tc (+ k_mask_colsum) (tcgen05.mma kind::tf32, 3-term hi/lo split; 2 terms where "
-                                "one operand is the exact 0/1 ReLU mask)"
+                     "kernel": ("tc::k_mlp_wg<train,wgrad> (wgmma tf32, 3-term hi/lo split; 2 terms where one operand is the exact 0/1 ReLU "
+                                "mask) + k_dw1 + tc::k_wg_cols (fp32 CUDA-core weight gradients)"
                                 if tc else "k_mlp<256,train,wgrad> + k_dw1 (fp32 CUDA-core FMA)"),
                      "achieved": ach_tf, "peak": pk["bf16_sustained"], "unit": "TFLOP/s", "frac": ach_tf / pk["bf16_sustained"],
-                     "traffic": traffic, "traffic_source": traffic_src,
                      "peak_source": pk["src"] + " dense bf16 cuBLAS (sustained).  The fp32-parity path runs on kind::tf32 (half the bf16 rate); a "
                                     "pure 3xTF32 evaluation (3 passes everywhere) could reach at most 1/6 of this peak = %.0f TFLOP/s of algorithmic "
                                     "fp32 FLOPs; two of the five GEMMs here need only 2 passes (exact 0/1 mask operand), so that figure is a "
@@ -375,9 +368,7 @@ def run_ours(args):
                      "tf32_pipe": {"issued_flops_per_sample": ISSUED_TF32_FLOPS_PER_SAMPLE,
                                    "achieved": n_local * ISSUED_TF32_FLOPS_PER_SAMPLE / (t_mlp * 1e-3) / 1e12,
                                    "peak": pk["bf16_sustained"] / 2, "unit": "TFLOP/s",
-                                   "frac": n_local * ISSUED_TF32_FLOPS_PER_SAMPLE / (t_mlp * 1e-3) / 1e12 / (pk["bf16_sustained"] / 2),
-                                   "note": "the 'sustained' cuBLAS peak was measured power-capped at ~1380 MHz while these kernels run at ~1965 MHz; "
-                                           "the clock-independent figure is ncu's sm__pipe_tensor_cycles_active (profiles/)"},
+                                   "frac": n_local * ISSUED_TF32_FLOPS_PER_SAMPLE / (t_mlp * 1e-3) / 1e12 / (pk["bf16_sustained"] / 2)},
                      "ms_per_launch": t_mlp, "algorithmic_flops_per_sample": FLOPS_PER_SAMPLE_MAP_DEC},
         "roofline_gather": {"bound": "hbm", "kernel": "k_gather_fwd + k_gather_bwd", "achieved": gather_gbs, "peak": pk["hbm"], "unit": "GB/s",
                             "frac": gather_gbs / pk["hbm"], "ms_fwd": t_gf, "ms_bwd": t_gb, "algorithmic_bytes_per_sample": BYTES_PER_SAMPLE_MAP,
@@ -505,9 +496,9 @@ def strong_scaling_block(nl, dev, rank, world, group, scan, ms, dec, steps, sync
 
 
 # ======================================================================================================
-# Baseline B (BASELINE.md section 3): the UNMODIFIED reference on the same B200 -- its eager PyTorch loop
+# Baseline B (BASELINE.md section 3): the UNMODIFIED reference on the same GPU -- its eager PyTorch loop
 # (oracle/_ref/src/variations/render_helpers.py, staged byte for byte) + its own CUDA extension (oracle/_ref/grid/grid_ref.so,
-# compiled for sm_100a from the sources where they lie).  Baseline legs only; never on the product path.
+# compiled for sm_90a from the sources where they lie).  Baseline legs only; never on the product path.
 # ======================================================================================================
 class _TimedExt:
     """Proxy for the reference's `grid` extension that brackets its two live kernels with CUDA events."""
@@ -555,8 +546,8 @@ def reference_gpu(nl, dev, steps, full_scan_pts, window_scans):
     syn = nl.synthetic
     vs = CFG["voxel_size"]
     crit = ref.Criterion(H.args(CFG["max_depth"], CFG["truncation"], CFG["fs_weight"], CFG["sdf_weight"]))
-    out = {"what": "unmodified reference (src/variations/render_helpers.py + voxel_helpers.py + grid CUDA extension built for sm_100a), "
-                   "same B200, same synthetic scans; wall clock between torch.cuda.synchronize() (the reference syncs the host several "
+    out = {"what": "unmodified reference (src/variations/render_helpers.py + voxel_helpers.py + grid CUDA extension built for sm_90a), "
+                   "same GPU, same synthetic scans; wall clock between torch.cuda.synchronize() (the reference syncs the host several "
                    "times per iteration itself)"}
 
     def build_map(scans):
@@ -787,8 +778,8 @@ def best_cpu_baseline(n_rays, iters):
 
 def run_reference(args):
     """Reference arm.  The reference's stock code path for this metric is a GPU path (eager PyTorch + its own CUDA extension), so when
-    the staged reference (oracle/_ref: grid_ref.so built for sm_100a + its unmodified Python) and a GPU are present the line's value
-    is THAT -- Baseline B of BASELINE.md, the same workload, same B200 -- and the CPU port of the path (Baseline A, host cores) is
+    the staged reference (oracle/_ref: grid_ref.so built for sm_90a + its unmodified Python) and a GPU are present the line's value
+    is THAT -- Baseline B of BASELINE.md, the same workload, same GPU -- and the CPU port of the path (Baseline A, host cores) is
     reported beside it in `cpu_baseline`.  Without them the CPU port is the value."""
     rank = int(os.environ.get("RANK", 0))
     if rank != 0:
@@ -814,7 +805,7 @@ def run_reference(args):
         out.update(value=gpu["value"], ms_per_step=gpu["ms_per_step"],
                    config={"workload": WORKLOAD, "rays_per_gpu": gpu["rays"], "samples_per_gpu_step": gpu["samples"],
                            "note": "UNMODIFIED reference (src/variations/render_helpers.py::bundle_adjust_frames + voxel_helpers.py + grid CUDA extension "
-                                   "compiled for sm_100a) on this box's GPU 0: one mapping iteration on all rays of the same scan per step, decoder + "
+                                   "compiled for sm_90a) on GPU 0: one mapping iteration on all rays of the same scan per step, decoder + "
                                    "embeddings + pose updated by torch.optim.Adam; host ray selection skipped (metric definition); wall clock between "
                                    "torch.cuda.synchronize() calls.  cpu_baseline = the oracle's CPU port of the same path on host cores"},
                    e2e={"value": gpu["value"], "unit": "samples/s", "h2d_bytes_per_step": gpu["h2d_bytes_per_step"], "d2h_bytes_per_step": 0,
@@ -865,12 +856,35 @@ def reference_gpu_headline(nl, dev, steps, warmup):
     return {"value": M * steps / dt, "ms_per_step": dt / steps * 1e3, "rays": R, "samples": M, "h2d_bytes_per_step": 0}
 
 
+def dump_outputs(out_dir, eng, st, bufs, pose6, emb):
+    """What a step computed, as float32 / float64 .npy files: under 64 MB in all (32 MB of embedding rows at most,
+    4 + 4 bytes per sample for sdf and voxel id, 2 M samples at most)."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = int(st.n_samples)
+    arrays = {"sdf": eng.sdf[:n], "sample_voxel": eng.s_vox[:n], "pose6": pose6,
+              "loss": torch.tensor([st.loss, st.fs_loss, st.sdf_loss], dtype=torch.float64)}
+    for i, p in enumerate(bufs.params):
+        arrays[f"decoder_param{i}"] = p.data
+    rows = emb.shape[0]
+    if rows > DUMP_EMB_ROWS:
+        idx = np.sort(np.random.default_rng(0).choice(rows, DUMP_EMB_ROWS, replace=False))
+        arrays["embedding_rows"] = torch.from_numpy(idx)
+        arrays["embedding"] = emb[torch.from_numpy(idx).to(emb.device)]
+    else:
+        arrays["embedding"] = emb
+    for k, v in arrays.items():
+        v = v.detach().cpu()
+        v = v.double() if v.dtype in (torch.float64, torch.int64) else v.float()
+        np.save(os.path.join(out_dir, k + ".npy"), v.numpy())
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     a = ap.parse_args()
     # stdout carries exactly one JSON line: while the benchmark runs, file descriptor 1 points at stderr, so that library
     # banners written with printf (NCCL prints its version there) cannot get in front of it

@@ -1,5 +1,5 @@
 /*
- * nerfloam_b200.h -- C ABI of libnerfloam_b200.so: the B200-native (sm_100a) replacement for the
+ * nerfloam_b200.h -- C ABI of libnerfloam_b200.so: the H100-native (sm_90a) replacement for the
  * per-iteration neural-SDF hot path of NeRF-LOAM (SURVEY.md section 8).
  *
  * Conventions
@@ -227,14 +227,14 @@ NL_API int nl_mlp_train(int64_t M, const int32_t *d_M_dev, const float *d_feats,
                  const uint8_t *d_s_flag, const float *d_s_depth, const int32_t *d_s_ray, const float *d_cos,
                  const float *d_gt_depth, nl_render_stats *d_stats, float truncation, float *d_sdf, float *d_dfeats,
                  const nl_mlp_grads *grads, float *d_act_h1, float *d_act_dh2, const float *d_dsdf_ext, void *stream);
-/* Tensor-core (tcgen05 3xTF32) forward for width 256: weights are pre-split into tf32 hi/lo and pre-swizzled
+/* Tensor-core (wgmma 3xTF32) forward for width 256: weights are pre-split into tf32 hi/lo and pre-swizzled
  * into shared-memory panel images by nl_mlp_tc_prepare (nl_mlp_tc_panel_bytes() bytes of device memory). */
 NL_API int64_t nl_mlp_tc_panel_bytes(void);
 NL_API int nl_mlp_tc_prepare(const float *d_W0, const float *d_W1, const float *d_w2, void *d_panels, void *stream);
 NL_API int nl_mlp_tc_forward(int64_t M, const int32_t *d_M_dev, const float *d_feats, const void *d_panels, const float *d_b0,
                       const float *d_b1, const float *d_w2, const float *d_b2, float *d_sdf, void *stream);
 /* Tensor-core forward + loss + backward (same contract as nl_mlp_train, width 256 only).  With grads != NULL d_act is a
- * scratch buffer of nl_mlp_tc_act_floats(M) floats (internal panel-major activations for the weight-gradient GEMMs).
+ * scratch buffer of nl_mlp_tc_act_floats(M) floats (internal activations for the weight-gradient kernels).
  * The panels must have been prepared from the same W0 / W1 / w2 (the backward panels hold diag(w2) W1).
  * wgrad_stream (may be NULL = stream): the weight-gradient kernels are enqueued there, ordered after the forward/backward
  * kernel by an event, so that they overlap with later work on `stream`; the caller joins the two streams before it reads

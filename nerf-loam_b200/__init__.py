@@ -1,4 +1,4 @@
-"""nerf-loam_b200 -- B200-native (sm_100a) neural-SDF LiDAR SLAM inner loop behind NeRF-LOAM's own API.
+"""nerf-loam_b200 -- H100-native (sm_90a) neural-SDF LiDAR SLAM inner loop behind NeRF-LOAM's own API.
 
 The directory name carries the reference's hyphen; import it as `nerfloam_b200` (the alias module at the
 repository root) or with importlib.import_module("nerf-loam_b200").

@@ -1,4 +1,4 @@
-"""Build libnerfloam_b200.so (hand-written sm_100a CUDA + host C++) in-tree with nvcc.
+"""Build libnerfloam_b200.so (hand-written sm_90a CUDA + host C++) in-tree with nvcc.
 
     python nerf-loam_b200/build.py            # incremental
     python nerf-loam_b200/build.py --force
@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libnerfloam_b200.so")
 SOURCES = ["nl_error.cpp", "octree_host.cpp", "grid_dropin.cu", "render.cu", "gather.cu", "mlp.cu", "mlp_tc.cu", "pose.cu", "optim.cu", "mc.cu", "peer.cu", "select.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--extended-lambda", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 
 

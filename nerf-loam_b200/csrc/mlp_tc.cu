@@ -1,54 +1,56 @@
-// Tensor-core version of the SDF decoder MLP (16 -> 256 -> 256 -> 1, ReLU) for sm_100a:
-// tcgen05.mma kind::tf32 with a 3-term hi/lo split (3xTF32: a*b ~= ah*bh + ah*bl + al*bh, fp32
-// accumulation in TMEM), which keeps the result within ~1e-6 of an fp32 evaluation -- single-pass
-// TF32/BF16 (1e-3) would break the 1e-5 SDF parity bar.
+// Tensor-core version of the SDF decoder MLP (16 -> 256 -> 256 -> 1, ReLU) for sm_90a: Hopper wgmma (m64nNk8, tf32
+// inputs, fp32 accumulation in registers) with a 3-term hi/lo split (3xTF32: a*b ~= ah*bh + ah*bl + al*bh), which keeps
+// the result within ~1e-6 of an fp32 evaluation -- single-pass TF32 (1e-3) would break the 1e-5 SDF parity bar.
 //
-// One persistent CTA per SM, 6 warps:
-//   warp 0   producer : streams pre-swizzled weight panels (hi+lo, 64 KB per K-block of 32) from L2 into a
-//                       2-stage shared-memory ring with cp.async.bulk (1-D TMA) + mbarrier complete_tx
-//   warp 1   MMA      : one elected thread issues tcgen05.mma (M=128 samples, N=256, K=8 per instruction),
-//                       releases ring stages with tcgen05.commit; owns the TMEM allocation (512 columns:
-//                       D1 = layer-1 accumulator, D2 = layer-2 accumulator)
-//   warps 2-5 epilogue: thread = sample row (TMEM lane).  Loads x, and for every K-block of layer 2 pulls 32
-//                       columns of D1 out of TMEM (tcgen05.ld), applies bias+ReLU, splits into tf32 hi/lo and
-//                       writes the A operand tile straight into the 128B-swizzled K-major layout the tensor
-//                       core reads; finally reduces relu(D2 + b1) . w2 + b2 per row.
-// Layer 1 (K = 16) runs through the same ring as one extra K-block with 2 k-steps.
-// Shared memory: 2 x 64 KB weight stages + 2 x 32 KB activation stages = 192 KB.
-#include <cstdlib>
+// One persistent CTA per SM, two warpgroups; each warpgroup owns 64 samples of a 128-sample tile end to end.
+//   * A operands come from registers.  A layer's fp32 accumulator fragment (thread holds columns 8j+2t, 8j+2t+1 of rows g
+//     and g+8) is, up to a fixed permutation of K inside every group of 8 (kperm), the tf32 A fragment of the next GEMM
+//     (columns t, t+4), so activations never go through shared memory.  The weight panels carry the same permutation.
+//   * B operands (weights, pre-split into tf32 hi/lo and pre-swizzled into the 128B-swizzle K-major image wgmma reads,
+//     k_tc_prepare) stream from L2 through a 4-slot shared-memory ring: 1-D bulk copies (TMA) completing on mbarriers,
+//     issued by thread 0 up to 3 slots ahead; a slot is refilled once the wgmmas of all 8 warps that read it retired.
+//   * Every N = 256 GEMM runs as two N = 128 halves, so the previous layer's activations (128 registers per thread) and
+//     one accumulator half (64) fit in the register file together.
+// Per 128-sample training tile the ring carries 42 items: layer 1 (2 halves), layer 2 (2 halves x 8 K-blocks of 32),
+// backward layer 2 (2 x 8) and backward layer 1 (8 K-blocks, N = 16).
+//
+// Decoder weight gradients (nl_mlp_tc_train with grads): the training kernel stores h1, h2, dh2, dh1 [cap][256] and
+// d loss / d sdf; gW1 = dh2^T h1 (K = samples) is a split-K 3xTF32 tensor-core GEMM (k_dw1_tc, mma.sync m16n8k8: both
+// operands are sample-major, which wgmma's tf32 forms cannot read), the column sums and gW0 (K = 16) come from one
+// streaming pass (k_wg_cols).
 #include <mutex>
 
 #include "nl_cuda.cuh"
 
 namespace tc {
 
-constexpr int TM = 128;               // samples per tile (UMMA M)
-constexpr int WN = 256;               // hidden width (UMMA N)
-constexpr int PANEL_A = TM * 128;     // 16 KB : 128 rows x 128 B (32 tf32 of K)
-constexpr int PANEL_B = WN * 128;     // 32 KB : 256 rows x 128 B
-constexpr int STAGE_A = 2 * PANEL_A;  // hi + lo
-constexpr int STAGE_B = 2 * PANEL_B;
-constexpr int NSTAGE = 2;
-constexpr int STEPS_FWD = 9;          // layer 1 + 8 K-blocks of layer 2
-constexpr int STEPS_TRAIN = 25;       // + 8 K-blocks of backward layer 2 + 8 of backward layer 1
-constexpr int PANEL_B16 = 16 * 128;   // 2 KB: the 16-row panels of backward layer 1
-constexpr int SMEM_DATA = NSTAGE * (STAGE_A + STAGE_B);
-constexpr int SMEM_TOTAL = SMEM_DATA + 8192 + 1024;  // + biases/barriers/exchange + alignment slack
-constexpr int NTHREADS_TRAIN = 320;   // producer warp, MMA warp, 2 groups of 4 epilogue warps
-constexpr int NTHREADS = 192;
+constexpr int TM = 128;                  // samples per CTA tile (2 warpgroups x 64)
+constexpr int WN = 256;                  // hidden width
+constexpr int PANEL_B = WN * 128;        // 32 KB: one weight K-block (256 rows x 32 tf32), hi or lo
+constexpr int STAGE_B = 2 * PANEL_B;     // hi + lo, in global memory
+constexpr int HALF = 128 * 128;          // 16 KB: 128 rows of a panel (one N = 128 half)
+constexpr int SLOT = 2 * HALF;           // ring slot: hi half | lo half
+constexpr int NSLOT = 4;
+constexpr int STEPS_TRAIN = 25;          // panel stages: layer 1, 8 x layer 2, 8 x backward layer 2, 8 x backward layer 1
+constexpr int ITEMS_FWD = 18;
+constexpr int ITEMS_TRAIN = 42;
+constexpr int NTHREADS = 256;
+constexpr int SMEM_TOTAL = NSLOT * SLOT + 3 * WN * 4 + 256 + 1024;   // ring + biases/w2 + barriers + alignment slack
 
 // byte offset of 16-byte chunk c (0..7) of row r inside a K-major SWIZZLE_128B panel
 __host__ __device__ __forceinline__ int panel_off(int r, int c) { return (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4); }
+// logical K index stored at panel position k: inside every group of 8, positions 0..3 hold the even, 4..7 the odd columns
+__host__ __device__ __forceinline__ int kperm(int k) { const int p = k & 7; return (k & ~7) | (p < 4 ? 2 * p : 2 * (p - 4) + 1); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ float tf32_rna(float x) {
+__device__ __forceinline__ uint32_t tf32_rna(float x) {
     uint32_t u;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-    return __uint_as_float(u);
+    return u;
 }
 
-// ---- mbarrier helpers -------------------------------------------------------------------------
+// ---- mbarrier / bulk-copy helpers ------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
@@ -57,6 +59,14 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("{ .reg .b64 st; mbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1; }" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+    return ok != 0;
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
@@ -71,91 +81,66 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
                  "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+
+// ---- wgmma -------------------------------------------------------------------------------------------
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90): start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled
+// K-major, 1), SBO>>4 = 1024>>4 [32,46) (8-row core-matrix groups), layout SWIZZLE_128B = 1 [62,64).  One k-step of 8 tf32
+// is 32 bytes further along the row: +2 in the address field.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// the same arrive delivered to the barrier at this offset in BOTH CTAs of a 2-CTA cluster (weight stages shared by multicast)
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"((uint16_t)3) : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit_wait() {
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
-// bulk copy global -> the same shared-memory offset of both CTAs of the pair; each CTA's barrier at `bar` receives the bytes
-__device__ __forceinline__ void bulk_g2s_pair(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar), "h"((uint16_t)3) : "memory");
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1));
 }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_cta_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1));
 }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30)
-// (ignored for swizzled K-major, set to 1), SBO>>4 = 1024>>4 [32,46), version 1 [46,48), layout SWIZZLE_128B = 2 [61,64)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 = 1 [4,6), a/b_format TF32 = 2 [7,10)/[10,13),
-// a/b K-major = 0, N>>3 [17,23), M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc),
-        "r"(accumulate) : "memory");
-}
-// One lane of a converged warp.  The single-thread roles (MMA issue, bulk copies) run their loops warp-uniformly and
-// predicate only the issuing instruction: every operand then lives in uniform registers and the compiler emits a plain
-// UTCHMMA / UBLKCP instead of a per-thread serialisation loop (R2UR + ELECT + BRA.U.ANY, ~100 cycles per MMA).
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// all MMAs of one K-block: NTERM tf32 terms (hi*hi, hi*lo, lo*hi) x NK k-steps of 8, fully unrolled
-template <int NK, int NTERM>
-__device__ __forceinline__ void issue_kblock(uint32_t d, uint32_t a_hi, uint32_t b_hi, uint32_t idesc, uint32_t acc) {
-    const uint64_t adh = make_desc(a_hi), adl = make_desc(a_hi + PANEL_A), bdh = make_desc(b_hi), bdl = make_desc(b_hi + PANEL_B);
+// A fragment of k-step j of `h` (a 256-column array in accumulator layout, index 4j + x: x = 0,1 row g columns 8j+2t, +1;
+// x = 2,3 row g+8) as tf32 hi and lo parts.  Hardware K position t holds column 8j+2t, t+4 holds 8j+2t+1 (see kperm).
+__device__ __forceinline__ void frag3(const float (&h)[128], int j, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+    const float v[4] = {h[4 * j], h[4 * j + 2], h[4 * j + 1], h[4 * j + 3]};
 #pragma unroll
-    for (int term = 0; term < NTERM; ++term) {
-        const uint64_t ad = (term == 2) ? adl : adh, bd = (term == 1) ? bdl : bdh;
-#pragma unroll
-        for (int ks = 0; ks < NK; ++ks) {
-            mma_tf32(d, ad + 2 * ks, bd + 2 * ks, idesc, acc);
-            acc = 1u;
-        }
+    for (int i = 0; i < 4; ++i) {
+        hi[i] = tf32_rna(v[i]);
+        lo[i] = tf32_rna(v[i] - __uint_as_float(hi[i]));
     }
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-        "%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// D[64 x N] += A x B with 3 terms: ah*bh + ah*bl + al*bh
+template <int NACC>
+__device__ __forceinline__ void mma3(float (&d)[NACC], const uint32_t (&a)[4], const uint32_t (&l)[4], uint64_t bh, uint64_t bl) {
+    if constexpr (NACC == 64) {
+        wgmma_n128(d, a[0], a[1], a[2], a[3], bh);
+        wgmma_n128(d, a[0], a[1], a[2], a[3], bl);
+        wgmma_n128(d, l[0], l[1], l[2], l[3], bh);
+    } else {
+        wgmma_n16(d, a[0], a[1], a[2], a[3], bh);
+        wgmma_n16(d, a[0], a[1], a[2], a[3], bl);
+        wgmma_n16(d, l[0], l[1], l[2], l[3], bh);
+    }
 }
+template <int NACC>
+__device__ __forceinline__ float (&sub64(float (&a)[NACC], int off))[64] { return *reinterpret_cast<float(*)[64]>(a + off); }
 
 // ------------------------------------------------------------------------------------------------
-// Weight panels: the exact shared-memory image (K-major, 128B swizzle, tf32 hi then lo) of every weight
-// K-block, laid out contiguously in global memory so one bulk copy fills a ring stage.
+// Weight panels: the exact shared-memory image (K-major, 128B swizzle, K permuted by kperm, tf32 hi then lo) of every
+// weight K-block, laid out contiguously in global memory so that bulk copies fill a ring slot.
 //   stage 0       : W0  [256 x 16]  (row j, k = e; only the first 64 B of each 128 B row are meaningful)
 //   stage 1 + kb  : W1[:, 32kb : 32kb+32]              forward layer 2
-//   stage 9 + jb  : (diag(w2) W1)^T[:, 32jb : 32jb+32] backward layer 2 (d h1 = dsdf * relu'(h2) . diag(w2) W1, see k_mlp_tc_train)
+//   stage 9 + jb  : (diag(w2) W1)^T[:, 32jb : 32jb+32] backward layer 2 (d h1 = dsdf * (relu'(h2) . diag(w2) W1) * relu'(h1))
 //   stage 17 + kb : W0^T[:, 32kb : 32kb+32] (16 rows)  backward layer 1 (d x  = d h1 . W0)
 // ------------------------------------------------------------------------------------------------
 __global__ void k_tc_prepare(const float *__restrict__ W0, const float *__restrict__ W1, const float *__restrict__ w2,
@@ -165,215 +150,31 @@ __global__ void k_tc_prepare(const float *__restrict__ W0, const float *__restri
     if (t >= WN * 8) return;
     const int r = t >> 3, c = t & 7;
     float v[4] = {0.f, 0.f, 0.f, 0.f};
-    if (stage == 0) {                                     // layer 1:   B[j][e] = W0[j][e]
-        if (c < 4) for (int i = 0; i < 4; ++i) v[i] = W0[r * 16 + c * 4 + i];
-    } else if (stage <= 8) {                              // layer 2:   B[j][k] = W1[j][k],      k in K-block stage-1
-        const int k0 = (stage - 1) * 32 + c * 4;
-        for (int i = 0; i < 4; ++i) v[i] = W1[(size_t)r * WN + k0 + i];
-    } else if (stage <= 16) {                             // bwd layer 2: B[k][j] = w2[j] W1[j][k], j in K-block stage-9
-        const int j0 = (stage - 9) * 32 + c * 4;
-        for (int i = 0; i < 4; ++i) v[i] = __fmul_rn(w2[j0 + i], W1[(size_t)(j0 + i) * WN + r]);
-    } else {                                              // bwd layer 1: B[e][k] = W0[k][e],    k in K-block stage-17 (16 rows)
-        if (r >= 16) return;
-        const int k0 = (stage - 17) * 32 + c * 4;
-        for (int i = 0; i < 4; ++i) v[i] = W0[(size_t)(k0 + i) * 16 + r];
+    if (stage >= 17 && r >= 16) return;
+    for (int i = 0; i < 4; ++i) {
+        const int k = kperm(c * 4 + i);                   // logical K index inside the 32-wide block
+        if (stage == 0) {                                 // layer 1:   B[j][e] = W0[j][e]
+            if (c < 4) v[i] = W0[r * 16 + k];
+        } else if (stage <= 8) {                          // layer 2:   B[j][k] = W1[j][k]
+            v[i] = W1[(size_t)r * WN + (stage - 1) * 32 + k];
+        } else if (stage <= 16) {                         // bwd layer 2: B[k][j] = w2[j] W1[j][k]
+            const int j = (stage - 9) * 32 + k;
+            v[i] = __fmul_rn(w2[j], W1[(size_t)j * WN + r]);
+        } else {                                          // bwd layer 1: B[e][k] = W0[k][e]
+            v[i] = W0[(size_t)((stage - 17) * 32 + k) * 16 + r];
+        }
     }
     float hi[4], lo[4];
-    for (int i = 0; i < 4; ++i) { hi[i] = tf32_rna(v[i]); lo[i] = tf32_rna(v[i] - hi[i]); }
+    for (int i = 0; i < 4; ++i) { hi[i] = __uint_as_float(tf32_rna(v[i])); lo[i] = __uint_as_float(tf32_rna(v[i] - hi[i])); }
     uint8_t *base = panels + (size_t)stage * STAGE_B;
     *reinterpret_cast<float4 *>(base + panel_off(r, c)) = make_float4(hi[0], hi[1], hi[2], hi[3]);
     *reinterpret_cast<float4 *>(base + PANEL_B + panel_off(r, c)) = make_float4(lo[0], lo[1], lo[2], lo[3]);
 }
 
-struct FwdParams {
+struct Params {
     long long M_host;
     const int32_t *M_dev;
-    const float *feats;       // [M,16]
-    const uint8_t *panels;    // 9 stages x 64 KB
-    const float *b0, *b1, *w2, *b2;
-    float *sdf;
-};
-
-__global__ void __launch_bounds__(NTHREADS, 1) k_mlp_tc_fwd(FwdParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B panels need 1024-byte alignment
-    uint8_t *sm = smem_raw + (base - raw);
-    const uint32_t sB = base, sA = base + NSTAGE * STAGE_B;
-    uint8_t *A_gen = sm + NSTAGE * STAGE_B;        // generic pointer to the activation stages
-    float *b0s = reinterpret_cast<float *>(sm + SMEM_DATA);
-    float *b1s = b0s + WN;
-    float *w2s = b1s + WN;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + SMEM_DATA + 3 * WN * 4);
-    // barriers: 0,1 b_full  2,3 b_empty  4,5 a_full  6,7 a_empty  8 d1_full  9 d2_full  10 d2_empty
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 12);
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const long long M = p.M_dev ? min((long long)*p.M_dev, p.M_host) : p.M_host;
-    const long long ntiles = (M + TM - 1) / TM;
-
-    for (int i = tid; i < WN; i += NTHREADS) { b0s[i] = p.b0[i]; b1s[i] = p.b1[i]; w2s[i] = p.w2[i]; }
-    if (tid == 0) {
-        mbar_init(BAR(0), 1); mbar_init(BAR(1), 1);      // b_full: producer's expect_tx arrive
-        mbar_init(BAR(2), 1); mbar_init(BAR(3), 1);      // b_empty: tcgen05.commit
-        mbar_init(BAR(4), 4); mbar_init(BAR(5), 4);      // a_full: one arrive per epilogue warp
-        mbar_init(BAR(6), 1); mbar_init(BAR(7), 1);      // a_empty: tcgen05.commit
-        mbar_init(BAR(8), 1); mbar_init(BAR(9), 1);      // d1_full, d2_full: tcgen05.commit
-        mbar_init(BAR(10), 4);                           // d2_empty: one arrive per epilogue warp
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {  // TMEM: all 512 columns (D1 at column 0, D2 at column 256)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t D1 = tmem, D2 = tmem + 256;
-
-    if (warp == 0) {
-        // ===================== producer: weight panels -> ring =====================
-        uint32_t it = 0;
-        for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-            for (int step = 0; step < STEPS_FWD; ++step, ++it) {
-                const uint32_t s = it & 1, ph = (it >> 1) & 1;
-                mbar_wait(BAR(2 + s), ph ^ 1);
-                if (elect_one()) {
-                    mbar_expect_tx(BAR(0 + s), STAGE_B);
-                    const uint8_t *src = p.panels + (size_t)step * STAGE_B;
-                    bulk_g2s(sB + s * STAGE_B, src, PANEL_B, BAR(0 + s));
-                    bulk_g2s(sB + s * STAGE_B + PANEL_B, src + PANEL_B, PANEL_B, BAR(0 + s));
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-        constexpr uint32_t idesc = make_idesc(TM, WN);
-        uint32_t it = 0, tl = 0;
-        for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tl) {
-            for (int step = 0; step < STEPS_FWD; ++step, ++it) {
-                const uint32_t s = it & 1, ph = (it >> 1) & 1;
-                if (step == 1) mbar_wait(BAR(10), (tl & 1) ^ 1);   // D2 of the previous tile fully read
-                mbar_wait(BAR(0 + s), ph);                          // weights landed
-                mbar_wait(BAR(4 + s), ph);                          // activations written
-                tc_fence_after();
-                const uint32_t a_hi = sA + s * STAGE_A, b_hi = sB + s * STAGE_B;
-                if (elect_one()) {
-                    if (step == 0) issue_kblock<2, 3>(D1, a_hi, b_hi, idesc, 0u);          // K = 16: 2 k-steps of 8
-                    else issue_kblock<4, 3>(D2, a_hi, b_hi, idesc, step == 1 ? 0u : 1u);   // first MMA of a layer overwrites
-                    tc_commit(BAR(2 + s));                              // ring stages free once these MMAs retire
-                    tc_commit(BAR(6 + s));
-                    if (step == 0) tc_commit(BAR(8));                   // D1 complete
-                    if (step == STEPS_FWD - 1) tc_commit(BAR(9));       // D2 complete
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        // ===================== epilogue warps: thread = sample row =====================
-        const int q = warp & 3;                       // TMEM lane quarter this warp may access
-        const int row = q * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        const float b2 = p.b2[0];
-        uint32_t it = 0, tl = 0;
-        for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tl) {
-            const long long m = tile * TM + row;
-            // ---- step 0: x (16 features = 4 chunks) -> A stage ----
-            {
-                const uint32_t s = it & 1, ph = (it >> 1) & 1;
-                mbar_wait(BAR(6 + s), ph ^ 1);
-                uint8_t *dst = A_gen + s * STAGE_A;
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (m < M) v = *reinterpret_cast<const float4 *>(p.feats + (size_t)m * 16 + c * 4);
-                    const float4 hi = make_float4(tf32_rna(v.x), tf32_rna(v.y), tf32_rna(v.z), tf32_rna(v.w));
-                    const float4 lo = make_float4(tf32_rna(v.x - hi.x), tf32_rna(v.y - hi.y), tf32_rna(v.z - hi.z), tf32_rna(v.w - hi.w));
-                    *reinterpret_cast<float4 *>(dst + panel_off(row, c)) = hi;
-                    *reinterpret_cast<float4 *>(dst + PANEL_A + panel_off(row, c)) = lo;
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(BAR(4 + s));
-                ++it;
-            }
-            // ---- steps 1..8: h1 K-block kb = relu(D1[:, 32kb:32kb+32] + b0) -> A stage ----
-            mbar_wait(BAR(8), tl & 1);
-            tc_fence_after();
-            for (int kb = 0; kb < 8; ++kb, ++it) {
-                const uint32_t s = it & 1, ph = (it >> 1) & 1;
-                uint32_t v[32];
-                tmem_ld32(D1 + lane_addr + kb * 32, v);
-                mbar_wait(BAR(6 + s), ph ^ 1);
-                uint8_t *dst = A_gen + s * STAGE_A;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    float h[4], hi[4], lo[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        h[i] = fmaxf(__uint_as_float(v[c * 4 + i]) + b0s[kb * 32 + c * 4 + i], 0.f);
-                        hi[i] = tf32_rna(h[i]);
-                        lo[i] = tf32_rna(h[i] - hi[i]);
-                    }
-                    *reinterpret_cast<float4 *>(dst + panel_off(row, c)) = make_float4(hi[0], hi[1], hi[2], hi[3]);
-                    *reinterpret_cast<float4 *>(dst + PANEL_A + panel_off(row, c)) = make_float4(lo[0], lo[1], lo[2], lo[3]);
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(BAR(4 + s));
-            }
-            // ---- output layer: sdf = relu(D2 + b1) . w2 + b2 ----
-            mbar_wait(BAR(9), tl & 1);
-            tc_fence_after();
-            float acc4[4] = {0.f, 0.f, 0.f, 0.f};
-            for (int cb = 0; cb < 8; ++cb) {
-                uint32_t v[32];
-                tmem_ld32(D2 + lane_addr + cb * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const float h = fmaxf(__uint_as_float(v[i]) + b1s[cb * 32 + i], 0.f);
-                    acc4[i & 3] = fmaf(h, w2s[cb * 32 + i], acc4[i & 3]);
-                }
-            }
-            const float acc = (acc4[0] + acc4[1]) + (acc4[2] + acc4[3]);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(BAR(10));
-            if (m < M) p.sdf[m] = acc + b2;
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-    }
-}
-
-
-// ================================================================================================
-// Training kernel: forward + loss + backward w.r.t. the input features in one pass per 128-sample tile.
-//   steps  0      layer 1            D1 = x . W0^T                      (TMEM cols 0..255)
-//          1..8   layer 2            D2 = relu(D1+b0) . W1^T            (TMEM cols 256..511)
-//                 epilogue: sdf = relu(D2+b1).w2 + b2, loss terms, d loss/d sdf (all thread-local: thread = sample)
-//          9..16  backward layer 2   D3 = relu'(h2) . (diag(w2) W1)     (reuses D1's columns)
-//          17..24 backward layer 1   D4 = (dsdf * D3 * relu'(h1)) . W0  (N = 16, reuses D2's first 16 columns) = d loss / d x
-// The output layer has ONE unit, so d h2 = dsdf (per sample) x w2 (per column) x relu'(h2) is rank-1 up to the mask:
-// the per-sample factor is pulled out of the GEMM (applied when D3 is read back), the per-column factor is folded into
-// the weight panels, and the A operand of backward layer 2 is the 0/1 mask itself -- exact in tf32, so that GEMM needs
-// two terms (mask x hi, mask x lo) instead of three and no lo panel.  ReLU masks are 2 x 256 bits per thread in registers.
-// With WGRAD the kernel writes h1 and dh1 to HBM in 16 KB "panel" blocks [(tile*8 + kblock)][row][32] (bulk copies of the
-// A stages) plus the relu'(h2) bits (32 B/sample) and dsdf; the same factorisation lets k_dw1_tc / k_dw0_tc / k_mask_colsum rebuild
-// everything that used to need dh2 and h2 panels (see there).
-// ================================================================================================
-struct TrainParams {
-    long long M_host;
-    const int32_t *M_dev;
-    const float *feats;
+    const float *feats;        // [M,16]
     const uint8_t *panels;     // 25 stages x 64 KB
     const float *b0, *b1, *w2, *b2;
     float *sdf, *dfeats;
@@ -384,985 +185,448 @@ struct TrainParams {
     nl_render_stats *stats;
     float truncation;
     const float *dsdf_ext;
-    float *act_h1, *act_dh1;             // WGRAD: panel-major [ntiles*8][128][32]
-    float *act_dsdf;                     // WGRAD: d loss / d sdf per sample [ntiles*128]
-    uint32_t *act_mask2;                 // WGRAD: relu'(h2) bits per sample [ntiles*128][8], word g*4+kk = columns 32(2kk+g)..+31
-    float *gb2;                          // WGRAD
-    long long *dbg;                      // optional timeline stamps (NL_TC_TIMELINE=1), else nullptr
+    float *act_h1, *act_h2, *act_dh2, *act_dh1, *act_d;   // WGRAD: [cap][256] x 4, [cap]
 };
 
-// registers -> TMEM, 32 lanes x 32 columns per warp (thread = lane/row); completion via tmem_wait_st()
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-        "%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]),
-        "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]),
-        "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// A operand from TMEM (lane = row, one 32-bit column per tf32 element, K = 8 columns per instruction), B from shared memory
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc),
-        "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ring item i of a tile -> panel stage and N half
+__device__ __forceinline__ void item_of(int i, int &stage, int &half) {
+    if (i < 2) { stage = 0; half = i; }
+    else if (i < 18) { half = (i - 2) >> 3; stage = 1 + ((i - 2) & 7); }
+    else if (i < 34) { half = (i - 18) >> 3; stage = 9 + ((i - 18) & 7); }
+    else { half = 0; stage = 17 + (i - 34); }
 }
 
-// smem -> global bulk copy (1-D TMA store) of this warp's rows of an activation panel; one instruction per warp and
-// chunk instead of 8 partially-coalesced STG.128 per thread
-__device__ __forceinline__ void bulk_s2g(void *gdst, uint32_t ssrc, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, float a, float b, float c, float d) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-// tf32 hi/lo split of an A-operand value computed in the epilogue.  The tensor core TRUNCATES its fp32 inputs to tf32.  "hi" is
-// therefore simply the raw fp32 bits (which also keeps the stored activation panels exact: the hi tile is what gets bulk-copied
-// to HBM for the weight-gradient kernels), and lo = x - trunc(x), exact in fp32.  What matters is how lo reaches 11 bits: left
-// to the hardware it is truncated too -- an error of up to 2^-21 |x| that always points towards zero, i.e. a BIAS shared by every
-// sample.  Gradients that are sums of 10^4..10^5 strongly cancelling per-sample terms (the pose gradient near convergence:
-// cancellation ~10^4) turned that into 10^-3 relative error, 100x what fp32 arithmetic gives (measured against an fp64 run of
-// the same function, tests/test_gpu_pipeline.py).  Rounding lo to nearest instead (integer add of half an ulp, then mask) makes
-// the hardware truncation of lo a no-op and the residual <= 2^-22 |x| with random sign.
-__device__ __forceinline__ float tf32_lo_part(float x) {
-    const float lo = x - __uint_as_float(__float_as_uint(x) & 0xffffe000u);
-    return __uint_as_float((__float_as_uint(lo) + 0x1000u) & 0xffffe000u);
-}
-// One 128 B row (32 fp32) of an A-operand K-block as hi and lo tiles.  off[c] = swizzled byte offset of chunk c for this thread's
-// row (loop invariant).
-__device__ __forceinline__ void store_a_row_fast(uint32_t stage, const uint32_t (&off)[8], const float (&h)[32]) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        st_shared_v4(stage + off[c], h[c * 4], h[c * 4 + 1], h[c * 4 + 2], h[c * 4 + 3]);
-        st_shared_v4(stage + PANEL_A + off[c], tf32_lo_part(h[c * 4]), tf32_lo_part(h[c * 4 + 1]), tf32_lo_part(h[c * 4 + 2]), tf32_lo_part(h[c * 4 + 3]));
-    }
-}
-
-// Warp roles (NTHREADS_TRAIN = 320): warps 0-7 epilogue (group g = warp >> 2, TMEM lane quarter q = warp & 3), warp 8
-// producer, warp 9 MMA issuer + TMEM owner.  The two single-thread roles get the HIGHEST warp ids: the per-SMSP arbiter
-// prefers the highest warp id, so the busy epilogue warps cannot starve the thread that feeds the tensor core.
-// TS = true: the A operands of both backward GEMMs come from TMEM instead of shared memory.  The 0/1 mask of backward
-// layer 2 is written (tcgen05.st) over the dead layer-2 accumulator right where each thread read its pre-activations, so
-// those 8 K-blocks need no activation stage, no smem stores and no per-chunk hand-shake; the dh1 chunks of backward
-// layer 1 go through two 64-column TMEM slots (hi | lo), one per epilogue group.  Shared-memory traffic of those 16
-// steps drops to the weight panels, and the tiny N = 16 MMAs no longer fetch a 4 KB A tile from smem each.
-// PAIR = true (launched as clusters of 2 CTAs): the two CTAs of a pair walk through the SAME sequence of weight stages, each
-// on its own tile, so every stage is fetched from L2 once per pair -- CTA 0 loads the hi panel, CTA 1 the lo panel, each copy
-// multicast into both shared memories -- instead of once per CTA.  Backward layer 2 is bound by exactly that stream (64 KB per
-// K-block and SM, ~57 B/clk/SM, the L2's limit chip-wide); halving it is what moves it towards its tensor floor.  A stage is
-// refilled only when BOTH CTAs' MMAs have retired it (their tcgen05.commit is multicast to both b_empty barriers, count 2), and
-// both CTAs run the same number of rounds (a missing last tile is processed with all rows dead).
-template <bool WGRAD, bool TS, bool PAIR>
-__global__ void __launch_bounds__(NTHREADS_TRAIN, 1) k_mlp_tc_train(TrainParams p) {
+template <bool TRAIN, bool WGRAD>
+__global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
+    constexpr int IPT = TRAIN ? ITEMS_TRAIN : ITEMS_FWD;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
+    const uint32_t base = (raw + 1023u) & ~1023u;    // SWIZZLE_128B panels need 1024-byte alignment
     uint8_t *sm = smem_raw + (base - raw);
-    const uint32_t sB = base, sA = base + NSTAGE * STAGE_B;
-    float *b0s = reinterpret_cast<float *>(sm + SMEM_DATA);
+    const uint32_t ring = base;
+    float *b0s = reinterpret_cast<float *>(sm + NSLOT * SLOT);
     float *b1s = b0s + WN;
     float *w2s = b1s + WN;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + SMEM_DATA + 3 * WN * 4);
-    // barriers: 0,1 b_full  2,3 b_empty  4,5 a_full  6,7 a_empty  8 d1_full  9 d2_full  10 d3_full  11 d4_full  12 d4_empty
-    //           TS: 14,15 slot_full[g]  16,17 slot_empty[g]  18..25 mask_full[K-block]
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 28);
-    float *sdf_part = reinterpret_cast<float *>(sm + SMEM_DATA + 4096);   // [tile parity][group][row]
+    const uint32_t bar0 = smem_u32(w2s + WN);       // FULL[s] at 8s, EMPTY[s] at 8 (NSLOT + s)
+    auto FULL = [&](uint32_t s) { return bar0 + 8u * s; };
+    auto EMPTY = [&](uint32_t s) { return bar0 + 8u * (NSLOT + s); };
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    long long *dbg = (blockIdx.x == 0) ? p.dbg : nullptr;   // [role 0..3][step 0..24][4 stamps]
-#define NL_STAMP(role, step, k) do { if (dbg && tl == 1 && (threadIdx.x & 31) == 0) dbg[((role) * 25 + (step)) * 8 + (k)] = clock64(); } while (0)
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
     const long long M = p.M_dev ? min((long long)*p.M_dev, p.M_host) : p.M_host;
     const long long ntiles = (M + TM - 1) / TM;
-    // tiles this CTA loops over: with PAIR every CTA runs the same number of rounds (tiles >= ntiles have only dead rows)
-    const long long nt_loop = PAIR ? ((ntiles + gridDim.x - 1) / gridDim.x) * gridDim.x : ntiles;
-    const uint32_t pair_rank = PAIR ? cluster_cta_rank() : 0u;
+    const long long my_tiles = (long long)blockIdx.x < ntiles ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+    const uint32_t total = (uint32_t)(my_tiles * IPT);
 
-    for (int i = tid; i < WN; i += NTHREADS_TRAIN) { b0s[i] = p.b0[i]; b1s[i] = p.b1[i]; w2s[i] = p.w2[i]; }
+    for (int i = tid; i < WN; i += NTHREADS) { b0s[i] = p.b0[i]; b1s[i] = p.b1[i]; w2s[i] = p.w2[i]; }
     if (tid == 0) {
-        mbar_init(BAR(0), 1); mbar_init(BAR(1), 1);
-        mbar_init(BAR(2), PAIR ? 2 : 1); mbar_init(BAR(3), PAIR ? 2 : 1);   // b_empty: the MMAs of both CTAs of a pair
-        mbar_init(BAR(4), 4); mbar_init(BAR(5), 4);      // a_full: the 4 warps of the group that owns the chunk
-        mbar_init(BAR(6), 1); mbar_init(BAR(7), 1);
-        mbar_init(BAR(8), 1); mbar_init(BAR(9), 1); mbar_init(BAR(10), 1); mbar_init(BAR(11), 1);
-        mbar_init(BAR(12), 4);
-        for (int i = 0; i < 8; ++i) mbar_init(BAR(18 + i), 4);   // mask_full[K-block]: the 4 warps of the group that owns it
-        mbar_init(BAR(14), 4); mbar_init(BAR(15), 4);    // slot_full: the 4 warps of the group
-        mbar_init(BAR(16), 1); mbar_init(BAR(17), 1);    // slot_empty: tcgen05.commit
+        for (int s = 0; s < NSLOT; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 9) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    if (PAIR) cluster_sync_all();                // the partner's barriers exist before any multicast copy / commit can reach them
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t D1 = tmem, D2 = tmem + 256;   // D3 aliases D1, D4 aliases D2[0:16]
-    // TS: mask2 overwrites D2 (all 256 columns) for steps 9..16; dh1 slot g = D2[64 + 64g, +64) (hi | lo) for steps 17..24
-    auto SLOT = [&](int g) { return D2 + 64u + 64u * (uint32_t)g; };
-    // activation-stage use index: without TS every step uses a stage, with TS only steps 0..8 of each tile do
-    auto AIT = [&](uint32_t tl, int step) { return TS ? tl * 9u + (uint32_t)step : tl * (uint32_t)STEPS_TRAIN + (uint32_t)step; };
 
-    if (warp == 8) {
-        // ===== producer (warp-uniform loop, one elected lane issues the copies) =====
-        uint32_t it = 0, tl = 0;
-        for (long long tile = blockIdx.x; tile < nt_loop; tile += gridDim.x, ++tl) {
-            for (int step = 0; step < STEPS_TRAIN; ++step, ++it) {
-                const uint32_t s = it & 1, ph = (it >> 1) & 1;
-                const uint32_t bytes = (step < 17) ? PANEL_B : PANEL_B16;
-                NL_STAMP(0, step, 0);
-                mbar_wait(BAR(2 + s), ph ^ 1);
-                NL_STAMP(0, step, 1);
-                if (elect_one()) {
-                    mbar_expect_tx(BAR(0 + s), 2 * bytes);            // hi + lo land in this CTA whoever fetches them
-                    const uint8_t *src = p.panels + (size_t)step * STAGE_B;
-                    if (PAIR) {                                       // this CTA fetches one of the two panels for both CTAs
-                        bulk_g2s_pair(sB + s * STAGE_B + pair_rank * PANEL_B, src + pair_rank * PANEL_B, bytes, BAR(0 + s));
-                    } else {
-                        bulk_g2s(sB + s * STAGE_B, src, bytes, BAR(0 + s));
-                        bulk_g2s(sB + s * STAGE_B + PANEL_B, src + PANEL_B, bytes, BAR(0 + s));
-                    }
-                }
-                __syncwarp();
+    // thread 0 feeds the ring: item n is always issued before anyone waits for it; items up to n + NSLOT - 1 are issued
+    // when their slot is already free (non-blocking test), so the copies run ahead of the MMAs
+    uint32_t issued = 0;
+    auto issue = [&](uint32_t n) {
+        const uint32_t s = n % NSLOT;
+        mbar_wait(EMPTY(s), ((n / NSLOT) & 1) ^ 1);
+        int stage, half;
+        item_of((int)(n % IPT), stage, half);
+        const uint32_t bytes = stage >= 17 ? 16 * 128 : HALF;
+        mbar_expect_tx(FULL(s), 2 * bytes);
+        const uint8_t *src = p.panels + (size_t)stage * STAGE_B + half * HALF;
+        bulk_g2s(ring + s * SLOT, src, bytes, FULL(s));
+        bulk_g2s(ring + s * SLOT + HALF, src + PANEL_B, bytes, FULL(s));
+    };
+    uint32_t n = 0;   // ring items consumed by this thread
+    // wait for item n; returns the descriptors of its hi and lo halves.  The caller computes its A fragments first and then
+    // issues wgmma.fence (registers written after the fence may not feed the wgmmas behind it)
+    auto acquire = [&](uint64_t &bh, uint64_t &bl) {
+        if (tid == 0) {
+            while (issued < total && issued < n + NSLOT) {
+                if (issued > n && !mbar_test(EMPTY(issued % NSLOT), ((issued / NSLOT) & 1) ^ 1)) break;
+                issue(issued++);
             }
         }
-    } else if (warp == 9) {
-        // ===== MMA issuer (warp-uniform loop, one elected lane issues) =====
-        constexpr uint32_t idesc256 = make_idesc(TM, WN), idesc16 = make_idesc(TM, 16);
-        uint32_t it = 0, tl = 0;
-        for (long long tile = blockIdx.x; tile < nt_loop; tile += gridDim.x, ++tl) {
-            for (int step = 0; step < STEPS_TRAIN; ++step, ++it) {
-                const uint32_t s = it & 1, ph = (it >> 1) & 1;
-                NL_STAMP(1, step, 0);
-                if (step == 1) mbar_wait(BAR(12), (tl & 1) ^ 1);   // D4 (in D2's columns) of the previous tile fully read
-                mbar_wait(BAR(0 + s), ph);
-                NL_STAMP(1, step, 1);
-                const uint32_t b_hi = sB + s * STAGE_B;
-                if (!TS || step <= 8) {
-                    const uint32_t ai = AIT(tl, step), as = ai & 1, aph = (ai >> 1) & 1;
-                    mbar_wait(BAR(4 + as), aph);
-                    NL_STAMP(1, step, 2);
-                    tc_fence_after();
-                    const uint32_t a_hi = sA + as * STAGE_A;
-                    if (elect_one()) {
-                        if (step == 0) issue_kblock<2, 3>(D1, a_hi, b_hi, idesc256, 0u);                      // layer 1 (K = 16)
-                        else if (step <= 8) issue_kblock<4, 3>(D2, a_hi, b_hi, idesc256, step == 1 ? 0u : 1u);    // layer 2
-                        else if (step <= 16) issue_kblock<4, 2>(D1, a_hi, b_hi, idesc256, step == 9 ? 0u : 1u);   // backward layer 2: the 0/1
-                                                                                                                  // mask operand has no lo part
-                        else issue_kblock<4, 3>(D2, a_hi, b_hi, idesc16, step == 17 ? 0u : 1u);                   // backward layer 1 (N = 16)
-                        if (PAIR) tc_commit_pair(BAR(2 + s)); else tc_commit(BAR(2 + s));
-                        tc_commit(BAR(6 + as));
-                        if (step == 0) tc_commit(BAR(8));
-                        if (step == 8) tc_commit(BAR(9));
-                        if (step == 16) tc_commit(BAR(10));
-                        if (step == 24) tc_commit(BAR(11));
-                    }
-                } else if (step <= 16) {
-                    // ---- TS backward layer 2: A = mask2 columns of K-block jb in TMEM ----
-                    mbar_wait(BAR(18 + (step - 9)), tl & 1);
-                    NL_STAMP(1, step, 2);
-                    tc_fence_after();
-                    const uint32_t a_t = D2 + (uint32_t)(step - 9) * 32u;
-                    if (elect_one()) {
-                        const uint64_t bdh = make_desc(b_hi), bdl = make_desc(b_hi + PANEL_B);
-                        uint32_t acc = step == 9 ? 0u : 1u;
+        __syncwarp();
+        const uint32_t s = n % NSLOT;
+        mbar_wait(FULL(s), (n / NSLOT) & 1);
+        bh = make_desc(ring + s * SLOT);
+        bl = make_desc(ring + s * SLOT + HALF);
+    };
+    auto release = [&]() {
+        wg_commit_wait();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(EMPTY(n % NSLOT));
+        ++n;
+    };
+
+    const float b2 = p.b2[0];
+    float g_fs = 0.f, g_sdf = 0.f;
+    if (TRAIN && !p.dsdf_ext) { g_fs = p.stats->g_fs; g_sdf = p.stats->g_sdf; }
+    double loss_fs = 0.0, loss_sdf = 0.0;
+
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long m0 = tile * TM + warp * 16 + g, m1 = m0 + 8;   // this thread's two rows
+        const bool live0 = m0 < M, live1 = m1 < M;
+
+        // ---- layer 1: D1 = x . W0^T (K = 16: two k-steps; A fragment of k-step ks = columns 8ks+2t, 8ks+2t+1) ----
+        float h[128];
+        {
+            float xa[8];
 #pragma unroll
-                        for (int term = 0; term < 2; ++term) {
+            for (int ks = 0; ks < 2; ++ks) {
+                const float2 r0 = live0 ? *reinterpret_cast<const float2 *>(p.feats + (size_t)m0 * 16 + 8 * ks + 2 * t) : make_float2(0.f, 0.f);
+                const float2 r1 = live1 ? *reinterpret_cast<const float2 *>(p.feats + (size_t)m1 * 16 + 8 * ks + 2 * t) : make_float2(0.f, 0.f);
+                xa[4 * ks] = r0.x; xa[4 * ks + 1] = r0.y; xa[4 * ks + 2] = r1.x; xa[4 * ks + 3] = r1.y;
+            }
+            float xh[128];   // only the first 8 entries are used: frag3 reads a k-step's fragment from a 128-entry array
 #pragma unroll
-                            for (int ks = 0; ks < 4; ++ks) {
-                                mma_tf32_ts(D1, a_t + 8 * ks, (term ? bdl : bdh) + 2 * ks, idesc256, acc);
-                                acc = 1u;
-                            }
-                        }
-                        if (PAIR) tc_commit_pair(BAR(2 + s)); else tc_commit(BAR(2 + s));
-                        if (step == 16) tc_commit(BAR(10));
-                    }
-                } else {
-                    // ---- TS backward layer 1: A = dh1 chunk (hi | lo) in the TMEM slot of the group that owns K-block kb ----
-                    const int kb = step - 17, g = kb & 1;
-                    const uint32_t u = tl * 4u + (uint32_t)(kb >> 1);
-                    mbar_wait(BAR(14 + g), u & 1);
-                    NL_STAMP(1, step, 2);
-                    tc_fence_after();
-                    const uint32_t a_t = SLOT(g);
-                    if (elect_one()) {
-                        const uint64_t bdh = make_desc(b_hi), bdl = make_desc(b_hi + PANEL_B);
-                        uint32_t acc = step == 17 ? 0u : 1u;
+            for (int i = 0; i < 8; ++i) xh[i] = xa[i];
 #pragma unroll
-                        for (int term = 0; term < 3; ++term) {
+            for (int i = 0; i < 128; ++i) h[i] = 0.f;
+            uint32_t ah[2][4], al[2][4];
 #pragma unroll
-                            for (int ks = 0; ks < 4; ++ks) {
-                                mma_tf32_ts(D2, a_t + (term == 2 ? 32u : 0u) + 8 * ks, (term == 1 ? bdl : bdh) + 2 * ks, idesc16, acc);
-                                acc = 1u;
-                            }
-                        }
-                        if (PAIR) tc_commit_pair(BAR(2 + s)); else tc_commit(BAR(2 + s));
-                        tc_commit(BAR(16 + g));
-                        if (step == 24) tc_commit(BAR(11));
-                    }
-                }
-                __syncwarp();
-                NL_STAMP(1, step, 3);
+            for (int ks = 0; ks < 2; ++ks) frag3(xh, ks, ah[ks], al[ks]);
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                uint64_t bh, bl;
+                acquire(bh, bl);
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < 2; ++ks) mma3<64>(sub64(h, 64 * half), ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
+                release();
             }
         }
-    } else {
-        // ===== epilogue: 2 groups x 4 warps; thread = (sample row, group); group g owns the K-blocks with (kb & 1) == g =====
-        const int q = warp & 3;                        // TMEM lane quarter this warp may access
-        const int g = warp >> 2;                       // 0: warps 0-3, 1: warps 4-7
-        const int row = q * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        uint32_t offc[8];
+        // h1 = relu(D1 + b0), relu'(h1) bits: bit (4j + x) of the 128-bit mask
+        uint32_t mask1[4] = {0u, 0u, 0u, 0u}, mask2[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-        for (int c = 0; c < 8; ++c) offc[c] = (uint32_t)panel_off(row, c);
-        const float b2 = p.b2[0];
-        float g_fs = 0.f, g_sdf = 0.f;
-        if (!p.dsdf_ext) { g_fs = p.stats->g_fs; g_sdf = p.stats->g_sdf; }
-        double loss_fs = 0.0, loss_sdf = 0.0;
-        float gb2r = 0.f;
-        // per-sample inputs of the next tile are fetched one tile ahead (their latency hides behind a whole tile)
-        float4 xn[4];
-        uint32_t fl_n = 0u;
-        float z_n = 0.f, dgt_n = 0.f, dext_n = 0.f;
-        auto prefetch = [&](long long tile) {
-            const long long mm = tile * TM + row;
-            const bool lv = tile < ntiles && mm < M;
+        for (int j = 0; j < 32; ++j)
 #pragma unroll
-            for (int c = 0; c < 4; ++c) xn[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-            fl_n = 0u; z_n = 0.f; dgt_n = 0.f; dext_n = 0.f;
-            if (lv) {
-                if (g == 0) {
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) xn[c] = *reinterpret_cast<const float4 *>(p.feats + (size_t)mm * 16 + c * 4);
-                }
-                if (p.dsdf_ext) {
-                    dext_n = p.dsdf_ext[mm];
-                } else {
-                    fl_n = p.s_flag[mm];
-                    const int r = p.s_ray[mm];
-                    z_n = __fmul_rn(p.s_depth[mm], p.cosv ? p.cosv[r] : 1.0f);
-                    dgt_n = p.gt_depth[r];
-                }
+            for (int x = 0; x < 4; ++x) {
+                const float v = h[4 * j + x] + b0s[8 * j + 2 * t + (x & 1)];
+                const bool on = v > 0.f;
+                h[4 * j + x] = on ? v : 0.f;
+                if (on) mask1[j >> 3] |= 1u << ((j & 7) * 4 + x);
             }
-        };
-        prefetch(blockIdx.x);
-        uint32_t tl = 0;
-        for (long long tile = blockIdx.x; tile < nt_loop; tile += gridDim.x, ++tl) {
-            const long long m = tile * TM + row;
-            const bool live = m < M;
-            const uint32_t fl = fl_n;
-            const float z = z_n, dgt = dgt_n, dext = dext_n;
-            uint32_t mask1[4], mask2[4];
-            // ---- step 0: x -> A (group 0).  With TS the activation stages are idle during the backward steps, so the next
-            // tile's x was already staged at the end of the previous tile (stage_x below) ----
-            if (g == 0 && (!TS || tl == 0)) {
-                const uint32_t it = AIT(tl, 0), s = it & 1, ph = (it >> 1) & 1;
-                if (WGRAD) { if (lane == 0) bulk_wait_read(); __syncwarp(); }
-                mbar_wait(BAR(6 + s), ph ^ 1);
-                const uint32_t dst = sA + s * STAGE_A;
+        if (WGRAD) {
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const float4 v = xn[c];
-                    const float4 hi = make_float4(tf32_rna(v.x), tf32_rna(v.y), tf32_rna(v.z), tf32_rna(v.w));
-                    st_shared_v4(dst + offc[c], hi.x, hi.y, hi.z, hi.w);
-                    st_shared_v4(dst + PANEL_A + offc[c], tf32_rna(v.x - hi.x), tf32_rna(v.y - hi.y), tf32_rna(v.z - hi.z), tf32_rna(v.w - hi.w));
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(BAR(4 + s));
+            for (int j = 0; j < 32; ++j) {
+                if (live0) *reinterpret_cast<float2 *>(p.act_h1 + (size_t)m0 * WN + 8 * j + 2 * t) = make_float2(h[4 * j], h[4 * j + 1]);
+                if (live1) *reinterpret_cast<float2 *>(p.act_h1 + (size_t)m1 * WN + 8 * j + 2 * t) = make_float2(h[4 * j + 2], h[4 * j + 3]);
             }
-            // ---- steps 1..8: h1 chunks ----
-            mbar_wait(BAR(8), tl & 1);
-            tc_fence_after();
-#pragma unroll 1
-            for (int kk = 0; kk < 4; ++kk) {
-                const int kb = 2 * kk + g;
-                const uint32_t it = AIT(tl, 1 + kb), s = it & 1, ph = (it >> 1) & 1;
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 0);
-                uint32_t v[32];
-                tmem_ld32(D1 + lane_addr + kb * 32, v);
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 4);
-                float h[32];
-                uint32_t mk = 0u;
+        }
+
+        // ---- layer 2 (two N halves) + output layer partial sums ----
+        float ps0 = 0.f, ps1 = 0.f;
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const float t = __uint_as_float(v[i]) + b0s[kb * 32 + i];
-                    const bool on = t > 0.f;
-                    h[i] = on ? t : 0.f;
-                    mk |= on ? (1u << i) : 0u;
-                }
-                mask1[kk] = mk;
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 5);
-                if (WGRAD) { if (lane == 0) bulk_wait_read(); __syncwarp(); }   // previous panel store of this warp left the stage
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 1);
-                mbar_wait(BAR(6 + s), ph ^ 1);
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 2);
-                store_a_row_fast(sA + s * STAGE_A, offc, h);
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 6);
-                fence_proxy_async();
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 7);
-                __syncwarp();
-                if (WGRAD && lane == 0 && tile < ntiles) bulk_s2g(p.act_h1 + ((size_t)(tile * 8 + kb) * TM + q * 32) * 32, sA + s * STAGE_A + q * 4096, 4096);
-                if (lane == 0) mbar_arrive(BAR(4 + s));
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 1 + kb, 3);
+        for (int half = 0; half < 2; ++half) {
+            float d[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) d[i] = 0.f;
+#pragma unroll
+            for (int kb = 0; kb < 8; ++kb) {
+                uint32_t ah[4][4], al[4][4];
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) frag3(h, 4 * kb + ks, ah[ks], al[ks]);
+                uint64_t bh, bl;
+                acquire(bh, bl);
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) mma3<64>(d, ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
+                release();
             }
-            // ---- output layer + loss: each group reduces its 4 column blocks, partial sums exchanged through smem ----
-            if (q == 0 && lane == 0) NL_STAMP(2 + g, 0, 0);
-            mbar_wait(BAR(9), tl & 1);
-            tc_fence_after();
-            if (q == 0 && lane == 0) NL_STAMP(2 + g, 0, 1);
-            float acc4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-            for (int kk = 0; kk < 4; ++kk) {
-                const int cb = 2 * kk + g;
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 0, 2 + kk);
-                uint32_t v[32];
-                tmem_ld32(D2 + lane_addr + cb * 32, v);
-                uint32_t mk = 0u;
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const float t = __uint_as_float(v[i]) + b1s[cb * 32 + i];
-                    const bool on = t > 0.f;
-                    mk |= on ? (1u << i) : 0u;
-                    acc4[i & 3] = fmaf(on ? t : 0.f, w2s[cb * 32 + i], acc4[i & 3]);
-                    if (TS) v[i] = on ? 0x3f800000u : 0u;       // 1.0f / 0.0f: the A operand of backward layer 2
+            for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+                for (int x = 0; x < 4; ++x) {
+                    const int col = 128 * half + 8 * jj + 2 * t + (x & 1), j = 16 * half + jj;
+                    const float v = d[4 * jj + x] + b1s[col];
+                    const bool on = v > 0.f;
+                    const float hv = on ? v : 0.f;
+                    d[4 * jj + x] = hv;
+                    if (on) mask2[j >> 3] |= 1u << ((j & 7) * 4 + x);
+                    if (x < 2) ps0 = fmaf(hv, w2s[col], ps0); else ps1 = fmaf(hv, w2s[col], ps1);
                 }
-                mask2[kk] = mk;
-                if (TS) {   // same lanes / columns this thread just read; backward layer 2 may start on this K-block right away
-                    tmem_st32(D2 + lane_addr + cb * 32, v);
-                    tmem_wait_st();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(BAR(18 + cb));
-                }
-            }
-            float *part = sdf_part + (tl & 1) * 256;
-            part[g * 128 + row] = (acc4[0] + acc4[1]) + (acc4[2] + acc4[3]);
-            if (q == 0 && lane == 0) NL_STAMP(2 + g, 0, 6);
-            asm volatile("bar.sync 1, 256;" ::: "memory");          // the 8 epilogue warps
-            if (q == 0 && lane == 0) NL_STAMP(2 + g, 0, 7);
-            const float sdf = (part[row] + part[128 + row]) + b2;
-            float dsdf = 0.f;
-            if (live) {
-                if (g == 0) p.sdf[m] = sdf;
-                if (p.dsdf_ext) {
-                    dsdf = dext;
-                } else {
-                    if (fl & 1u) {
-                        const float e = sdf - 1.0f;
-                        if (g == 0) loss_fs += (double)e * (double)e;
-                        dsdf += 2.0f * g_fs * e;
-                    }
-                    if (fl & 2u) {
-                        const float e = __fsub_rn(__fadd_rn(z, __fmul_rn(sdf, p.truncation)), dgt);
-                        if (g == 0) loss_sdf += (double)e * (double)e;
-                        dsdf += 2.0f * g_sdf * p.truncation * e;
-                    }
-                }
-            }
-            if (WGRAD && tile < ntiles) {            // (PAIR: a padding tile beyond the data has no panel rows)
-                if (g == 0) {
-                    gb2r += dsdf;
-                    p.act_dsdf[tile * TM + row] = dsdf;
-                }
-                *reinterpret_cast<uint4 *>(p.act_mask2 + (size_t)(tile * TM + row) * 8 + g * 4) = make_uint4(mask2[0], mask2[1], mask2[2], mask2[3]);
-            }
-            // ---- steps 9..16: the 0/1 mask chunks as activation stages (TS: already in TMEM) ----
-#pragma unroll 1
-            for (int kk = 0; kk < (TS ? 0 : 4); ++kk) {
-                const int jb = 2 * kk + g;
-                const uint32_t it = AIT(tl, 9 + jb), s = it & 1, ph = (it >> 1) & 1;
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 9 + jb, 0);
-                if (WGRAD) { if (lane == 0) bulk_wait_read(); __syncwarp(); }
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 9 + jb, 1);
-                mbar_wait(BAR(6 + s), ph ^ 1);
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 9 + jb, 2);
-                {   // A = relu'(h2) as exact 0/1 tf32 values; dsdf and w2 are folded into the epilogue / the weight panels
-                    const uint32_t mk = mask2[kk], dst = sA + s * STAGE_A;
+            if (WGRAD) {
 #pragma unroll
-                    for (int c = 0; c < 8; ++c)
-                        st_shared_v4(dst + offc[c], (mk >> (4 * c)) & 1u ? 1.f : 0.f, (mk >> (4 * c + 1)) & 1u ? 1.f : 0.f,
-                                     (mk >> (4 * c + 2)) & 1u ? 1.f : 0.f, (mk >> (4 * c + 3)) & 1u ? 1.f : 0.f);
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(BAR(4 + s));
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 9 + jb, 3);
-            }
-            prefetch(tile + gridDim.x);                 // next tile's x / loss inputs: a whole backward pass to arrive
-            // ---- steps 17..24: dh1 (masked) chunks from D3 ----
-            mbar_wait(BAR(10), tl & 1);
-            tc_fence_after();
-#pragma unroll 1
-            for (int kk = 0; kk < 4; ++kk) {
-                const int kb = 2 * kk + g;
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 17 + kb, 0);
-                uint32_t v[32];
-                tmem_ld32(D1 + lane_addr + kb * 32, v);
-                float h[32];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) h[i] = ((mask1[kk] >> i) & 1u) ? dsdf * __uint_as_float(v[i]) : 0.f;
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 17 + kb, 1);
-                if (TS) {
-                    // hi = the fp32 bits (the tensor core truncates to tf32), lo = x - trunc(x) rounded to tf32 (tf32_lo_part); both into this group's TMEM slot
-                    const uint32_t u = tl * 4u + (uint32_t)kk;
-                    mbar_wait(BAR(16 + g), (u & 1) ^ 1);               // the MMAs of this group's previous chunk retired
-                    if (q == 0 && lane == 0) NL_STAMP(2 + g, 17 + kb, 2);
-                    uint32_t w[32];
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) w[i] = __float_as_uint(h[i]);
-                    tmem_st32(SLOT(g) + lane_addr, w);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) w[i] = __float_as_uint(tf32_lo_part(h[i]));
-                    tmem_st32(SLOT(g) + lane_addr + 32, w);
-                    tmem_wait_st();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(BAR(14 + g));
-                    if (WGRAD) {   // panel store for gW0 / gb0: staged through the activation stage this group used in steps 1..8
-                        const uint32_t sg = sA + ((tl + 1u + (uint32_t)g) & 1u) * STAGE_A;
-                        if (lane == 0) bulk_wait_read();
-                        __syncwarp();
-#pragma unroll
-                        for (int c = 0; c < 8; ++c) st_shared_v4(sg + offc[c], h[c * 4], h[c * 4 + 1], h[c * 4 + 2], h[c * 4 + 3]);
-                        fence_proxy_async();
-                        __syncwarp();
-                        if (lane == 0 && tile < ntiles) bulk_s2g(p.act_dh1 + ((size_t)(tile * 8 + kb) * TM + q * 32) * 32, sg + q * 4096, 4096);
-                    }
-                } else {
-                    const uint32_t it = AIT(tl, 17 + kb), s = it & 1, ph = (it >> 1) & 1;
-                    if (WGRAD) { if (lane == 0) bulk_wait_read(); __syncwarp(); }
-                    mbar_wait(BAR(6 + s), ph ^ 1);
-                    if (q == 0 && lane == 0) NL_STAMP(2 + g, 17 + kb, 2);
-                    store_a_row_fast(sA + s * STAGE_A, offc, h);
-                    fence_proxy_async();
-                    __syncwarp();
-                    if (WGRAD && lane == 0 && tile < ntiles) bulk_s2g(p.act_dh1 + ((size_t)(tile * 8 + kb) * TM + q * 32) * 32, sA + s * STAGE_A + q * 4096, 4096);
-                    if (lane == 0) mbar_arrive(BAR(4 + s));
-                }
-                if (q == 0 && lane == 0) NL_STAMP(2 + g, 17 + kb, 3);
-            }
-            if (WGRAD) {   // stages change hands between the groups at the tile boundary: all panel stores must have left smem
-                if (lane == 0) bulk_wait_read();
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-            }
-            if (TS && g == 0 && tile + gridDim.x < nt_loop) {
-                // x of the next tile (prefetched above) -> its activation stage now: the MMA warp can issue the next layer 1
-                // right behind this tile's last backward MMAs instead of waiting for the d x read-back below
-                const uint32_t it = AIT(tl + 1, 0), s = it & 1, ph = (it >> 1) & 1;
-                if (WGRAD) { if (lane == 0) bulk_wait_read(); __syncwarp(); }
-                mbar_wait(BAR(6 + s), ph ^ 1);
-                const uint32_t dst = sA + s * STAGE_A;
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const float4 v = xn[c];
-                    const float4 hi = make_float4(tf32_rna(v.x), tf32_rna(v.y), tf32_rna(v.z), tf32_rna(v.w));
-                    st_shared_v4(dst + offc[c], hi.x, hi.y, hi.z, hi.w);
-                    st_shared_v4(dst + PANEL_A + offc[c], tf32_rna(v.x - hi.x), tf32_rna(v.y - hi.y), tf32_rna(v.z - hi.z), tf32_rna(v.w - hi.w));
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(BAR(4 + s));
-            }
-            // ---- d loss / d x (group 0) ----
-            if (g == 0) {
-                mbar_wait(BAR(11), tl & 1);
-                tc_fence_after();
-                uint32_t v[16];
-                tmem_ld16(D2 + lane_addr, v);
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(BAR(12));
-                if (live) {
-                    float4 *o = reinterpret_cast<float4 *>(p.dfeats + (size_t)m * 16);
-#pragma unroll
-                    for (int c = 0; c < 4; ++c)
-                        o[c] = make_float4(__uint_as_float(v[c * 4]), __uint_as_float(v[c * 4 + 1]), __uint_as_float(v[c * 4 + 2]),
-                                           __uint_as_float(v[c * 4 + 3]));
+                for (int jj = 0; jj < 16; ++jj) {
+                    const int col = 128 * half + 8 * jj + 2 * t;
+                    if (live0) *reinterpret_cast<float2 *>(p.act_h2 + (size_t)m0 * WN + col) = make_float2(d[4 * jj], d[4 * jj + 1]);
+                    if (live1) *reinterpret_cast<float2 *>(p.act_h2 + (size_t)m1 * WN + col) = make_float2(d[4 * jj + 2], d[4 * jj + 3]);
                 }
             }
         }
-        if (!p.dsdf_ext && g == 0) {
-            for (int off = 16; off > 0; off >>= 1) {
-                loss_fs += __shfl_down_sync(0xffffffffu, loss_fs, off);
-                loss_sdf += __shfl_down_sync(0xffffffffu, loss_sdf, off);
+        // the 4 threads of a quad hold the 4 column classes of the same two rows
+        ps0 += __shfl_xor_sync(0xffffffffu, ps0, 1); ps0 += __shfl_xor_sync(0xffffffffu, ps0, 2);
+        ps1 += __shfl_xor_sync(0xffffffffu, ps1, 1); ps1 += __shfl_xor_sync(0xffffffffu, ps1, 2);
+        const float sdf0 = ps0 + b2, sdf1 = ps1 + b2;
+        if (t == 0) {
+            if (live0) p.sdf[m0] = sdf0;
+            if (live1) p.sdf[m1] = sdf1;
+        }
+        if constexpr (TRAIN) {
+            // ---- loss (criterion.py:92-103) and d loss / d sdf for both rows ----
+            float dsdf[2] = {0.f, 0.f};
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const long long m = r ? m1 : m0;
+                const float s = r ? sdf1 : sdf0;
+                if (!(r ? live1 : live0)) continue;
+                if (p.dsdf_ext) { dsdf[r] = p.dsdf_ext[m]; continue; }
+                const uint32_t fl = p.s_flag[m];
+                const int ray = p.s_ray[m];
+                const float z = __fmul_rn(p.s_depth[m], p.cosv ? p.cosv[ray] : 1.0f);
+                const float dgt = p.gt_depth[ray];
+                if (fl & 1u) {
+                    const float e = s - 1.0f;
+                    if (t == 0) loss_fs += (double)e * (double)e;
+                    dsdf[r] += 2.0f * g_fs * e;
+                }
+                if (fl & 2u) {
+                    const float e = __fsub_rn(__fadd_rn(z, __fmul_rn(s, p.truncation)), dgt);
+                    if (t == 0) loss_sdf += (double)e * (double)e;
+                    dsdf[r] += 2.0f * g_sdf * p.truncation * e;
+                }
             }
-            if (lane == 0) {
-                if (loss_fs != 0.0) atomicAdd(&p.stats->fs_sum, loss_fs);
-                if (loss_sdf != 0.0) atomicAdd(&p.stats->sdf_sum, loss_sdf);
+            if (WGRAD) {
+                if (t == 0) {
+                    if (live0) p.act_d[m0] = dsdf[0];
+                    if (live1) p.act_d[m1] = dsdf[1];
+                }
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    const int col = 8 * j + 2 * t;
+                    float v[4];
+#pragma unroll
+                    for (int x = 0; x < 4; ++x)
+                        v[x] = ((mask2[j >> 3] >> ((j & 7) * 4 + x)) & 1u) ? dsdf[x >> 1] * w2s[col + (x & 1)] : 0.f;
+                    if (live0) *reinterpret_cast<float2 *>(p.act_dh2 + (size_t)m0 * WN + col) = make_float2(v[0], v[1]);
+                    if (live1) *reinterpret_cast<float2 *>(p.act_dh2 + (size_t)m1 * WN + col) = make_float2(v[2], v[3]);
+                }
+            }
+            // ---- backward layer 2: D3 = relu'(h2) . (diag(w2) W1).  The A operand is the 0/1 mask (exact in tf32: 2 terms) ----
+#pragma unroll
+            for (int i = 0; i < 128; ++i) h[i] = 0.f;
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+#pragma unroll
+                for (int kb = 0; kb < 8; ++kb) {
+                    uint32_t a[4][4];
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks) {
+                        const int j = 4 * kb + ks;
+                        const uint32_t w = mask2[j >> 3] >> ((j & 7) * 4);
+                        a[ks][0] = (w & 1u) ? 0x3f800000u : 0u; a[ks][1] = (w & 4u) ? 0x3f800000u : 0u;
+                        a[ks][2] = (w & 2u) ? 0x3f800000u : 0u; a[ks][3] = (w & 8u) ? 0x3f800000u : 0u;
+                    }
+                    uint64_t bh, bl;
+                    acquire(bh, bl);
+                    wg_fence();
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks) {
+                        wgmma_n128(sub64(h, 64 * half), a[ks][0], a[ks][1], a[ks][2], a[ks][3], bh + 2 * ks);
+                        wgmma_n128(sub64(h, 64 * half), a[ks][0], a[ks][1], a[ks][2], a[ks][3], bl + 2 * ks);
+                    }
+                    release();
+                }
+            }
+            // dh1 = dsdf * D3 * relu'(h1)
+#pragma unroll
+            for (int j = 0; j < 32; ++j)
+#pragma unroll
+                for (int x = 0; x < 4; ++x)
+                    h[4 * j + x] = ((mask1[j >> 3] >> ((j & 7) * 4 + x)) & 1u) ? dsdf[x >> 1] * h[4 * j + x] : 0.f;
+            if (WGRAD) {
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    if (live0) *reinterpret_cast<float2 *>(p.act_dh1 + (size_t)m0 * WN + 8 * j + 2 * t) = make_float2(h[4 * j], h[4 * j + 1]);
+                    if (live1) *reinterpret_cast<float2 *>(p.act_dh1 + (size_t)m1 * WN + 8 * j + 2 * t) = make_float2(h[4 * j + 2], h[4 * j + 3]);
+                }
+            }
+            // ---- backward layer 1: d x = dh1 . W0 (N = 16) ----
+            float dx[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) dx[i] = 0.f;
+#pragma unroll
+            for (int kb = 0; kb < 8; ++kb) {
+                uint32_t ah[4][4], al[4][4];
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) frag3(h, 4 * kb + ks, ah[ks], al[ks]);
+                uint64_t bh, bl;
+                acquire(bh, bl);
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) mma3<8>(dx, ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
+                release();
+            }
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj) {
+                if (live0) *reinterpret_cast<float2 *>(p.dfeats + (size_t)m0 * 16 + 8 * jj + 2 * t) = make_float2(dx[4 * jj], dx[4 * jj + 1]);
+                if (live1) *reinterpret_cast<float2 *>(p.dfeats + (size_t)m1 * 16 + 8 * jj + 2 * t) = make_float2(dx[4 * jj + 2], dx[4 * jj + 3]);
             }
         }
-        if (WGRAD && g == 0) {
-            for (int off = 16; off > 0; off >>= 1) gb2r += __shfl_down_sync(0xffffffffu, gb2r, off);
-            if (lane == 0) atomicAdd(p.gb2, gb2r);
-        }
-        if (WGRAD && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // panel stores complete before exit
     }
-    tc_fence_before();
-    __syncthreads();
-    if (PAIR) cluster_sync_all();                // neither CTA leaves while the other may still multicast into it
-    if (warp == 9) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+    if (TRAIN && !p.dsdf_ext) {
+        for (int off = 16; off > 0; off >>= 1) {
+            loss_fs += __shfl_down_sync(0xffffffffu, loss_fs, off);
+            loss_sdf += __shfl_down_sync(0xffffffffu, loss_sdf, off);
+        }
+        if (lane == 0) {
+            if (loss_fs != 0.0) atomicAdd(&p.stats->fs_sum, loss_fs);
+            if (loss_sdf != 0.0) atomicAdd(&p.stats->sdf_sum, loss_sdf);
+        }
     }
 }
 
-// launch as clusters of two CTAs (even grid, at most one CTA per SM)
-template <class K>
-int launch_pair(K kernel, int grid, int sms, const TrainParams &p, cudaStream_t stream) {
-    grid = (grid + 1) & ~1;
-    if (grid > (sms & ~1)) grid = sms & ~1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid, 1, 1);
-    cfg.blockDim = dim3(NTHREADS_TRAIN, 1, 1);
-    cfg.dynamicSmemBytes = SMEM_TOTAL;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p);
+// gW1[j][k] += sum_s dh2[s][j] h1[s][k]: CTA = 128 x 128 output tile, split-K over samples (grid = 4 tiles x nsplit, one CTA
+// per SM: 148 registers per thread).
+// Chunks of 32 samples of both operands are double-buffered in shared memory by cp.async (rows padded to 136 floats: the
+// fragment loads (sample t / t+4, column g) hit 32 distinct banks); warp w owns rows 64 (w & 1) .. +63 and columns
+// 32 (w >> 1) .. +31 of the tile, 4 x 4 m16n8 accumulators.  hi/lo split of both operands at fragment load.
+constexpr int DW_KC = 32, DW_LD = 136;
+constexpr int DW_SMEM = 2 * 2 * DW_KC * DW_LD * 4;   // 68 KB: 2 operands x 2 buffers
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ dh2,
+                                                const float *__restrict__ h1, float *__restrict__ gW1, int nsplit) {
+    extern __shared__ float4 dw_smem[];
+    auto As = reinterpret_cast<float(*)[DW_KC][DW_LD]>(dw_smem);
+    auto Bs = reinterpret_cast<float(*)[DW_KC][DW_LD]>(reinterpret_cast<float *>(dw_smem) + 2 * DW_KC * DW_LD);
+    const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
+    const int tile = blockIdx.x & 3, split = blockIdx.x >> 2;
+    const int j0 = (tile >> 1) * 128, k0 = (tile & 1) * 128;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
+    const int wj = (warp & 1) * 64, wk = (warp >> 1) * 32;
+    float acc[4][4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
+    const long long nch = (M + DW_KC - 1) / DW_KC;
+    auto load = [&](long long ch, int buf) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int f = tid + i * 256, r = f >> 5, c4 = (f & 31) * 4;   // 32 rows x 32 float4
+            const long long s = ch * DW_KC + r;
+            const bool v = s < M;
+            const size_t o = (size_t)(v ? s : 0) * WN;
+            cp_async16(smem_u32(&As[buf][r][c4]), dh2 + o + j0 + c4, v);
+            cp_async16(smem_u32(&Bs[buf][r][c4]), h1 + o + k0 + c4, v);
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    int buf = 0;
+    if (split < nch) load(split, 0);
+    for (long long ch = split; ch < nch; ch += nsplit, buf ^= 1) {
+        if (ch + nsplit < nch) {
+            load(ch + nsplit, buf ^ 1);
+            asm volatile("cp.async.wait_group 1;" ::: "memory");
+        } else {
+            asm volatile("cp.async.wait_group 0;" ::: "memory");
+        }
+        __syncthreads();
+#pragma unroll
+        for (int ks = 0; ks < DW_KC / 8; ++ks) {
+            const int s0 = ks * 8 + t;
+            uint32_t ah[4][4], al[4][4], bh[4][2], bl[4][2];
+#pragma unroll
+            for (int mi = 0; mi < 4; ++mi) {
+                const int j = wj + mi * 16 + g;
+                const float v[4] = {As[buf][s0][j], As[buf][s0][j + 8], As[buf][s0 + 4][j], As[buf][s0 + 4][j + 8]};
+#pragma unroll
+                for (int i = 0; i < 4; ++i) { ah[mi][i] = tf32_rna(v[i]); al[mi][i] = tf32_rna(v[i] - __uint_as_float(ah[mi][i])); }
+            }
+#pragma unroll
+            for (int ni = 0; ni < 4; ++ni) {
+                const int n = wk + ni * 8 + g;
+                const float v[2] = {Bs[buf][s0][n], Bs[buf][s0 + 4][n]};
+#pragma unroll
+                for (int i = 0; i < 2; ++i) { bh[ni][i] = tf32_rna(v[i]); bl[ni][i] = tf32_rna(v[i] - __uint_as_float(bh[ni][i])); }
+            }
+#pragma unroll
+            for (int mi = 0; mi < 4; ++mi)
+#pragma unroll
+                for (int ni = 0; ni < 4; ++ni) {
+                    mma_tf32(acc[mi][ni], ah[mi], bh[ni][0], bh[ni][1]);
+                    mma_tf32(acc[mi][ni], ah[mi], bl[ni][0], bl[ni][1]);
+                    mma_tf32(acc[mi][ni], al[mi], bh[ni][0], bh[ni][1]);
+                }
+        }
+        __syncthreads();
+    }
+    if (split >= nch) return;
+#pragma unroll
+    for (int mi = 0; mi < 4; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < 4; ++ni) {
+            const int j = j0 + wj + mi * 16 + g, k = k0 + wk + ni * 8 + 2 * t;
+            atomicAdd(gW1 + (size_t)j * WN + k, acc[mi][ni][0]);
+            atomicAdd(gW1 + (size_t)j * WN + k + 1, acc[mi][ni][1]);
+            atomicAdd(gW1 + (size_t)(j + 8) * WN + k, acc[mi][ni][2]);
+            atomicAdd(gW1 + (size_t)(j + 8) * WN + k + 1, acc[mi][ni][3]);
+        }
+}
+
+// Column sums of the stored activations, thread = column k, one contiguous range of samples per CTA:
+//   gW0[k][e] += sum_s dh1[s][k] x[s][e]   gb0[k] += sum_s dh1[s][k]   gW2[k] += sum_s d[s] h2[s][k]
+//   gb1[k]    += sum_s dh2[s][k]           gb2    += sum_s d[s]
+constexpr int COLS_CHUNK = 64;
+__global__ void __launch_bounds__(WN) k_wg_cols(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ feats,
+                                                const float *__restrict__ dh1, const float *__restrict__ h2, const float *__restrict__ dh2,
+                                                const float *__restrict__ d, nl_mlp_grads g) {
+    __shared__ float xs[COLS_CHUNK][16];
+    __shared__ float ds[COLS_CHUNK];
+    const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
+    const long long per = ((M + gridDim.x - 1) / gridDim.x + COLS_CHUNK - 1) / COLS_CHUNK * COLS_CHUNK;
+    const long long s0 = (long long)blockIdx.x * per, s1 = min(M, s0 + per);
+    const int k = threadIdx.x;
+    float gw0[16], gb0 = 0.f, gw2 = 0.f, gb1 = 0.f, gb2 = 0.f;
+#pragma unroll
+    for (int e = 0; e < 16; ++e) gw0[e] = 0.f;
+    for (long long c0 = s0; c0 < s1; c0 += COLS_CHUNK) {
+        const int n = (int)min((long long)COLS_CHUNK, s1 - c0);
+        __syncthreads();
+        for (int i = k; i < n * 16; i += WN) xs[i >> 4][i & 15] = feats[(size_t)c0 * 16 + i];
+        if (k < n) ds[k] = d[c0 + k];
+        __syncthreads();
+        for (int i = 0; i < n; ++i) {
+            const size_t o = (size_t)(c0 + i) * WN + k;
+            const float a = dh1[o];
+#pragma unroll
+            for (int e = 0; e < 16; ++e) gw0[e] = fmaf(a, xs[i][e], gw0[e]);
+            gb0 += a;
+            gw2 = fmaf(ds[i], h2[o], gw2);
+            gb1 += dh2[o];
+            if (k == 0) gb2 += ds[i];
+        }
+    }
+    if (s0 >= s1) return;
+#pragma unroll
+    for (int e = 0; e < 16; ++e) atomicAdd(g.gW0 + k * 16 + e, gw0[e]);
+    atomicAdd(g.gb0 + k, gb0);
+    atomicAdd(g.gW2 + k, gw2);
+    atomicAdd(g.gb1 + k, gb1);
+    if (k == 0) atomicAdd(g.gb2, gb2);
+}
+
+template <bool TRAIN, bool WGRAD>
+int launch(const Params &p, cudaStream_t stream) {
+    static NlPerDevice configured;
+    const cudaError_t e = configured.once([] { return cudaFuncSetAttribute(k_mlp_wg<TRAIN, WGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL); });
     if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
+    const long long ntiles = (p.M_host + TM - 1) / TM;
+    const int grid = (int)(ntiles < (long long)nl_num_sms() ? ntiles : (long long)nl_num_sms());
+    k_mlp_wg<TRAIN, WGRAD><<<grid, NTHREADS, SMEM_TOTAL, stream>>>(p);
     return NL_OK;
-}
-
-// ================================================================================================
-// Weight gradients of the hidden and output layers on tensor cores.  With m2 = relu'(h2) (0/1) and d = dsdf:
-//   G[j][k]  = sum_s m2[s][j] * (d[s] h1[s][k])                 (256 x 256, fp32 in TMEM: 2 accumulators x 256 columns)
-//   gW1[j][k] += w2[j] G[j][k]                                   (= sum_s dh2[s][j] h1[s][k])
-//   gW2[j]    += sum_k W1[j][k] G[j][k]   (+ b1[j] c[j], added by k_mask_colsum;  = sum_s d[s] h2[s][j] because
-//                                            h2 = m2 * (h1 . W1^T + b1), c[j] = sum_s m2[s][j] d[s])
-//   K = samples, streamed in K-blocks of 16 rows.  Both operands are MN-major (SWIZZLE_128B_BASE32B, the only layout
-//   tcgen05 takes for MN-major tf32).  Per K-block the producer bulk-copies the 16 rows of the h1 panels (16 KB, the
-//   K-major image k_mlp_tc_train stored), 512 B of mask bits and 64 B of dsdf; 4 converter warps expand the bits into
-//   the 0/1 A operand (exact in tf32: one term fewer than 3xTF32) and write hi/lo of d*h1 as the B operand.
-//   3-deep raw ring (17 KB) + 2-deep converted ring (48 KB).  Every CTA finally adds its partial sums with atomics.
-// ================================================================================================
-constexpr int DW_KROWS = 16;
-constexpr int DW_PANEL = DW_KROWS * 128;        // 2 KB: 16 sample rows x 128 B
-constexpr int DW_OPER = 8 * DW_PANEL;           // 16 KB: all 256 columns of one operand
-constexpr int DW_BITS = DW_KROWS * 32;          // 512 B of relu'(h2) bits
-constexpr int DW_RAW = DW_OPER + 1024;          // h1 raw (K-major SWIZZLE_128B image as stored in HBM) | bits | dsdf
-constexpr int DW_CONV = 3 * DW_OPER;            // 48 KB: A mask | B hi | B lo (MN-major SWIZZLE_128B_BASE32B)
-// ring depths are kept small enough (149 KB / 161 KB of shared memory) that blocks of other kernels -- the next iteration's
-// traversal needs 48 KB -- can share the SM with these persistent CTAs when the engine pipelines iterations
-constexpr int dw_smem(int nraw, int nconv) { return nraw * DW_RAW + nconv * DW_CONV + 1024 + 1024; }
-
-// MN-major SWIZZLE_128B_BASE32B descriptor (layout type 1): LBO = byte stride between 32-element MN groups (= one 2 KB
-// panel), SBO = byte stride between groups of 4 K rows (512 B); one k-step (K = 8) spans two such groups
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(DW_PANEL >> 4) << 16) | (32ull << 32) | (1ull << 46) | (1ull << 61);
-}
-
-template <int NCW, int NRAW, int NCONV>   // converter warps (4 or 8), ring depths
-__global__ void __launch_bounds__(64 + 32 * NCW, 1) k_dw1_tc(long long M_host, const int32_t *__restrict__ M_dev, const uint32_t *__restrict__ act_mask2,
-                                                         const float *__restrict__ act_dsdf, const float *__restrict__ act_h1,
-                                                         const float *__restrict__ W1, const float *__restrict__ w2, float *__restrict__ gW1,
-                                                         float *__restrict__ gW2) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    uint8_t *sm = smem_raw + (base - raw);
-    // converted stages first: their operand tiles need 1024-byte alignment, the raw stages only 16
-    const uint32_t sConv = base, sRaw = base + NCONV * DW_CONV;
-    uint8_t *conv_gen = sm, *raw_gen = sm + NCONV * DW_CONV;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + NCONV * DW_CONV + NRAW * DW_RAW);
-    // barriers: 0..3 raw_full  4..7 raw_empty  8..10 conv_full  11..13 conv_empty  14 d_full
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 16);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
-    const long long nkb = ((M + TM - 1) / TM) * (TM / DW_KROWS);   // K-blocks of 16 rows (whole tiles: padded rows have dsdf = 0)
-    if (tid == 0) {
-        for (int i = 0; i < NRAW; ++i) { mbar_init(BAR(i), 1); mbar_init(BAR(4 + i), NCW); }
-        for (int i = 0; i < NCONV; ++i) { mbar_init(BAR(8 + i), NCW); mbar_init(BAR(11 + i), 1); }
-        mbar_init(BAR(14), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const bool has_work = (long long)blockIdx.x < nkb;
-
-    if (warp == 0) {
-        uint32_t it = 0;
-        for (long long kb = blockIdx.x; kb < nkb; kb += gridDim.x, ++it) {
-            const uint32_t s = it % NRAW, ph = (it / NRAW) & 1;
-            mbar_wait(BAR(4 + s), ph ^ 1);
-            if (elect_one()) {
-                mbar_expect_tx(BAR(0 + s), DW_OPER + DW_BITS + DW_KROWS * 4);
-                const long long tile = kb >> 3;
-                const int r0 = (int)(kb & 7) * DW_KROWS;
-                const uint32_t dst = sRaw + s * DW_RAW;
-#pragma unroll
-                for (int pnl = 0; pnl < 8; ++pnl)
-                    bulk_g2s(dst + pnl * DW_PANEL, act_h1 + ((size_t)(tile * 8 + pnl) * TM + r0) * 32, DW_PANEL, BAR(0 + s));
-                bulk_g2s(dst + DW_OPER, act_mask2 + (size_t)(tile * TM + r0) * 8, DW_BITS, BAR(0 + s));
-                bulk_g2s(dst + DW_OPER + DW_BITS, act_dsdf + tile * TM + r0, DW_KROWS * 4, BAR(0 + s));
-            }
-            __syncwarp();
-        }
-    } else if (warp == 1) {
-        if (has_work) {
-            // M = 128 (rows j), N = 256 (columns k), both operands MN-major (bits 15, 16)
-            constexpr uint32_t idesc = make_idesc(TM, WN) | (1u << 15) | (1u << 16);
-            uint32_t it = 0;
-            for (long long kb = blockIdx.x; kb < nkb; kb += gridDim.x, ++it) {
-                const uint32_t s = it % NCONV, ph = (it / NCONV) & 1;
-                mbar_wait(BAR(8 + s), ph);
-                tc_fence_after();
-                const uint32_t a_m = sConv + s * DW_CONV, b_hi = a_m + DW_OPER, b_lo = a_m + 2 * DW_OPER;
-                if (elect_one()) {
-#pragma unroll
-                    for (int jt = 0; jt < 2; ++jt) {
-                        uint32_t acc = it > 0 ? 1u : 0u;
-#pragma unroll
-                        for (int term = 0; term < 2; ++term) {
-                            const uint32_t a0 = a_m + jt * 4 * DW_PANEL;
-                            const uint32_t b0 = (term == 1 ? b_lo : b_hi);
-#pragma unroll
-                            for (int ks = 0; ks < DW_KROWS / 8; ++ks) {
-                                mma_tf32(tmem + jt * 256, make_desc_mn(a0 + ks * 1024), make_desc_mn(b0 + ks * 1024), idesc, acc);
-                                acc = 1u;
-                            }
-                        }
-                    }
-                    tc_commit(BAR(11 + s));
-                }
-                __syncwarp();
-            }
-            if (elect_one()) tc_commit(BAR(14));
-            __syncwarp();
-        }
-    } else {
-        // converters (128 threads).  Stored h1 image: K-major SWIZZLE_128B (16 B chunk c of row r at c ^ (r & 7)); operand
-        // tiles: MN-major SWIZZLE_128B_BASE32B (32 B chunk c of row r at c ^ (r & 3)).  hi = the fp32 bits of d*h1
-        // (truncated to tf32 by the hardware), lo = tf32(x - trunc(x)).
-        constexpr int NCT = 32 * NCW;                              // converter threads
-        const int ct = tid - 64;
-        // mask expansion: one (column block, sample row) per group of NCT/128 threads, 8 / (NCT/128) float4 each
-        constexpr int MSPLIT = NCT / 128;
-        const int m_pair = ct / MSPLIT, m_part = ct % MSPLIT;
-        const int m_pnl = m_pair >> 4, m_lr = m_pair & 15;
-        const int m_word = (m_pnl & 1) * 4 + (m_pnl >> 1);         // storage order of k_mlp_tc_train: [group][kk]
-        uint32_t it = 0;
-        for (long long kb = blockIdx.x; kb < nkb; kb += gridDim.x, ++it) {
-            const uint32_t rs = it % NRAW, rph = (it / NRAW) & 1;
-            const uint32_t cs = it % NCONV, cph = (it / NCONV) & 1;
-            mbar_wait(BAR(0 + rs), rph);          // raw tiles landed
-            mbar_wait(BAR(11 + cs), cph ^ 1);     // converted stage free (its MMAs retired)
-            const uint8_t *rawp = raw_gen + rs * DW_RAW;
-            const float4 *src = reinterpret_cast<const float4 *>(rawp);
-            const uint32_t *bits = reinterpret_cast<const uint32_t *>(rawp + DW_OPER);
-            const float *dsd = reinterpret_cast<const float *>(rawp + DW_OPER + DW_BITS);
-            float4 *am = reinterpret_cast<float4 *>(conv_gen + cs * DW_CONV);
-            float4 *hi = reinterpret_cast<float4 *>(conv_gen + cs * DW_CONV + DW_OPER);
-            float4 *lo = reinterpret_cast<float4 *>(conv_gen + cs * DW_CONV + 2 * DW_OPER);
-            {
-                const uint32_t mk = bits[m_lr * 8 + m_word];
-#pragma unroll
-                for (int cc = 0; cc < 8 / MSPLIT; ++cc) {
-                    const int c16 = m_part * (8 / MSPLIT) + cc;
-                    const int d16 = (((c16 >> 1) ^ (m_lr & 3)) << 1) | (c16 & 1);
-                    am[(m_pnl << 7) | (m_lr << 3) | d16] =
-                        make_float4((mk >> (4 * c16)) & 1u ? 1.f : 0.f, (mk >> (4 * c16 + 1)) & 1u ? 1.f : 0.f,
-                                    (mk >> (4 * c16 + 2)) & 1u ? 1.f : 0.f, (mk >> (4 * c16 + 3)) & 1u ? 1.f : 0.f);
-                }
-            }
-#pragma unroll 4
-            for (int f = ct; f < DW_OPER / 16; f += NCT) {        // f: float4 index = (panel, local row, stored chunk)
-                const int pnl = f >> 7, lr = (f >> 3) & 15, p16 = f & 7;
-                const int c16 = p16 ^ (lr & 7);                   // logical 16 B chunk (r0 is a multiple of 16: r & 7 == lr & 7)
-                const int d16 = (((c16 >> 1) ^ (lr & 3)) << 1) | (c16 & 1);
-                const float d = dsd[lr];
-                float4 v = src[f];
-                v.x *= d; v.y *= d; v.z *= d; v.w *= d;
-                float4 l;
-                l.x = tf32_rna(v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u));
-                l.y = tf32_rna(v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u));
-                l.z = tf32_rna(v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u));
-                l.w = tf32_rna(v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u));
-                const int o = (pnl << 7) | (lr << 3) | d16;
-                hi[o] = v;
-                lo[o] = l;
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(BAR(8 + cs)); mbar_arrive(BAR(4 + rs)); }
-        }
-        // epilogue: thread = row j of each accumulator; add the CTA's partial sums into gW1 (scaled by w2[j]) and gW2
-        if (has_work) {
-            mbar_wait(BAR(14), 0);
-            tc_fence_after();
-            const int q = warp & 3;
-            const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-            // all CTAs finish at about the same time: start each one at a different (accumulator, column block) so the
-            // 148 partial sums do not hammer the same L2 lines simultaneously.  With 8 converter warps each accumulator
-            // half is drained by its own 4 warps.
-            for (int jj = 0; jj < (NCW == 8 ? 1 : 2); ++jj) {
-                const int jt = NCW == 8 ? ((warp - 2) >> 2) : ((jj + (blockIdx.x >> 3)) & 1);
-                const int j = jt * 128 + q * 32 + lane;
-                const float w2j = w2[j];
-                float dot = 0.f;
-                for (int cc = 0; cc < 8; ++cc) {
-                    const int cb = (cc + blockIdx.x) & 7;
-                    uint32_t v[32];
-                    tmem_ld32(tmem + lane_addr + jt * 256 + cb * 32, v);
-                    float4 *o = reinterpret_cast<float4 *>(gW1 + (size_t)j * WN + cb * 32);
-                    const float4 *wr = reinterpret_cast<const float4 *>(W1 + (size_t)j * WN + cb * 32);
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        const float4 w = wr[c];
-                        const float g0 = __uint_as_float(v[c * 4]), g1 = __uint_as_float(v[c * 4 + 1]), g2 = __uint_as_float(v[c * 4 + 2]),
-                                    g3 = __uint_as_float(v[c * 4 + 3]);
-                        dot = fmaf(w.x, g0, fmaf(w.y, g1, fmaf(w.z, g2, fmaf(w.w, g3, dot))));
-                        atomicAdd(o + c, make_float4(w2j * g0, w2j * g1, w2j * g2, w2j * g3));
-                    }
-                }
-                atomicAdd(gW2 + j, dot);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-    }
-}
-
-// ================================================================================================
-// Weight gradient of the first layer on tensor cores:  gW0[k][e] += sum_s dh1[s][k] x[s][e],  gb0[k] += sum_s dh1[s][k]
-//   Same streaming skeleton as k_dw1_tc (K = samples in K-blocks of 16 rows, MN-major operands).  A = dh1^T from the
-//   stored panels (hi = fp32 bits, lo = x - trunc(x)), B = one 32-column panel [x (16) | 1 | 0 ...] (hi/lo), so column 16 of
-//   the accumulator is the bias gradient.  D = 256 x 32 fp32 in TMEM (2 x 32 columns), 3 tf32 terms, N = 32 MMAs.
-// ================================================================================================
-constexpr int D0_RAW = DW_OPER + 1024;          // dh1 raw (16 KB) | x rows (16 x 64 B)
-constexpr int D0_CONV = 2 * DW_OPER + 2 * DW_PANEL;   // A hi | A lo | B hi | B lo = 36 KB
-constexpr int d0_smem(int nraw, int nconv) { return nraw * D0_RAW + nconv * D0_CONV + 1024 + 1024; }
-
-template <int NCW, int NRAW, int NCONV>
-__global__ void __launch_bounds__(64 + 32 * NCW, 1) k_dw0_tc(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ act_dh1,
-                                                         const float *__restrict__ feats, float *__restrict__ gW0, float *__restrict__ gb0) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    uint8_t *sm = smem_raw + (base - raw);
-    const uint32_t sConv = base, sRaw = base + NCONV * D0_CONV;
-    uint8_t *conv_gen = sm, *raw_gen = sm + NCONV * D0_CONV;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + NCONV * D0_CONV + NRAW * D0_RAW);
-    // barriers: 0..3 raw_full  4..7 raw_empty  8..11 conv_full  12..15 conv_empty  16 d_full
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 18);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
-    const long long nkb = ((M + TM - 1) / TM) * (TM / DW_KROWS);
-    if (tid == 0) {
-        for (int i = 0; i < NRAW; ++i) { mbar_init(BAR(i), 1); mbar_init(BAR(4 + i), NCW); }
-        for (int i = 0; i < NCONV; ++i) { mbar_init(BAR(8 + i), NCW); mbar_init(BAR(12 + i), 1); }
-        mbar_init(BAR(16), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(64u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const bool has_work = (long long)blockIdx.x < nkb;
-
-    if (warp == 0) {
-        uint32_t it = 0;
-        for (long long kb = blockIdx.x; kb < nkb; kb += gridDim.x, ++it) {
-            const uint32_t s = it % NRAW, ph = (it / NRAW) & 1;
-            mbar_wait(BAR(4 + s), ph ^ 1);
-            if (elect_one()) {
-                const long long tile = kb >> 3;
-                const int r0 = (int)(kb & 7) * DW_KROWS;
-                const long long left = M - (tile * TM + r0);                       // feature rows that exist (the panels are tile-padded,
-                const uint32_t xrows = left >= DW_KROWS ? DW_KROWS : (left > 0 ? (uint32_t)left : 0u);   // the feature array is not)
-                mbar_expect_tx(BAR(0 + s), DW_OPER + xrows * 64);
-                const uint32_t dst = sRaw + s * D0_RAW;
-#pragma unroll
-                for (int pnl = 0; pnl < 8; ++pnl)
-                    bulk_g2s(dst + pnl * DW_PANEL, act_dh1 + ((size_t)(tile * 8 + pnl) * TM + r0) * 32, DW_PANEL, BAR(0 + s));
-                if (xrows) bulk_g2s(dst + DW_OPER, feats + (size_t)(tile * TM + r0) * 16, xrows * 64, BAR(0 + s));
-            }
-            __syncwarp();
-        }
-    } else if (warp == 1) {
-        if (has_work) {
-            constexpr uint32_t idesc = make_idesc(TM, 32) | (1u << 15) | (1u << 16);   // both operands MN-major
-            uint32_t it = 0;
-            for (long long kb = blockIdx.x; kb < nkb; kb += gridDim.x, ++it) {
-                const uint32_t s = it % NCONV, ph = (it / NCONV) & 1;
-                mbar_wait(BAR(8 + s), ph);
-                tc_fence_after();
-                const uint32_t a_hi = sConv + s * D0_CONV, a_lo = a_hi + DW_OPER, b_hi = a_hi + 2 * DW_OPER, b_lo = b_hi + DW_PANEL;
-                if (elect_one()) {
-#pragma unroll
-                    for (int jt = 0; jt < 2; ++jt) {
-                        uint32_t acc = it > 0 ? 1u : 0u;
-#pragma unroll
-                        for (int term = 0; term < 3; ++term) {
-                            const uint32_t a0 = (term == 2 ? a_lo : a_hi) + jt * 4 * DW_PANEL;
-                            const uint32_t b0 = (term == 1 ? b_lo : b_hi);
-#pragma unroll
-                            for (int ks = 0; ks < DW_KROWS / 8; ++ks) {
-                                mma_tf32(tmem + jt * 32, make_desc_mn(a0 + ks * 1024), make_desc_mn(b0 + ks * 1024), idesc, acc);
-                                acc = 1u;
-                            }
-                        }
-                    }
-                    tc_commit(BAR(12 + s));
-                }
-                __syncwarp();
-            }
-            if (elect_one()) tc_commit(BAR(16));
-            __syncwarp();
-        }
-    } else {
-        const int ct = tid - 64;
-        uint32_t it = 0;
-        for (long long kb = blockIdx.x; kb < nkb; kb += gridDim.x, ++it) {
-            const uint32_t rs = it % NRAW, rph = (it / NRAW) & 1;
-            const uint32_t cs = it % NCONV, cph = (it / NCONV) & 1;
-            mbar_wait(BAR(0 + rs), rph);
-            mbar_wait(BAR(12 + cs), cph ^ 1);
-            const uint8_t *rawp = raw_gen + rs * D0_RAW;
-            const float4 *src = reinterpret_cast<const float4 *>(rawp);
-            float4 *hi = reinterpret_cast<float4 *>(conv_gen + cs * D0_CONV);
-            float4 *lo = reinterpret_cast<float4 *>(conv_gen + cs * D0_CONV + DW_OPER);
-            float4 *bh = reinterpret_cast<float4 *>(conv_gen + cs * D0_CONV + 2 * DW_OPER);
-            float4 *bl = reinterpret_cast<float4 *>(conv_gen + cs * D0_CONV + 2 * DW_OPER + DW_PANEL);
-            if (ct < 128) {   // B panel: row lr = [x (16 floats) | 1 | 0 x 15], 32-byte chunk c stored at c ^ (lr & 3)
-                const int lr = (ct & 63) >> 2, j = ct & 3;
-                const long long m = (kb >> 3) * TM + (kb & 7) * DW_KROWS + lr;
-                float4 v, l = make_float4(0.f, 0.f, 0.f, 0.f);
-                int chunk;
-                if (ct < 64) {
-                    chunk = j >> 1;
-                    v = (m < M) ? reinterpret_cast<const float4 *>(rawp + DW_OPER)[lr * 4 + j] : make_float4(0.f, 0.f, 0.f, 0.f);
-                    l.x = tf32_rna(v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u));
-                    l.y = tf32_rna(v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u));
-                    l.z = tf32_rna(v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u));
-                    l.w = tf32_rna(v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u));
-                } else {
-                    chunk = 2 + (j >> 1);
-                    v = make_float4(j == 0 ? 1.f : 0.f, 0.f, 0.f, 0.f);
-                }
-                const int o = (lr << 3) | ((chunk ^ (lr & 3)) << 1) | (j & 1);
-                bh[o] = v;
-                bl[o] = l;
-            }
-#pragma unroll 4
-            for (int f = ct; f < DW_OPER / 16; f += 32 * NCW) {
-                const int pnl = f >> 7, lr = (f >> 3) & 15, p16 = f & 7;
-                const int c16 = p16 ^ (lr & 7);
-                const int d16 = (((c16 >> 1) ^ (lr & 3)) << 1) | (c16 & 1);
-                const float4 v = src[f];
-                float4 l;
-                l.x = tf32_rna(v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u));
-                l.y = tf32_rna(v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u));
-                l.z = tf32_rna(v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u));
-                l.w = tf32_rna(v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u));
-                const int o = (pnl << 7) | (lr << 3) | d16;
-                hi[o] = v;
-                lo[o] = l;
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(BAR(8 + cs)); mbar_arrive(BAR(4 + rs)); }
-        }
-        if (has_work) {
-            mbar_wait(BAR(16), 0);
-            tc_fence_after();
-            const int q = warp & 3;
-            const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-            for (int jj = 0; jj < (NCW == 8 ? 1 : 2); ++jj) {
-                const int jt = NCW == 8 ? ((warp - 2) >> 2) : ((jj + (blockIdx.x >> 3)) & 1);
-                const int k = jt * 128 + q * 32 + lane;
-                uint32_t v[32];
-                tmem_ld32(tmem + lane_addr + jt * 32, v);
-                float4 *o = reinterpret_cast<float4 *>(gW0 + (size_t)k * 16);
-#pragma unroll
-                for (int c = 0; c < 4; ++c)
-                    atomicAdd(o + c, make_float4(__uint_as_float(v[c * 4]), __uint_as_float(v[c * 4 + 1]), __uint_as_float(v[c * 4 + 2]),
-                                                 __uint_as_float(v[c * 4 + 3])));
-                atomicAdd(gb0 + k, __uint_as_float(v[16]));
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(64u) : "memory");
-    }
-}
-
-// c[j] = sum_m relu'(h2)[m][j] dsdf[m]  ->  gb1[j] += w2[j] c[j],  gW2[j] += b1[j] c[j]  (the other part of gW2 comes from
-// k_dw1_tc).  thread = (storage word w = tid & 7, row lane tid >> 3); 36 B/sample, a few tens of microseconds
-__global__ void __launch_bounds__(256) k_mask_colsum(long long M_host, const int32_t *__restrict__ M_dev, const uint32_t *__restrict__ mask2,
-                                                      const float *__restrict__ dsdf, const float *__restrict__ b1, const float *__restrict__ w2,
-                                                      float *__restrict__ gb1, float *__restrict__ gW2) {
-    const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
-    const int w = threadIdx.x & 7, rl = threadIdx.x >> 3;
-    float acc[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-    const long long stride = (long long)gridDim.x * 32;
-    for (long long m0 = (long long)blockIdx.x * 32 + rl; m0 < M; m0 += 4 * stride) {   // 4 independent rows in flight per thread
-        uint32_t mk[4];
-        float d[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const long long m = m0 + u * stride;
-            mk[u] = m < M ? mask2[(size_t)m * 8 + w] : 0u;
-            d[u] = m < M ? dsdf[m] : 0.f;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-#pragma unroll
-            for (int i = 0; i < 32; ++i) acc[i] += (mk[u] >> i) & 1u ? d[u] : 0.f;
-    }
-    __shared__ float red[32][257];
-    const int cb = 2 * (w & 3) + (w >> 2);               // storage word g*4+kk holds columns 32(2kk+g)..+31
-#pragma unroll
-    for (int i = 0; i < 32; ++i) red[rl][cb * 32 + i] = acc[i];
-    __syncthreads();
-    const int j = threadIdx.x;
-    float c = 0.f;
-#pragma unroll 8
-    for (int r = 0; r < 32; ++r) c += red[r][j];
-    atomicAdd(gb1 + j, w2[j] * c);
-    atomicAdd(gW2 + j, b1[j] * c);
 }
 
 }  // namespace tc
@@ -1382,21 +646,16 @@ extern "C" int nl_mlp_tc_forward(int64_t M, const int32_t *d_M_dev, const float 
     if (M < 0) return nl_set_error("nl_mlp_tc_forward: negative M");
     if (M == 0) return NL_OK;
     if (!feats || !panels || !b0 || !b1 || !w2 || !b2 || !sdf) return nl_set_error("nl_mlp_tc_forward: null pointer");
-    static NlPerDevice configured;
-    const cudaError_t e0 = configured.once([] { return cudaFuncSetAttribute(tc::k_mlp_tc_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL); });
-    if (e0 != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e0));
-    tc::FwdParams p;
+    tc::Params p = {};
     p.M_host = M; p.M_dev = d_M_dev; p.feats = feats; p.panels = (const uint8_t *)panels;
     p.b0 = b0; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.sdf = sdf;
-    const long long ntiles = (M + tc::TM - 1) / tc::TM;
-    const int grid = (int)(ntiles < (long long)nl_num_sms() ? ntiles : (long long)nl_num_sms());
-    tc::k_mlp_tc_fwd<<<grid, tc::NTHREADS, tc::SMEM_TOTAL, (cudaStream_t)stream>>>(p);
+    if (int rc = tc::launch<false, false>(p, (cudaStream_t)stream)) return rc;
     NL_CHECK_LAUNCH("nl_mlp_tc_forward");
     return NL_OK;
 }
 
-// per 128-sample tile: h1 and dh1 panels (2 x 128 KB), dsdf (512 B), relu'(h2) bits (4 KB)
-extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * (2 * 8 * tc::TM * 32 + tc::TM + tc::TM * 8); }
+// h1, h2, dh2, dh1 [cap][256] and d loss / d sdf [cap], cap = M rounded up to whole tiles
+extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * (4 * tc::WN + 1); }
 
 extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *feats, const void *panels, const float *W1, const float *b0,
                                const float *b1, const float *w2, const float *b2, const uint8_t *s_flag, const float *s_depth,
@@ -1411,129 +670,40 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
         return nl_set_error("nl_mlp_tc_train: the loss needs s_flag, s_depth, s_ray, gt_depth and stats");
     if (grads && (!grads->gW0 || !grads->gb0 || !grads->gW1 || !grads->gb1 || !grads->gW2 || !grads->gb2 || !act))
         return nl_set_error("nl_mlp_tc_train: decoder gradients requested but a buffer is null");
-    // per-device one-time state (kernel attributes are per device; so is the event that orders the weight-gradient stream)
-    constexpr int NL_MAX_DEV = 64;
-    static std::mutex dev_mu;
-    static bool configured_dev[NL_MAX_DEV] = {};
-    static cudaEvent_t ev_dev[NL_MAX_DEV] = {};
-    static cudaStream_t s2_dev[NL_MAX_DEV] = {};                    // internal stream of k_dw0_tc when the two weight-gradient kernels run side by side
-    static cudaEvent_t e2_dev[NL_MAX_DEV] = {}, e3_dev[NL_MAX_DEV] = {};
-    int cur_dev = 0;
-    if (cudaGetDevice(&cur_dev) != cudaSuccess || cur_dev < 0 || cur_dev >= NL_MAX_DEV) return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: cudaGetDevice");
-    std::lock_guard<std::mutex> dev_lock(dev_mu);
-    bool &configured = configured_dev[cur_dev];
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(tc::k_mlp_tc_train<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::k_mlp_tc_train<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::k_mlp_tc_train<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::k_mlp_tc_train<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::k_mlp_tc_train<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::k_mlp_tc_train<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL);
-#define NL_DW_ATTR(K, NR, NC, SM)                                                                                               \
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::K<4, NR, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SM(NR, NC)); \
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::K<8, NR, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SM(NR, NC));
-        NL_DW_ATTR(k_dw1_tc, 4, 3, dw_smem) NL_DW_ATTR(k_dw1_tc, 3, 3, dw_smem) NL_DW_ATTR(k_dw1_tc, 3, 2, dw_smem)
-        NL_DW_ATTR(k_dw0_tc, 4, 4, d0_smem) NL_DW_ATTR(k_dw0_tc, 4, 3, d0_smem) NL_DW_ATTR(k_dw0_tc, 3, 3, d0_smem)
-#undef NL_DW_ATTR
-        if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
-        configured = true;
-    }
-    tc::TrainParams p = {};
+    tc::Params p = {};
     p.M_host = M; p.M_dev = d_M_dev; p.feats = feats; p.panels = (const uint8_t *)panels;
     p.b0 = b0; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.sdf = sdf; p.dfeats = dfeats;
     p.s_flag = s_flag; p.s_depth = s_depth; p.s_ray = s_ray; p.cosv = cosv; p.gt_depth = gt_depth; p.stats = stats;
     p.truncation = truncation; p.dsdf_ext = dsdf_ext;
-    const long long ntiles = (M + tc::TM - 1) / tc::TM;
-    const int sms = nl_num_sms();
-    int grid = (int)(ntiles < (long long)sms ? ntiles : (long long)sms);
-    // NL_TC_PAIR=1: CTA pairs share every weight stage through multicast copies (see k_mlp_tc_train); needs TS and an even grid
-    static const bool use_pair = [] { const char *e = getenv("NL_TC_PAIR"); return e ? atoi(e) != 0 : false; }();
-    static long long *dbg_dev = nullptr;
-    static int dbg_calls = 0;
-    const bool want_dbg = getenv("NL_TC_TIMELINE") != nullptr;
-    static const int conv_warps = [] { const char *e = getenv("NL_DW_CONV_WARPS"); return (e && atoi(e) == 4) ? 4 : 8; }();   // converter warps of the weight-gradient kernels
-    static const int dw_rings = [] {
-        const char *e = getenv("NL_DW_RINGS");
-        return !e ? 2 : (e[0] == 's' ? 0 : (e[0] == 'm' ? 1 : 2));
-    }();
-    static const bool use_ts = [] { const char *e = getenv("NL_TC_TS"); return e ? atoi(e) != 0 : true; }();   // A operands of the backward GEMMs from TMEM (NL_TC_TS=0: shared memory)
-    if (want_dbg && !dbg_dev) { cudaMalloc(&dbg_dev, 4 * 25 * 8 * sizeof(long long)); cudaMemset(dbg_dev, 0, 4 * 25 * 8 * sizeof(long long)); }
-    p.dbg = want_dbg ? dbg_dev : nullptr;
-    if (grads) {
-        const size_t panel = (size_t)ntiles * 8 * tc::TM * 32;   // capacity-based carve (M is the host-side bound)
-        p.act_h1 = act; p.act_dh1 = act + panel; p.act_dsdf = act + 2 * panel;
-        p.act_mask2 = reinterpret_cast<uint32_t *>(act + 2 * panel + (size_t)ntiles * tc::TM);
-        p.gb2 = grads->gb2;
-        if (use_ts && use_pair) { if (int rc = tc::launch_pair(tc::k_mlp_tc_train<true, true, true>, grid, sms, p, stream)) return rc; }
-        else if (use_ts) tc::k_mlp_tc_train<true, true, false><<<grid, tc::NTHREADS_TRAIN, tc::SMEM_TOTAL, stream>>>(p);
-        else tc::k_mlp_tc_train<true, false, false><<<grid, tc::NTHREADS_TRAIN, tc::SMEM_TOTAL, stream>>>(p);
-        // The weight-gradient kernels only need what the kernel above wrote; on a second stream they overlap with whatever the
-        // caller enqueues next on `stream` (the embedding scatter, which is L2-atomic bound and leaves the SMs mostly idle).
-        cudaStream_t ws = wgrad_stream_ ? (cudaStream_t)wgrad_stream_ : stream;
-        if (ws != stream) {
-            cudaEvent_t &ev = ev_dev[cur_dev];
-            if (!ev && cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, "cudaEventCreate");
-            if (cudaEventRecord(ev, stream) != cudaSuccess || cudaStreamWaitEvent(ws, ev, 0) != cudaSuccess)
-                return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not order the weight-gradient stream behind the decoder kernel");
-        }
-        // ring depths (raw, converted): "deep" (4,3)/(4,4) = 219 KB of shared memory per CTA, "mid" (3,3)/(4,3) = 201/183 KB,
-        // "shallow" (3,2)/(3,3) = 149/161 KB -- the smaller ones leave room for blocks of other kernels on the same SM when
-        // the engine pipelines iterations (NL_DW_RINGS)
-        // Experiment kept behind a switch (default off): the two weight-gradient kernels are independent -- k_dw1_tc tensor-bound,
-        // k_dw0_tc streaming 1 KB/sample for a 256x32 result -- so they could run side by side on disjoint SM subsets
-        // (NL_DW_SPLIT = SMs given to k_dw1_tc, the rest to k_dw0_tc on an internal third stream) instead of back to back.
-        // Measured on the B200: slower for every split (100: +0.05 ms ... 126: +0.6 ms per step) -- k_dw0_tc is limited per SM
-        // (its converter warps), not by HBM chip-wide, so it needs all 148 SMs.
-        static const int dw_split = [] { const char *e = getenv("NL_DW_SPLIT"); return e ? atoi(e) : 0; }();
-        const bool split = dw_split > 0 && dw_split < sms - 8;
-        const int sms1 = split ? dw_split : sms, sms0 = split ? sms - dw_split : sms;
-        cudaStream_t ws0 = ws;
-        if (split) {
-            if (!s2_dev[cur_dev] && (cudaStreamCreateWithFlags(&s2_dev[cur_dev], cudaStreamNonBlocking) != cudaSuccess ||
-                                     cudaEventCreateWithFlags(&e2_dev[cur_dev], cudaEventDisableTiming) != cudaSuccess ||
-                                     cudaEventCreateWithFlags(&e3_dev[cur_dev], cudaEventDisableTiming) != cudaSuccess))
-                return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not create the internal weight-gradient stream");
-            ws0 = s2_dev[cur_dev];
-            if (cudaEventRecord(e2_dev[cur_dev], ws) != cudaSuccess || cudaStreamWaitEvent(ws0, e2_dev[cur_dev], 0) != cudaSuccess)   // fork behind the decoder kernel
-                return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not fork the internal weight-gradient stream");
-        }
-#define NL_DW_LAUNCH(NCW_, THR, R1, C1, R0, C0)                                                                                     \
-        tc::k_dw1_tc<NCW_, R1, C1><<<sms1, THR, tc::dw_smem(R1, C1), ws>>>(M, d_M_dev, p.act_mask2, p.act_dsdf, p.act_h1, W1, w2, grads->gW1, \
-                                                                            grads->gW2);                                             \
-        tc::k_dw0_tc<NCW_, R0, C0><<<sms0, THR, tc::d0_smem(R0, C0), ws0>>>(M, d_M_dev, p.act_dh1, feats, grads->gW0, grads->gb0);
-        if (conv_warps == 8) {
-            if (dw_rings == 2) { NL_DW_LAUNCH(8, 320, 4, 3, 4, 4) } else if (dw_rings == 1) { NL_DW_LAUNCH(8, 320, 3, 3, 4, 3) } else { NL_DW_LAUNCH(8, 320, 3, 2, 3, 3) }
-        } else {
-            if (dw_rings == 2) { NL_DW_LAUNCH(4, 192, 4, 3, 4, 4) } else if (dw_rings == 1) { NL_DW_LAUNCH(4, 192, 3, 3, 4, 3) } else { NL_DW_LAUNCH(4, 192, 3, 2, 3, 3) }
-        }
-#undef NL_DW_LAUNCH
-        if (split) {      // join: `ws` (what the caller waits on) completes only after k_dw0_tc
-            if (cudaEventRecord(e3_dev[cur_dev], ws0) != cudaSuccess || cudaStreamWaitEvent(ws, e3_dev[cur_dev], 0) != cudaSuccess)
-                return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not join the internal weight-gradient stream");
-        }
-        tc::k_mask_colsum<<<sms * 8, 256, 0, ws>>>(M, d_M_dev, p.act_mask2, p.act_dsdf, b1, w2, grads->gb1, grads->gW2);
-    } else {
-        if (use_ts && use_pair) { if (int rc = tc::launch_pair(tc::k_mlp_tc_train<false, true, true>, grid, sms, p, stream)) return rc; }
-        else if (use_ts) tc::k_mlp_tc_train<false, true, false><<<grid, tc::NTHREADS_TRAIN, tc::SMEM_TOTAL, stream>>>(p);
-        else tc::k_mlp_tc_train<false, false, false><<<grid, tc::NTHREADS_TRAIN, tc::SMEM_TOTAL, stream>>>(p);
+    if (!grads) {
+        if (int rc = tc::launch<true, false>(p, stream)) return rc;
+        NL_CHECK_LAUNCH("nl_mlp_tc_train");
+        return NL_OK;
     }
+    const size_t cap = (size_t)((M + tc::TM - 1) / tc::TM) * tc::TM, plane = cap * tc::WN;
+    p.act_h1 = act; p.act_h2 = act + plane; p.act_dh2 = act + 2 * plane; p.act_dh1 = act + 3 * plane; p.act_d = act + 4 * plane;
+    if (int rc = tc::launch<true, true>(p, stream)) return rc;
+    // The weight-gradient kernels only need what the kernel above wrote; on a second stream they overlap with whatever the
+    // caller enqueues next on `stream` (the embedding scatter).
+    cudaStream_t ws = wgrad_stream_ ? (cudaStream_t)wgrad_stream_ : stream;
+    if (ws != stream) {
+        constexpr int NL_MAX_DEV = 64;
+        static std::mutex mu;
+        static cudaEvent_t ev_dev[NL_MAX_DEV] = {};
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= NL_MAX_DEV) return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: cudaGetDevice");
+        std::lock_guard<std::mutex> lock(mu);
+        cudaEvent_t &ev = ev_dev[dev];
+        if (!ev && cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, "cudaEventCreate");
+        if (cudaEventRecord(ev, stream) != cudaSuccess || cudaStreamWaitEvent(ws, ev, 0) != cudaSuccess)
+            return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not order the weight-gradient stream behind the decoder kernel");
+    }
+    static NlPerDevice dw_configured;
+    const cudaError_t e = dw_configured.once([] { return cudaFuncSetAttribute(tc::k_dw1_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::DW_SMEM); });
+    if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
+    const int nsplit = nl_num_sms() / 4 > 0 ? nl_num_sms() / 4 : 1;
+    tc::k_dw1_tc<<<4 * nsplit, 256, tc::DW_SMEM, ws>>>(M, d_M_dev, p.act_dh2, p.act_h1, grads->gW1, nsplit);
+    tc::k_wg_cols<<<nl_num_sms() * 4, tc::WN, 0, ws>>>(M, d_M_dev, feats, p.act_dh1, p.act_h2, p.act_dh2, p.act_d, *grads);
     NL_CHECK_LAUNCH("nl_mlp_tc_train");
-    if (want_dbg && ++dbg_calls == 8) {   // debug only: dump one steady-state tile timeline of CTA 0 (synchronises)
-        long long h[800];
-        cudaStreamSynchronize(stream);
-        cudaMemcpy(h, dbg_dev, sizeof(h), cudaMemcpyDeviceToHost);
-        long long t0 = h[0];
-        for (int i = 0; i < 800; ++i) if (h[i] && h[i] < t0) t0 = h[i];
-        const char *roles[4] = {"producer", "mma", "epi_g0", "epi_g1"};
-        for (int r = 0; r < 4; ++r)
-            for (int st = 0; st < 25; ++st) {
-                long long *q = h + (r * 25 + st) * 8;
-                if (q[0] || q[1] || q[2] || q[3]) {
-                    fprintf(stderr, "TL %-8s step %2d :", roles[r], st);
-                    for (int k = 0; k < 8; ++k) fprintf(stderr, " %7lld", q[k] ? q[k] - t0 : -1);
-                    fprintf(stderr, "\n");
-                }
-            }
-    }
     return NL_OK;
 }

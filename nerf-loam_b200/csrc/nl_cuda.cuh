@@ -1,4 +1,4 @@
-// Small CUDA helpers shared by the kernels of libnerfloam_b200.so (sm_100a only).
+// Small CUDA helpers shared by the kernels of libnerfloam_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -39,14 +39,14 @@ struct NlPerDevice {
     }
 };
 
-// Number of SMs of the current device (148 on B200); cached.
+// Number of SMs of the current device (132 on H100 SXM); cached.
 static inline int nl_num_sms() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (sms <= 0) sms = 148;
+        if (sms <= 0) sms = 132;
     }
     return sms;
 }

@@ -840,7 +840,7 @@ extern "C" int nl_render_samples(const nl_render_args *a, void *stream_) {
     cudaMemsetAsync(a->d_stats, 0, sizeof(nl_render_stats), stream);
     const int blocks = nl_div_up(R, 128);
     // lanes per ray: 8 (one per child) while the launch is latency-bound -- a tracking / real-size mapping iteration has 2-10 k rays,
-    // far fewer than the GPU holds threads for (B200: 5.99 -> 5.53 ms per 25-iteration scan, 15.8 -> 15.2 ms per 5-frame mapping call);
+    // far fewer than the GPU holds threads for;
     // 4 once the rays alone fill the SMs (83 k rays: 1.575 vs 1.617 ms per step).  NL_TRAVERSE_LANES=4|8 overrides.
     static const int co_lanes_env = [] { const char *e = getenv("NL_TRAVERSE_LANES"); return e ? atoi(e) : 0; }();
     const int co_lanes = (co_lanes_env == 4 || co_lanes_env == 8) ? co_lanes_env : (R <= 32768 ? 8 : 4);

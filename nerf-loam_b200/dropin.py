@@ -1,4 +1,4 @@
-"""Install the B200 kernels behind the reference's own module names, so that the reference's driver
+"""Install the native kernels behind the reference's own module names, so that the reference's driver
 (demo/run.py -> src/nerfloam.py -> src/mapping.py / src/tracking.py) runs on them unmodified apart from
 the one line the reference's README already tells users to edit (mapping.py:19-20, the absolute path of
 the svo library).  See INTEGRATION.md.

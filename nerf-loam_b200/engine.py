@@ -19,7 +19,7 @@ N_SAMPLES_OFFSET = RenderStats.n_samples.offset
 
 
 def mlp_impl(width):
-    """'tc' = tcgen05 3xTF32 tensor-core kernels (width 256), 'simt' = fp32 CUDA-core kernels.  NL_MLP_IMPL overrides."""
+    """'tc' = wgmma 3xTF32 tensor-core kernels (width 256), 'simt' = fp32 CUDA-core kernels.  NL_MLP_IMPL overrides."""
     want = os.environ.get("NL_MLP_IMPL", "tc")
     return "tc" if (want == "tc" and width == 256) else "simt"
 
@@ -52,7 +52,7 @@ def mlp_train(bufs, M_cap, M_dev, feats, sdf, dfeats, want_wgrad, act, s_flag=No
                                         _capi.ptr(dfeats), gp, _capi.ptr(act["buf"]) if want_wgrad else None, _capi.ptr(dsdf_ext),
                                         C.c_void_p(wgrad_stream.cuda_stream) if (want_wgrad and wgrad_stream is not None) else None, st),
                     "nl_mlp_tc_train")
-        _capi.LAUNCHES += 4 if want_wgrad else 1
+        _capi.LAUNCHES += 3 if want_wgrad else 1
     else:
         w = bufs.weights_struct()
         _capi.check(lib.nl_mlp_train(M_cap, M_dev, _capi.ptr(feats), C.byref(w), _capi.ptr(s_flag), _capi.ptr(s_depth), _capi.ptr(s_ray),

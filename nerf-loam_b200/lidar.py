@@ -3,7 +3,7 @@
 
 Parameters live in ordinary nn.Linear modules (`pts_linears.{0,1}`, `sdf_out`), so deepcopy, pickling,
 .cuda(), optimisers and checkpoints behave exactly like the reference module; the arithmetic of
-get_values / forward on CUDA tensors is the fused sm_100a kernel (csrc/mlp.cu) behind an autograd.Function.
+get_values / forward on CUDA tensors is the fused sm_90a kernel (csrc/mlp.cu) behind an autograd.Function.
 Supported: depth=2, skips=[], embedder='none', in_dim=16, width in {32,64,128,256} -- the shape of every
 config the reference ships; anything else raises NotImplementedError at construction.
 """

@@ -1,5 +1,5 @@
 """Drop-in for src/variations/render_helpers.py: render_rays (:190), bundle_adjust_frames (:321),
-track_frame (:428), get_scores (:97) with the reference signatures, running on the fused sm_100a kernel
+track_frame (:428), get_scores (:97) with the reference signatures, running on the fused sm_90a kernel
 chain (engine.SDFEngine) instead of ~60 eager PyTorch ops + 2 CUDA kernels + autograd per iteration.
 
 Behavioural notes (also in DESIGN.md):
@@ -253,7 +253,7 @@ def select_rays_device(dirs_all, gt_all, cos_all, n_select, n_dev=None, seed=Non
 class _few_threads:
     """The reference's host-side ray selection is a handful of small element-wise CPU ops + a top-k over ~10^5 values; on a
     many-core host torch fans each of them out over every core and the fork/join costs far more than the work (measured on the
-    128-CPU B200 box: 11 ms per frame and iteration, vs ~2 ms with 8 threads).  Same arithmetic, same RNG stream."""
+    128-CPU host: 11 ms per frame and iteration, vs ~2 ms with 8 threads).  Same arithmetic, same RNG stream."""
 
     def __init__(self, n=8):
         self.n = n

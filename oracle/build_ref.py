@@ -1,7 +1,7 @@
 """Build the UNMODIFIED reference native extensions into oracle/_ref/ (test infrastructure only).
 
   svo  : /root/reference/third_party/sparse_octree  (C++ TorchScript custom class, CPU)
-  grid : /root/reference/third_party/sparse_voxels  (C++ + CUDA, pybind11), compiled for sm_100a
+  grid : /root/reference/third_party/sparse_voxels  (C++ + CUDA, pybind11), compiled for sm_90a
 
 Sources are compiled where they lie under /root/reference (never copied); outputs go only to
 oracle/_ref/ (git-ignored, but shipped to the GPU box by gpurun).  The reference's own setup.py is
@@ -11,7 +11,7 @@ The one missing dependency (Eigen, used for a 3-int return type) is satisfied by
 The reference's hot-path PYTHON (render_helpers / voxel_helpers / lidar / criterion / se3pose / lidarFrame /
 sample_util, ~1500 lines) is *staged* by stage_src() into oracle/_ref/src/ the same way: a build product in the
 git-ignored oracle/_ref/ (never committed, never imported by the product) that travels to the GPU box with the
-snapshot, so that the B200 tests and bench.py can run the UNMODIFIED reference loop (with grid_ref.so) beside the
+snapshot, so that the GPU tests and bench.py can run the UNMODIFIED reference loop (with grid_ref.so) beside the
 product on the same GPU (oracle/ref_harness.py).
 
 Usage:  python oracle/build_ref.py [svo] [grid] [src]
@@ -36,7 +36,7 @@ def build_svo():
 
 
 def build_grid():
-    os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0a"
+    os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"
     from torch.utils.cpp_extension import load
     src = os.path.join(REF, "third_party", "sparse_voxels", "src")
     bdir = os.path.join(OUT, "grid")

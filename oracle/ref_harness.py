@@ -1,7 +1,7 @@
 """Run the UNMODIFIED reference hot path on the GPU beside the product (test / baseline infrastructure only).
 
 What this loads is the reference itself, staged by oracle/build_ref.py into the git-ignored oracle/_ref/:
-  * oracle/_ref/grid/grid_ref.so  -- third_party/sparse_voxels compiled for sm_100a from the sources where they lie;
+  * oracle/_ref/grid/grid_ref.so  -- third_party/sparse_voxels compiled for sm_90a from the sources where they lie;
   * oracle/_ref/src/...           -- the reference's hot-path Python files, byte for byte (render_helpers.py,
                                      voxel_helpers.py, lidar.py, criterion.py, se3pose.py, lidarFrame.py, sample_util.py).
 Nothing here is imported by the product (nerf-loam_b200/); callers are tests/, and bench.py's baseline legs.

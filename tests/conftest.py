@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -23,7 +23,7 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200 box: pytest -m gpu)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100: pytest -m gpu)")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

@@ -34,6 +34,9 @@ sys.path.insert(0, os.path.join(REF, "src"))
 
 from oracle import kernels as OK  # noqa: E402
 
+sys.path.insert(0, os.path.dirname(HERE))
+from util import save_golden  # noqa: E402
+
 syn = importlib.import_module("nerf-loam_b200.synthetic")
 
 # ---------------------------------------------------------------- substitutions
@@ -279,7 +282,7 @@ def golden_render():
     torch.manual_seed(123)
     out = RH.render_rays(rays_o, rays_d, map_states, dec, step, voxel_size, 0.3, 20, max_distance, chunk_size=-1)
     assert np.array_equal(RECORD["noise"][0], noise)
-    np.savez_compressed(
+    save_golden(
         os.path.join(HERE, "render.npz"), vox=vox, pts=pts, cos=cos, pose=pose, voxel_size=np.float32(voxel_size),
         max_distance=np.float32(max_distance), step=np.float32(step), emb_bf16=bf16_bits(m["emb"]),
         id2emb=m["id2emb"].numpy(), rays_o=rays_o[0].numpy(), rays_d=rays_d[0].numpy(),
@@ -380,7 +383,7 @@ def golden_mapping_tracking():
     for i, nz in enumerate(RECORD["noise"]):
         out[f"track_noise{i}"] = nz
     print("track losses", RECORD["loss"])
-    np.savez_compressed(
+    save_golden(
         os.path.join(HERE, "mapping_tracking.npz"), vox=vox, voxel_size=np.float32(voxel_size),
         max_distance=np.float32(max_distance), emb_bf16=bf16_bits(m["emb"]), id2emb=m["id2emb"].numpy(),
         **{f"scan{i}_pts": s[0] for i, s in enumerate(scans)}, **{f"scan{i}_cos": s[1] for i, s in enumerate(scans)},

@@ -1,36 +1,44 @@
-"""The drop-in boundary, proven with the REFERENCE'S OWN objects on the B200 (SURVEY.md section 8 b-4).
+"""The drop-in boundary against the REFERENCE'S OWN results on the GPU (SURVEY.md section 8 b-4).
 
-On the GPU box oracle/_ref/ holds the compiled, unmodified reference `grid` extension and the reference's hot-path Python
-files, staged byte for byte by oracle/build_ref.py (git-ignored build products, like grid_ref.so).  These tests
-
-  1. run the reference's own bundle_adjust_frames / track_frame (render_helpers.py:321-514: eager PyTorch + grid_ref +
-     autograd + torch.optim.Adam) on the GPU, and
-  2. run the functions `nerfloam_b200.dropin.install()` binds in their place,
-
-both times with objects built from the reference's own classes -- Criterion, LidarFrame, OptimizablePose, Decoder and a
-`map_states` dict in mapping.py's exact format (CPU index tensors, [N,1] int32 voxel_id2embedding_id, duplicate-row bf16 CUDA
-leaf table) -- on identical inputs, seeds and (pinned) sampling noise, and compare the parameters after 3 optimiser steps.
+The reference side of every comparison is what the reference's own bundle_adjust_frames / track_frame / render_rays
+(render_helpers.py:321-514: eager PyTorch + its compiled `grid` extension + autograd + torch.optim.Adam) computed on the GPU
+from these inputs, stored in tests/golden/dropin_reference.*.npz by tests/golden/make_golden_gpu.py.  The drop-in side
+runs the functions `nerfloam_b200.dropin.install()` binds in the reference's place:
+  * where oracle/_ref/ holds the compiled reference and its staged hot-path Python (oracle/build_ref.py), through install()
+    itself and with objects built from the reference's own classes -- Criterion, LidarFrame, OptimizablePose, Decoder;
+  * otherwise with the product's classes of the same names, which follow the same interfaces;
+both times with a `map_states` dict in mapping.py's exact format (CPU index tensors, [N,1] int32 voxel_id2embedding_id,
+duplicate-row bf16 CUDA leaf table), the same seeds and the same initial decoder.
 """
 import copy
 import os
 import sys
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
 import torch
+
+from util import bf16_from_bits, golden
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 VS, MD, TR = 0.3, 40.0, 0.3          # configs/kitti/kitti.yaml
 LR = [0.01, 0.005, 0.001]
+BA_KW = dict(voxel_size=VS, step_size=0.5 * VS, N_rays=1024, num_iterations=3, truncation=TR, max_voxel_hit=20, max_distance=MD,
+             learning_rate=LR, update_pose=True)
+TRACK_KW = dict(voxel_size=VS, N_rays=1024, step_size=0.2 * VS, num_iterations=3, truncation=TR, learning_rate=0.06, max_voxel_hit=20,
+                max_distance=MD, depth_variance=True)
+RENDER_ARGS = (0.5 * VS, VS, TR, 20, MD)
 
 
 @pytest.fixture(scope="module")
 def ref():
+    """The live reference (oracle/_ref), or None where it was not built."""
     from oracle import ref_harness as H
     if not H.available():
-        pytest.skip("oracle/_ref (compiled reference grid + staged reference Python) not present")
+        return None
     assert torch.cuda.is_available()
     return H.load()
 
@@ -41,7 +49,31 @@ def nl():
     return nl
 
 
-def _scene(nl, n_scans=3):
+@pytest.fixture(scope="module")
+def gold():
+    return golden("dropin_reference.npz")
+
+
+def classes(ref, nl):
+    """The classes the drop-in is driven with: the reference's own, or the product's of the same names."""
+    if ref is not None:
+        return ref
+    return SimpleNamespace(Decoder=nl.lidar.Decoder, Criterion=nl.criterion.Criterion, OptimizablePose=nl.se3pose.OptimizablePose,
+                           LidarFrame=nl.frame.LidarFrame)
+
+
+def dropin_helpers(ref, nl):
+    """The module whose render_rays / bundle_adjust_frames / track_frame the caller uses: the reference's render_helpers after
+    dropin.install(), or the product's render_helpers that install() binds there."""
+    if ref is None:
+        return nl.render_helpers
+    import nerfloam_b200.dropin as dropin
+    dropin.install(reference_src=ref.src)
+    assert ref.RH.bundle_adjust_frames is nl.render_helpers.bundle_adjust_frames       # what mapping.py:179 now calls
+    return ref.RH
+
+
+def scene(nl, n_scans=3):
     syn = nl.synthetic
     scans = [syn.make_scan(n_beams=32, n_az=600, seed=100 + i, sensor_xyz=(1.0 * i, 0.1 * i, 0.0), yaw=0.02 * i) for i in range(n_scans)]
     o = nl.svo.Octree()
@@ -51,34 +83,68 @@ def _scene(nl, n_scans=3):
     return scans, o.get_centres_and_children()
 
 
-def _ref_frames(ref, scans, perturb=True):
-    """The reference's LidarFrame / OptimizablePose objects (lidarFrame.py:10-25 with new_keyframe=True adopts the pose object).
+def make_frames(cls, scans, perturb=True):
+    """LidarFrame / OptimizablePose objects (lidarFrame.py:10-25 with new_keyframe=True adopts the pose object).
     The scan tensors are handed over device-resident: the reference indexes `frame.rays_d` (wherever the points live) with a CUDA
     mask (render_helpers.py:371-372), which torch 1.10 accepted for CPU tensors and torch >= 2 rejects -- with CUDA points the
     unmodified reference runs on this torch, and its per-iteration `.cuda()` uploads become no-ops (in its favour)."""
     frames = []
     g = torch.Generator().manual_seed(5)
     for i, (pts, cos, pose) in enumerate(scans):
-        p6 = ref.OptimizablePose.from_matrix(torch.from_numpy(pose.copy())).data.detach().clone()
+        p6 = cls.OptimizablePose.from_matrix(torch.from_numpy(pose.copy())).data.detach().clone()
         if perturb and i > 0:
             p6 = p6 + torch.cat([torch.randn(3, generator=g) * 0.02, torch.randn(3, generator=g) * 0.002])
-        frames.append(ref.LidarFrame(i, torch.from_numpy(pts).cuda(), torch.from_numpy(cos).cuda(), ref.OptimizablePose(p6.float()), new_keyframe=True))
+        frames.append(cls.LidarFrame(i, torch.from_numpy(pts).cuda(), torch.from_numpy(cos).cuda(), cls.OptimizablePose(p6.float()), new_keyframe=True))
     return frames
 
 
-def _state(ref, nl, table_rows=None):
+def state(cls, nl, table_rows=None, dec0=None):
+    """Scans, map_states and the initial decoder (dec0: a state dict to start from instead of the seeded initialisation)."""
     from oracle import ref_harness as H
-    scans, (voxels, children, features) = _scene(nl)
+    scans, (voxels, children, features) = scene(nl)
     ms = H.reference_map_states(voxels, children, features, VS, table_rows=table_rows, init_std=0.01, seed=3)
     torch.manual_seed(777)
-    dec = ref.Decoder(depth=2, width=256, in_dim=16, skips=[], embedder="none", multires=0).cuda()
+    dec = cls.Decoder(depth=2, width=256, in_dim=16, skips=[], embedder="none", multires=0).cuda()
+    if dec0 is not None:
+        dec.load_state_dict(dec0)
     return scans, ms, dec
 
 
-def _clone_ms(ms):
+def vertex_emb(ms):
+    """The embedding of every vertex the map references, in vertex-id order, as float32 on the host.  The table has one row per
+    *reference* to a vertex (duplicates included) and which duplicate the id table keeps is decided by a racy index_put_
+    (SURVEY.md A.1), so two builds of the same map agree per vertex, not per row."""
+    vidx = ms["voxel_vertex_idx"]
+    v = torch.unique(vidx[vidx >= 0].long())
+    rows = ms["voxel_id2embedding_id"].reshape(-1)[v].long()
+    emb = ms["voxel_vertex_emb"].detach()
+    return emb[rows.to(emb.device)].float().cpu()
+
+
+def clone_ms(ms):
     out = dict(ms)
     out["voxel_vertex_emb"] = ms["voxel_vertex_emb"].detach().clone().requires_grad_()
     return out
+
+
+def track_input(cls, scans):
+    f = make_frames(cls, scans)[1]
+    f.index = 5                                            # lr/3 branch of render_helpers.py:448-450
+    return f
+
+
+def render_input(scans):
+    pts, cos, pose = scans[0]
+    sel = np.sort(np.random.default_rng(0).choice(pts.shape[0], 2048, replace=False))
+    P, Cn = torch.from_numpy(pts[sel]).cuda(), torch.from_numpy(cos[sel]).cuda()
+    T = torch.from_numpy(pose).cuda()
+    rd = ((P / (P.norm(dim=-1, keepdim=True) + 1e-8)) @ T[:3, :3].T)[None].contiguous()
+    ro = T[:3, 3].reshape(1, 1, 3).expand_as(rd).contiguous()
+    return ro, rd, P, Cn
+
+
+def _dec0(gold):
+    return {k[len("dec0_"):]: torch.from_numpy(gold[k]) for k in gold.files if k.startswith("dec0_")}
 
 
 def _rel(a, b):
@@ -87,33 +153,29 @@ def _rel(a, b):
 
 
 @pytest.mark.parametrize("update_decoder", [True, False])
-def test_bundle_adjust_frames_reference_objects_through_dropin(ref, nl, update_decoder):
+def test_bundle_adjust_frames_reference_objects_through_dropin(ref, nl, gold, update_decoder):
     from oracle import ref_harness as H
-    scans, ms0, dec0 = _state(ref, nl, table_rows=4_000_000)
-    crit = ref.Criterion(H.args(MD, TR))
-    kw = dict(voxel_size=VS, step_size=0.5 * VS, N_rays=1024, num_iterations=3, truncation=TR, max_voxel_hit=20, max_distance=MD,
-              learning_rate=LR, update_pose=True, update_decoder=update_decoder)
+    cls = classes(ref, nl)
+    scans, ms0, dec0 = state(cls, nl, table_rows=4_000_000, dec0=_dec0(gold))
+    crit = cls.Criterion(H.args(MD, TR))
+    tag = f"ba{int(update_decoder)}_"
 
-    # ---- (1) the reference's own loop on the GPU ----
-    ms_r, dec_r, fr_r = _clone_ms(ms0), copy.deepcopy(dec0), _ref_frames(ref, scans)
-    torch.manual_seed(11)
-    with H.pinned(ref):
-        ref.orig["bundle_adjust_frames"](fr_r, ms_r["voxel_vertex_emb"], ms_r, dec_r, crit, **kw)
-    torch.cuda.synchronize()
+    # ---- (1) the reference's own loop on the GPU (stored) ----
+    p_r = torch.from_numpy(gold[tag + "poses"])
+    e_r = bf16_from_bits(gold[tag + "emb_bf16"]).float()             # per vertex (vertex_emb)
+    dec_r = {k[len(tag + "dec_"):]: torch.from_numpy(gold[k]) for k in gold.files if k.startswith(tag + "dec_")} if update_decoder else dec0.state_dict()
 
-    # ---- (2) the same call through dropin.install(), same reference objects ----
-    import nerfloam_b200.dropin as dropin
-    dropin.install(reference_src=ref.src)
-    assert ref.RH.bundle_adjust_frames is nl.render_helpers.bundle_adjust_frames       # what mapping.py:179 now calls
-    ms_p, dec_p, fr_p = _clone_ms(ms0), copy.deepcopy(dec0), _ref_frames(ref, scans)
+    # ---- (2) the same call through the drop-in ----
+    rh = dropin_helpers(ref, nl)
+    ms_p, dec_p, fr_p = clone_ms(ms0), copy.deepcopy(dec0), make_frames(cls, scans)
     torch.manual_seed(11)
-    ref.RH.bundle_adjust_frames(fr_p, ms_p["voxel_vertex_emb"], ms_p, dec_p, crit, deterministic=True, ray_selection="host", **kw)
+    rh.bundle_adjust_frames(fr_p, ms_p["voxel_vertex_emb"], ms_p, dec_p, crit, deterministic=True, ray_selection="host",
+                            update_decoder=update_decoder, **BA_KW)
     torch.cuda.synchronize()
 
     # poses: frame 0 frozen, the others moved and agree
-    p_r = torch.stack([f.pose.data.detach().cpu() for f in fr_r])
     p_p = torch.stack([f.pose.data.detach().cpu() for f in fr_p])
-    p_0 = torch.stack([f.pose.data.detach().cpu() for f in _ref_frames(ref, scans)])
+    p_0 = torch.stack([f.pose.data.detach().cpu() for f in make_frames(cls, scans)])
     assert torch.equal(p_p[0], p_0[0]) and torch.equal(p_r[0], p_0[0])
     assert float((p_r[1:] - p_0[1:]).abs().max()) > 1e-3
     # 3 Adam steps of lr 1e-3: the first step moves every coordinate by exactly +-lr, so agreement to a small fraction of lr
@@ -123,16 +185,17 @@ def test_bundle_adjust_frames_reference_objects_through_dropin(ref, nl, update_d
     # zero (its sign is rounding noise on BOTH sides) may legitimately differ by a fraction of lr: all but a sliver agree to 2e-4
     # (4 % of one step), none by more than a step
     lr_dec = LR[1]
-    for (k, a), (_, b) in zip(dec_p.state_dict().items(), dec_r.state_dict().items()):
+    for k, a in dec_p.state_dict().items():
+        b = dec_r[k].to(a.device)
         if update_decoder:
             assert float((b - dec0.state_dict()[k]).abs().max()) > 1e-3
             d = (a - b).abs()
             assert float((d > 2e-4).float().mean()) < 5e-3 and float(d.max()) < lr_dec, (k, float((d > 2e-4).float().mean()), float(d.max()))
         else:
             assert torch.equal(a, dec0.state_dict()[k]) and torch.equal(b, dec0.state_dict()[k])
-    # embeddings (bf16, same row numbering: both sides use the reference's table).  The update as a whole agrees (norm-wise), the
-    # same entries moved, and only a sliver of entries differs by more than a fifth of one Adam step
-    e_r, e_p, e_0 = (t["voxel_vertex_emb"].detach().float().cpu() for t in (ms_r, ms_p, ms0))
+    # embeddings (bf16, per vertex).  The update as a whole agrees (norm-wise), the same entries moved, and only a sliver of
+    # entries differs by more than a fifth of one Adam step
+    e_p, e_0 = vertex_emb(ms_p), vertex_emb(ms0)
     u_r, u_p = e_r - e_0, e_p - e_0
     moved_r, moved_p = u_r.abs() > 1e-3, u_p.abs() > 1e-3
     stats = dict(moved_ref=float(moved_r.float().mean()), moved_ours=float(moved_p.float().mean()),
@@ -146,7 +209,7 @@ def test_bundle_adjust_frames_reference_objects_through_dropin(ref, nl, update_d
 
 
 @pytest.mark.parametrize("impl", ["simt", "tc"])
-def test_track_frame_reference_objects_through_dropin(ref, nl, impl, monkeypatch):
+def test_track_frame_reference_objects_through_dropin(ref, nl, gold, impl, monkeypatch):
     """Three tracking iterations, reference vs drop-in.  The pose gradient of a nearly converged pose is a sum of ~2e4 per-sample
     terms that cancel to ~1e-4 of their absolute sum, so it amplifies every rounding difference by ~1e4:
       * with the fp32 CUDA-core decoder (NL_MLP_IMPL=simt) the drop-in reproduces the reference's poses to 2e-5 -- the fused
@@ -157,28 +220,16 @@ def test_track_frame_reference_objects_through_dropin(ref, nl, impl, monkeypatch
         cancellation) meet 1e-4 with the same kernels (test_single_iteration_gradients_vs_oracle_autograd)."""
     from oracle import ref_harness as H
     monkeypatch.setenv("NL_MLP_IMPL", impl)
-    scans, ms0, dec0 = _state(ref, nl)
-    crit = ref.Criterion(H.args(MD, TR))
-    kw = dict(voxel_size=VS, N_rays=1024, step_size=0.2 * VS, num_iterations=3, truncation=TR, learning_rate=0.06, max_voxel_hit=20,
-              max_distance=MD, depth_variance=True)
+    cls = classes(ref, nl)
+    scans, ms0, dec0 = state(cls, nl, dec0=_dec0(gold))
+    crit = cls.Criterion(H.args(MD, TR))
+    pose_in = track_input(cls, scans).pose
+    pose_r, hit_r = SimpleNamespace(data=torch.from_numpy(gold["track_pose"])), torch.from_numpy(gold["track_hit"])
 
-    def frame():
-        f = _ref_frames(ref, scans)[1]
-        f.index = 5                                            # lr/3 branch of render_helpers.py:448-450
-        return f
-
-    f_r = frame()
-    pose_in = copy.deepcopy(f_r.pose)
+    rh = dropin_helpers(ref, nl)
+    f_p = track_input(cls, scans)
     torch.manual_seed(21)
-    with H.pinned(ref):
-        pose_r, hit_r = ref.orig["track_frame"](pose_in, f_r, _clone_ms(ms0), copy.deepcopy(dec0), crit, **kw)
-    torch.cuda.synchronize()
-
-    import nerfloam_b200.dropin as dropin
-    dropin.install(reference_src=ref.src)
-    f_p = frame()
-    torch.manual_seed(21)
-    pose_p, hit_p = ref.RH.track_frame(copy.deepcopy(f_p.pose), f_p, _clone_ms(ms0), copy.deepcopy(dec0), crit, deterministic=True, ray_selection="host", **kw)
+    pose_p, hit_p = rh.track_frame(copy.deepcopy(f_p.pose), f_p, clone_ms(ms0), copy.deepcopy(dec0), crit, deterministic=True, ray_selection="host", **TRACK_KW)
     assert type(pose_p).__name__ == "OptimizablePose" and pose_p.data.is_cuda
     assert hit_p is not None and hit_r is not None
     assert torch.equal(hit_p.cpu(), hit_r.cpu())
@@ -191,26 +242,18 @@ def test_track_frame_reference_objects_through_dropin(ref, nl, impl, monkeypatch
     assert float(d[:3].max()) < 1e-3
 
 
-def test_render_rays_and_criterion_reference_objects(ref, nl):
-    """render_rays through the drop-in feeding the REFERENCE'S Criterion.forward + autograd: same loss, same ray mask and
-    sample layout as the reference's own render_rays."""
+def test_render_rays_and_criterion_reference_objects(ref, nl, gold):
+    """render_rays through the drop-in feeding Criterion.forward + autograd: same loss, same ray mask and sample layout as the
+    reference's own render_rays."""
     from oracle import ref_harness as H
-    scans, ms0, dec0 = _state(ref, nl)
-    crit = ref.Criterion(H.args(MD, TR))
-    pts, cos, pose = scans[0]
-    sel = np.sort(np.random.default_rng(0).choice(pts.shape[0], 2048, replace=False))
-    P, Cn = torch.from_numpy(pts[sel]).cuda(), torch.from_numpy(cos[sel]).cuda()
-    T = torch.from_numpy(pose).cuda()
-    rd = ((P / (P.norm(dim=-1, keepdim=True) + 1e-8)) @ T[:3, :3].T)[None].contiguous()
-    ro = T[:3, 3].reshape(1, 1, 3).expand_as(rd).contiguous()
-    args = (0.5 * VS, VS, TR, 20, MD)
-    with H.pinned(ref):
-        out_r = ref.orig["render_rays"](ro, rd, _clone_ms(ms0), copy.deepcopy(dec0), *args, chunk_size=-1)
-        loss_r, _ = crit(out_r, P[None], Cn[None, :, None])
-    out_p = nl.render_helpers.render_rays(ro, rd, _clone_ms(ms0), copy.deepcopy(dec0), *args, chunk_size=-1, deterministic=True)
+    cls = classes(ref, nl)
+    scans, ms0, dec0 = state(cls, nl, dec0=_dec0(gold))
+    crit = cls.Criterion(H.args(MD, TR))
+    ro, rd, P, Cn = render_input(scans)
+    out_p = nl.render_helpers.render_rays(ro, rd, clone_ms(ms0), copy.deepcopy(dec0), *RENDER_ARGS, chunk_size=-1, deterministic=True)
     loss_p, _ = crit(out_p, P[None], Cn[None, :, None])
-    assert torch.equal(out_p["ray_mask"].view(-1), out_r["ray_mask"].view(-1))
-    assert torch.equal(out_p["valid_mask"], out_r["valid_mask"])
-    np.testing.assert_allclose(out_p["z_vals"].cpu().numpy(), out_r["z_vals"].cpu().numpy(), rtol=2e-6)
-    np.testing.assert_allclose(out_p["sdf"].detach().cpu().numpy(), out_r["sdf"].detach().cpu().numpy(), atol=1e-5)
-    np.testing.assert_allclose(float(loss_p), float(loss_r), rtol=1e-5)
+    assert np.array_equal(out_p["ray_mask"].view(-1).cpu().numpy(), gold["render_ray_mask"])
+    assert np.array_equal(out_p["valid_mask"].cpu().numpy(), gold["render_valid_mask"])
+    np.testing.assert_allclose(out_p["z_vals"].cpu().numpy(), gold["render_z_vals"], rtol=2e-6)
+    np.testing.assert_allclose(out_p["sdf"].detach().cpu().numpy(), gold["render_sdf"], atol=1e-5)
+    np.testing.assert_allclose(float(loss_p), float(gold["render_loss"]), rtol=1e-5)

@@ -1,5 +1,6 @@
 """GPU parity tests of the individual C-ABI ops against the oracle, the golden vectors produced by the
-executed reference, and (when oracle/_ref/grid was built) the compiled unmodified reference kernels."""
+executed reference, and the outputs of the compiled unmodified reference kernels on the same inputs (stored in
+tests/golden/reference_grid.*.npz by tests/golden/make_golden_gpu.py)."""
 import ctypes as C
 import os
 
@@ -7,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import bf16_from_bits, golden, product_map, ref_grid, load_decoder
+from util import bf16_from_bits, golden, product_map, load_decoder
 
 pytestmark = pytest.mark.gpu
 
@@ -26,43 +27,31 @@ def scene(nl):
     return z, m
 
 
-def canon_ties(idx, mn, mx):
-    """Order hits with bit-identical min_depth canonically (the tie order is unspecified in the reference)."""
-    key = np.lexsort((idx, mn), axis=-1) if False else None
-    out_i, out_a, out_b = idx.copy(), mn.copy(), mx.copy()
-    for r in range(idx.shape[0]):
-        o = np.lexsort((idx[r], mn[r]))
-        out_i[r], out_a[r], out_b[r] = idx[r][o], mn[r][o], mx[r][o]
-    return out_i, out_a, out_b
+@pytest.fixture(scope="module")
+def ref_grid_out():
+    """What the reference's compiled `grid` kernels returned for the inputs below (svo_*: svo_intersect on all rays of
+    render.npz; svo4_*: the same rays batched 4 ways like its wrapper does; icdf_*: inverse_cdf_sampling on icdf_args())."""
+    return golden("reference_grid.npz")
 
 
-def test_svo_intersect_vs_oracle_and_reference(nl, scene):
-    from oracle import kernels as OK
-    z, m = scene
-    vs = float(z["voxel_size"])
+def scene_rays(z, m):
     ro = torch.from_numpy(z["rays_o"]).cuda()[None].contiguous()
     rd = torch.from_numpy(z["rays_d"]).cuda()[None].contiguous()
-    pts = m["centres"].cuda()[None].contiguous()
-    ch = m["structure"].cuda()[None].contiguous()
-    idx, mn, mx = nl.grid.svo_intersect(ro, rd, pts, ch, vs, 20)
-    oi, omn, omx = OK.svo_intersect(z["rays_o"], z["rays_d"], m["centres"].numpy(), m["structure"].numpy(), vs, 20)
-    assert np.array_equal(idx[0].cpu().numpy(), oi)                     # voxel ids: bit-exact, DFS order
-    np.testing.assert_allclose(mn[0].cpu().numpy(), omn, rtol=2e-6, atol=1e-6)   # __fdividef vs 1.0f/x
-    np.testing.assert_allclose(mx[0].cpu().numpy(), omx, rtol=2e-6, atol=1e-6)
-    g = ref_grid()
-    if g is not None:                                                   # the real reference kernel, same GPU
-        G = 4                                                           # its wrapper batches rays and replicates the octree
-        K = ro.shape[1] // G
-        rs = ro[:, :G * K].reshape(G, K, 3).contiguous()
-        rdd = rd[:, :G * K].reshape(G, K, 3).contiguous()
-        ri, rmn, rmx = g.svo_intersect(rs, rdd, pts.expand(G, -1, -1).contiguous(), ch.expand(G, -1, -1).contiguous(), vs, 20)
-        mi, mmn, mmx = nl.grid.svo_intersect(rs, rdd, pts.expand(G, -1, -1).contiguous(), ch.expand(G, -1, -1).contiguous(), vs, 20)
-        assert torch.equal(ri, mi) and torch.equal(rmn, mmn) and torch.equal(rmx, mmx)   # bit-exact incl. depths
+    return ro, rd, m["centres"].cuda()[None].contiguous(), m["structure"].cuda()[None].contiguous()
 
 
-def test_inverse_cdf_sampling_vs_oracle_and_reference(nl, scene):
+def batched4(ro, rd, pts, ch):
+    """The rays split into 4 batches of equal size, the octree replicated per batch (the reference wrapper's layout)."""
+    G = 4
+    K = ro.shape[1] // G
+    rs = ro[:, :G * K].reshape(G, K, 3).contiguous()
+    rdd = rd[:, :G * K].reshape(G, K, 3).contiguous()
+    return rs, rdd, pts.expand(G, -1, -1).contiguous(), ch.expand(G, -1, -1).contiguous()
+
+
+def icdf_args(z):
+    """inverse_cdf_sampling inputs built from the hits of render.npz, padded to 200 batches, seeded noise."""
     from oracle import kernels as OK
-    z, m = scene
     hits = z["hits"]
     P = z["hit_idx"].shape[1]
     idx = z["hit_idx"][hits]; mn = z["hit_min"][hits]; mx = z["hit_max"][hits]
@@ -80,34 +69,62 @@ def test_inverse_cdf_sampling_vs_oracle_and_reference(nl, scene):
     noise = rng.uniform(0.001, 0.999, size=(Gb, H // Gb, S)).astype(np.float32)
     shp = (Gb, H // Gb, P)
     t = lambda a, s: torch.from_numpy(np.ascontiguousarray(a.reshape(s))).cuda()
-    args = (t(I, shp), t(A, shp), t(B, shp), torch.from_numpy(noise).cuda(), t(PR, shp), t(ST, (Gb, H // Gb)))
-    si, sd, sl = nl.grid.inverse_cdf_sampling(*args, -1.0)
-    oi = np.empty((Gb, H // Gb, S), np.int32); od = np.empty_like(oi, dtype=np.float32); ol = np.empty_like(od)
-    a = [np.ascontiguousarray(x.cpu().numpy()) for x in args]
-    OK.lib().nlo_inverse_cdf_sampling(Gb, H // Gb, P, S, -1.0, OK._p(a[0]), OK._p(a[1]), OK._p(a[2]), OK._p(a[3]), OK._p(a[4]),
-                                      OK._p(a[5]), OK._p(oi), OK._p(od), OK._p(ol))
-    assert np.array_equal(si.cpu().numpy(), oi)
-    assert np.array_equal(sd.cpu().numpy(), od) and np.array_equal(sl.cpu().numpy(), ol)   # same fp ops incl. the FMA
-    g = ref_grid()
-    if g is not None:
-        ri, rd_, rl = g.inverse_cdf_sampling(*args, -1.0)
-        assert torch.equal(ri, si) and torch.equal(rd_, sd) and torch.equal(rl, sl)
+    return (t(I, shp), t(A, shp), t(B, shp), torch.from_numpy(noise).cuda(), t(PR, shp), t(ST, (Gb, H // Gb)))
 
 
-def test_reference_grid_pins_the_oracle(nl, scene):
-    """The oracle's C restatement of the two CUDA kernels against the compiled reference itself."""
-    g = ref_grid()
-    if g is None:
-        pytest.skip("oracle/_ref/grid not built")
+def canon_ties(idx, mn, mx):
+    """Order hits with bit-identical min_depth canonically (the tie order is unspecified in the reference)."""
+    key = np.lexsort((idx, mn), axis=-1) if False else None
+    out_i, out_a, out_b = idx.copy(), mn.copy(), mx.copy()
+    for r in range(idx.shape[0]):
+        o = np.lexsort((idx[r], mn[r]))
+        out_i[r], out_a[r], out_b[r] = idx[r][o], mn[r][o], mx[r][o]
+    return out_i, out_a, out_b
+
+
+def test_svo_intersect_vs_oracle_and_reference(nl, scene, ref_grid_out):
     from oracle import kernels as OK
     z, m = scene
     vs = float(z["voxel_size"])
-    ro = torch.from_numpy(z["rays_o"]).cuda()[None].contiguous()
-    rd = torch.from_numpy(z["rays_d"]).cuda()[None].contiguous()
-    ri, rmn, rmx = g.svo_intersect(ro, rd, m["centres"].cuda()[None].contiguous(), m["structure"].cuda()[None].contiguous(), vs, 20)
+    ro, rd, pts, ch = scene_rays(z, m)
+    idx, mn, mx = nl.grid.svo_intersect(ro, rd, pts, ch, vs, 20)
     oi, omn, omx = OK.svo_intersect(z["rays_o"], z["rays_d"], m["centres"].numpy(), m["structure"].numpy(), vs, 20)
-    assert np.array_equal(ri[0].cpu().numpy(), oi)
-    np.testing.assert_allclose(rmn[0].cpu().numpy(), omn, rtol=2e-6, atol=1e-6)
+    assert np.array_equal(idx[0].cpu().numpy(), oi)                     # voxel ids: bit-exact, DFS order
+    np.testing.assert_allclose(mn[0].cpu().numpy(), omn, rtol=2e-6, atol=1e-6)   # __fdividef vs 1.0f/x
+    np.testing.assert_allclose(mx[0].cpu().numpy(), omx, rtol=2e-6, atol=1e-6)
+    # the real reference kernel; its wrapper batches rays and replicates the octree
+    mi, mmn, mmx = nl.grid.svo_intersect(*batched4(ro, rd, pts, ch), vs, 20)
+    r = ref_grid_out
+    assert np.array_equal(r["svo4_idx"], mi.cpu().numpy()) and np.array_equal(r["svo4_min"], mmn.cpu().numpy()) \
+        and np.array_equal(r["svo4_max"], mmx.cpu().numpy())   # bit-exact incl. depths
+
+
+def test_inverse_cdf_sampling_vs_oracle_and_reference(nl, scene, ref_grid_out):
+    from oracle import kernels as OK
+    z, m = scene
+    args = icdf_args(z)
+    Gb, Hg, P = args[0].shape
+    S = args[3].shape[-1]
+    si, sd, sl = nl.grid.inverse_cdf_sampling(*args, -1.0)
+    oi = np.empty((Gb, Hg, S), np.int32); od = np.empty_like(oi, dtype=np.float32); ol = np.empty_like(od)
+    a = [np.ascontiguousarray(x.cpu().numpy()) for x in args]
+    OK.lib().nlo_inverse_cdf_sampling(Gb, Hg, P, S, -1.0, OK._p(a[0]), OK._p(a[1]), OK._p(a[2]), OK._p(a[3]), OK._p(a[4]),
+                                      OK._p(a[5]), OK._p(oi), OK._p(od), OK._p(ol))
+    assert np.array_equal(si.cpu().numpy(), oi)
+    assert np.array_equal(sd.cpu().numpy(), od) and np.array_equal(sl.cpu().numpy(), ol)   # same fp ops incl. the FMA
+    r = ref_grid_out
+    assert np.array_equal(r["icdf_idx"], si.cpu().numpy()) and np.array_equal(r["icdf_depth"], sd.cpu().numpy()) \
+        and np.array_equal(r["icdf_dist"], sl.cpu().numpy())
+
+
+def test_reference_grid_pins_the_oracle(nl, scene, ref_grid_out):
+    """The oracle's C restatement of the two CUDA kernels against the compiled reference itself."""
+    from oracle import kernels as OK
+    z, m = scene
+    vs = float(z["voxel_size"])
+    oi, omn, omx = OK.svo_intersect(z["rays_o"], z["rays_d"], m["centres"].numpy(), m["structure"].numpy(), vs, 20)
+    assert np.array_equal(ref_grid_out["svo_idx"][0], oi)
+    np.testing.assert_allclose(ref_grid_out["svo_min"][0], omn, rtol=2e-6, atol=1e-6)
 
 
 @pytest.mark.parametrize("width", [256, 32])

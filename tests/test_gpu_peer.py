@@ -2,7 +2,7 @@
 symmetric-memory statistics exchange (dist.PeerStats) in a 1-rank process group: the kernels then read / write their "peers"
 through the same pointer tables and must reproduce nl_adam_bf16_ctl and nl_stats_unpack exactly.  The W > 1 behaviour (NVLS
 multicast, bit-identity with NCCL all-reduce + Adam, identical replicas) is checked by scripts/test_peer.py under torchrun
-(2 x B200: profiles/r02_peer_2gpu.txt) and by bench.py's strong-scaling block on every multi-GPU run."""
+and by bench.py's strong-scaling block on every multi-GPU run."""
 import os
 import socket
 

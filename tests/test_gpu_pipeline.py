@@ -373,13 +373,13 @@ def test_single_iteration_gradients_vs_oracle_autograd(nl):
 
 
 def test_tensor_core_mlp_forward_matches_fp32_kernel(nl):
-    """tcgen05 3xTF32 decoder forward vs the fp32 CUDA-core kernel (same inputs): SDF within 1e-5 (north-star bar)."""
+    """wgmma 3xTF32 decoder forward vs the fp32 CUDA-core kernel (same inputs): SDF within 1e-5 (north-star bar)."""
     from nerfloam_b200 import engine as E
     z = golden("render.npz")
     dec = load_decoder(z, "dec_")
     dev = torch.device("cuda")
     torch.manual_seed(3)
-    for M in (1, 77, 128, 129, 5000, 148 * 128 * 2 + 37):
+    for M in (1, 77, 128, 129, 5000, 132 * 128 * 2 + 37):
         x = (torch.randn(M, 16, device=dev) * 0.05).contiguous()
         out = {}
         for impl in ("simt", "tc"):
@@ -405,14 +405,14 @@ def test_tensor_core_mlp_forward_matches_fp32_kernel(nl):
 
 @pytest.mark.parametrize("wgrad", [False, True])
 def test_tensor_core_mlp_train_matches_fp32_kernel(nl, wgrad):
-    """tcgen05 3xTF32 fused forward+backward vs the fp32 CUDA-core kernel on identical inputs (external d sdf):
+    """wgmma 3xTF32 fused forward+backward vs the fp32 CUDA-core kernel on identical inputs (external d sdf):
     sdf, d feats and every decoder gradient."""
     z = golden("render.npz")
     dec = load_decoder(z, "dec_")
     dev = torch.device("cuda")
     from nerfloam_b200 import engine as E
     torch.manual_seed(11)
-    for M in (300, 148 * 128 + 77):
+    for M in (300, 132 * 128 + 77):
         x = (torch.randn(M, 16, device=dev) * 0.05).contiguous()
         g = (torch.randn(M, device=dev) * 0.1).contiguous()
         res = {}

@@ -8,6 +8,7 @@ import torch
 
 from oracle import chain as C
 from oracle import kernels as K
+from util import golden
 
 G = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -111,7 +112,7 @@ def test_criterion():
 def test_ray_intersect_and_sample_wrappers():
     """numpy restatement of voxel_helpers.ray_intersect / ray_sample / InverseCDFRaySampling vs the
     reference's own Python wrappers run over the same kernel restatement."""
-    z = np.load(os.path.join(G, "render.npz"))
+    z = golden("render.npz")
     vs, md, step = float(z["voxel_size"]), float(z["max_distance"]), float(z["step"])
     m = build_oracle_map(z["vox"], vs, z["id2emb"])
     inter, hits = K.ray_intersect(z["rays_o"], z["rays_d"], m["centres"], m["structure"], vs, 20, md)
@@ -131,7 +132,7 @@ def test_ray_intersect_and_sample_wrappers():
 
 
 def test_render_rays_vs_reference():
-    z = np.load(os.path.join(G, "render.npz"))
+    z = golden("render.npz")
     vs, md, step = float(z["voxel_size"]), float(z["max_distance"]), float(z["step"])
     m = build_oracle_map(z["vox"], vs, z["id2emb"])
     dec = C.Decoder(depth=2, width=256, in_dim=16)
@@ -144,7 +145,7 @@ def test_render_rays_vs_reference():
 
 
 def _load_mt():
-    return np.load(os.path.join(G, "mapping_tracking.npz"))
+    return golden("mapping_tracking.npz")
 
 
 @pytest.mark.parametrize("name,upd_dec", [("map", True), ("mapfrozen", False)])

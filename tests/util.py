@@ -11,8 +11,63 @@ if ROOT not in sys.path:
 G = os.path.join(ROOT, "tests", "golden")
 
 
+PART_BYTES = 900_000
+
+
+def save_golden(path, **arrays):
+    """np.savez_compressed, split into parts <stem>.<i>.npz of at most PART_BYTES of raw array bytes each, so that every stored
+    file stays under 1 MB (golden() merges them).  A larger array is stored as row chunks <key>@<j>."""
+    stem = path[:-len(".npz")]
+    chunks = {}
+    for k, v in arrays.items():
+        v = np.asarray(v)
+        if v.nbytes <= PART_BYTES:
+            chunks[k] = v
+            continue
+        rows = max(1, PART_BYTES // (v.nbytes // v.shape[0]))
+        for j in range(0, v.shape[0], rows):
+            chunks[f"{k}@{j // rows}"] = v[j:j + rows]
+    parts, cur, size = [], {}, 0
+    for k, v in chunks.items():
+        if cur and size + v.nbytes > PART_BYTES:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = v
+        size += v.nbytes
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(f"{stem}.{i}.npz", **part)
+
+
 def golden(name):
-    return np.load(os.path.join(G, name))
+    """tests/golden/<name>; an archive above 1 MB is stored as parts <stem>.<i>.npz (save_golden), merged here."""
+    p = os.path.join(G, name)
+    if os.path.exists(p):
+        return np.load(p)
+    stem = name[:-len(".npz")]
+    parts = sorted(f for f in os.listdir(G) if f.startswith(stem + ".") and f[len(stem) + 1:-len(".npz")].isdigit())
+    if not parts:
+        raise FileNotFoundError(p)
+    out, chunks = _Archive(), {}
+    for f in parts:
+        with np.load(os.path.join(G, f)) as z:
+            for k in z.files:
+                if "@" in k:
+                    name, j = k.rsplit("@", 1)
+                    chunks.setdefault(name, {})[int(j)] = z[k]
+                else:
+                    out[k] = z[k]
+    for name, c in chunks.items():
+        out[name] = np.concatenate([c[j] for j in range(len(c))])
+    return out
+
+
+class _Archive(dict):
+    """The merged parts of a split archive, with np.load's `files`."""
+
+    @property
+    def files(self):
+        return list(self)
 
 
 def bf16_from_bits(a):
