@@ -238,7 +238,7 @@ NL_API int nl_mlp_tc_forward(int64_t M, const int32_t *d_M_dev, const float *d_f
  * The panels must have been prepared from the same W0 / W1 / w2 (the backward panels hold diag(w2) W1).
  * wgrad_stream (may be NULL = stream): the weight-gradient kernels are enqueued there, ordered after the forward/backward
  * kernel by an event, so that they overlap with later work on `stream`; the caller joins the two streams before it reads
- * `grads` or reuses d_act. */
+ * `grads`, reuses d_act or changes d_W1 / d_b1 / d_w2 (the weight-gradient kernels read them). */
 NL_API int64_t nl_mlp_tc_act_floats(int64_t M);
 NL_API int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *d_feats, const void *d_panels, const float *d_W1,
                     const float *d_b0, const float *d_b1, const float *d_w2, const float *d_b2, const uint8_t *d_s_flag, const float *d_s_depth,

@@ -14,10 +14,13 @@
 // Per 128-sample training tile the ring carries 42 items: layer 1 (2 halves), layer 2 (2 halves x 8 K-blocks of 32),
 // backward layer 2 (2 x 8) and backward layer 1 (8 K-blocks, N = 16).
 //
-// Decoder weight gradients (nl_mlp_tc_train with grads): the training kernel stores h1, h2, dh2, dh1 [cap][256] and
-// d loss / d sdf; gW1 = dh2^T h1 (K = samples) is a split-K 3xTF32 tensor-core GEMM (k_dw1_tc, mma.sync m16n8k8: both
-// operands are sample-major, which wgmma's tf32 forms cannot read), the column sums and gW0 (K = 16) come from one
-// streaming pass (k_wg_cols).
+// Decoder weight gradients (nl_mlp_tc_train with grads): the training kernel stores h1, dh1 [cap][256], the relu'(h2) bits
+// (32 B per sample) and d loss / d sdf.  The output layer has one unit, so dh2 = dsdf * w2 * m2 (m2 = relu'(h2)) and everything
+// that would read h2 or dh2 follows from G = m2^T (dsdf * h1) and c = m2^T dsdf:
+//   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c
+// G (K = samples) is a split-K 2-term TF32 tensor-core GEMM whose A operand is the exact 0/1 mask (k_dw1_tc, mma.sync
+// m16n8k8: both operands are sample-major, which wgmma's tf32 forms cannot read); every CTA scales and contracts its partial G
+// before its atomics.  c, gb0, gb2 and gW0 = dh1^T x (K = 16) come from one streaming pass (k_wg_cols).
 #include <mutex>
 
 #include "nl_cuda.cuh"
@@ -185,8 +188,21 @@ struct Params {
     nl_render_stats *stats;
     float truncation;
     const float *dsdf_ext;
-    float *act_h1, *act_h2, *act_dh2, *act_dh1, *act_d;   // WGRAD: [cap][256] x 4, [cap]
+    float *act_h1, *act_dh1, *act_d;   // WGRAD: [cap][256] x 2, [cap]
+    uint32_t *act_m2;                  // WGRAD: relu'(h2) rows, [cap][8] (see m2_word)
 };
+
+// relu'(h2) of one sample as 8 words (32 B): quad thread t of the training kernel holds columns 8j + 2t + e (j = 0..31,
+// e = 0, 1) and stores them as 64 bits at word 2t, bit 2j + e.  Column c is therefore bit m2_bit(c) of word m2_word(c).
+__host__ __device__ __forceinline__ int m2_word(int c) { return 2 * ((c >> 1) & 3) + (c >> 7); }
+__host__ __device__ __forceinline__ int m2_bit(int c) { return (2 * (c >> 3) + (c & 1)) & 31; }
+// bits 0 and 1 of nibble i of `m` -> bits 2i and 2i + 1 of the result (16 bits)
+__device__ __forceinline__ uint32_t m2_pack(uint32_t m) {
+    m &= 0x33333333u;
+    m = (m | (m >> 2)) & 0x0F0F0F0Fu;
+    m = (m | (m >> 4)) & 0x00FF00FFu;
+    return (m | (m >> 8)) & 0x0000FFFFu;
+}
 
 // ring item i of a tile -> panel stage and N half
 __device__ __forceinline__ void item_of(int i, int &stage, int &half) {
@@ -349,14 +365,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                     if (on) mask2[j >> 3] |= 1u << ((j & 7) * 4 + x);
                     if (x < 2) ps0 = fmaf(hv, w2s[col], ps0); else ps1 = fmaf(hv, w2s[col], ps1);
                 }
-            if (WGRAD) {
-#pragma unroll
-                for (int jj = 0; jj < 16; ++jj) {
-                    const int col = 128 * half + 8 * jj + 2 * t;
-                    if (live0) *reinterpret_cast<float2 *>(p.act_h2 + (size_t)m0 * WN + col) = make_float2(d[4 * jj], d[4 * jj + 1]);
-                    if (live1) *reinterpret_cast<float2 *>(p.act_h2 + (size_t)m1 * WN + col) = make_float2(d[4 * jj + 2], d[4 * jj + 3]);
-                }
-            }
         }
         // the 4 threads of a quad hold the 4 column classes of the same two rows
         ps0 += __shfl_xor_sync(0xffffffffu, ps0, 1); ps0 += __shfl_xor_sync(0xffffffffu, ps0, 2);
@@ -395,16 +403,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                     if (live0) p.act_d[m0] = dsdf[0];
                     if (live1) p.act_d[m1] = dsdf[1];
                 }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int col = 8 * j + 2 * t;
-                    float v[4];
-#pragma unroll
-                    for (int x = 0; x < 4; ++x)
-                        v[x] = ((mask2[j >> 3] >> ((j & 7) * 4 + x)) & 1u) ? dsdf[x >> 1] * w2s[col + (x & 1)] : 0.f;
-                    if (live0) *reinterpret_cast<float2 *>(p.act_dh2 + (size_t)m0 * WN + col) = make_float2(v[0], v[1]);
-                    if (live1) *reinterpret_cast<float2 *>(p.act_dh2 + (size_t)m1 * WN + col) = make_float2(v[2], v[3]);
-                }
+                // mask2 bit 4j + x: row x >> 1, column 8j + 2t + (x & 1)
+                if (live0) *reinterpret_cast<uint2 *>(p.act_m2 + (size_t)m0 * 8 + 2 * t) =
+                    make_uint2(m2_pack(mask2[0]) | m2_pack(mask2[1]) << 16, m2_pack(mask2[2]) | m2_pack(mask2[3]) << 16);
+                if (live1) *reinterpret_cast<uint2 *>(p.act_m2 + (size_t)m1 * 8 + 2 * t) =
+                    make_uint2(m2_pack(mask2[0] >> 2) | m2_pack(mask2[1] >> 2) << 16, m2_pack(mask2[2] >> 2) | m2_pack(mask2[3] >> 2) << 16);
             }
             // ---- backward layer 2: D3 = relu'(h2) . (diag(w2) W1).  The A operand is the 0/1 mask (exact in tf32: 2 terms) ----
 #pragma unroll
@@ -480,30 +483,44 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
     }
 }
 
-// gW1[j][k] += sum_s dh2[s][j] h1[s][k]: CTA = 128 x 128 output tile, split-K over samples (grid = 4 tiles x nsplit, one CTA
-// per SM: 148 registers per thread).
-// Chunks of 32 samples of both operands are double-buffered in shared memory by cp.async (rows padded to 136 floats: the
-// fragment loads (sample t / t+4, column g) hit 32 distinct banks); warp w owns rows 64 (w & 1) .. +63 and columns
-// 32 (w >> 1) .. +31 of the tile, 4 x 4 m16n8 accumulators.  hi/lo split of both operands at fragment load.
-constexpr int DW_KC = 32, DW_LD = 136;
-constexpr int DW_SMEM = 2 * 2 * DW_KC * DW_LD * 4;   // 68 KB: 2 operands x 2 buffers
+// G = m2^T (dsdf * h1), i.e. G[j][k] = sum_s relu'(h2[s][j]) dsdf[s] h1[s][k]: CTA = 128 x 128 tile of G, split-K over samples
+// (grid = 4 tiles x nsplit, one CTA per SM).  Chunks of 32 samples of h1, the mask rows and dsdf stream through a DW_NS-slot
+// shared-memory ring filled by cp.async DW_NS - 1 chunks ahead (h1 rows padded to 136 floats: the fragment loads (sample t / t+4,
+// column g) hit 32 distinct banks); warp w owns rows 64 (w & 1) .. +63 and columns 32 (w >> 1) .. +31 of the tile, 4 x 4 m16n8
+// accumulators.  The A operand is the mask itself (1.0f / 0, exact in tf32), so only B = dsdf * h1 is split into hi + lo: 2 MMAs
+// per fragment pair.  A thread's A rows j0 + wj + 16 mi + g (+8) all sit in word m2_word(g) + j0 / 128 of a mask row, at bit
+// m2_bit(wj + 16 mi + g) (+2).
+// The tensor core truncates the sums it accumulates, a bias that grows with the number of MMAs into one accumulator; so every
+// chunk's MMAs start from zero and the chunk sums are added up in fp32 (rounded to nearest) over the ~2e4 samples of a split.
+// The partial G is folded into the gradients it determines before the atomics:
+//   gW1[j][k] += w2[j] G[j][k]      gW2[j] += sum_k W1[j][k] G[j][k]   (the b1 * c part of gW2 comes from k_wg_cols)
+constexpr int DW_KC = 32, DW_LD = 136, DW_NS = 2;
+constexpr int DW_SMEM = DW_NS * DW_KC * (DW_LD + 8 + 1) * 4;   // 37 KB: DW_NS slots of h1, mask rows, dsdf
+static_assert(DW_SMEM + 4 * 128 * 4 <= 48 * 1024, "k_dw1_tc is launched without a shared-memory opt-in");
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t dst, const void *src, bool valid) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(valid ? 4 : 0) : "memory");
 }
 __device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ dh2,
-                                                const float *__restrict__ h1, float *__restrict__ gW1, int nsplit) {
+__global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t *__restrict__ M_dev, const uint32_t *__restrict__ m2,
+                                                const float *__restrict__ dsdf, const float *__restrict__ h1, const float *__restrict__ W1,
+                                                const float *__restrict__ w2, float *__restrict__ gW1, float *__restrict__ gW2, int nsplit) {
     extern __shared__ float4 dw_smem[];
-    auto As = reinterpret_cast<float(*)[DW_KC][DW_LD]>(dw_smem);
-    auto Bs = reinterpret_cast<float(*)[DW_KC][DW_LD]>(reinterpret_cast<float *>(dw_smem) + 2 * DW_KC * DW_LD);
+    auto Hs = reinterpret_cast<float(*)[DW_KC][DW_LD]>(dw_smem);
+    auto Ms = reinterpret_cast<uint32_t(*)[DW_KC][8]>(reinterpret_cast<float *>(dw_smem) + DW_NS * DW_KC * DW_LD);
+    auto Ds = reinterpret_cast<float(*)[DW_KC]>(reinterpret_cast<float *>(dw_smem) + DW_NS * DW_KC * (DW_LD + 8));
+    __shared__ float red[4][128];   // gW2 partials of the 4 warps that share a row range
     const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
     const int tile = blockIdx.x & 3, split = blockIdx.x >> 2;
     const int j0 = (tile >> 1) * 128, k0 = (tile & 1) * 128;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int wj = (warp & 1) * 64, wk = (warp >> 1) * 32;
+    const int mw = m2_word(g) + (j0 >> 7);
     float acc[4][4][4];
 #pragma unroll
     for (int a = 0; a < 4; ++a)
@@ -512,43 +529,61 @@ __global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t 
 #pragma unroll
             for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
     const long long nch = (M + DW_KC - 1) / DW_KC;
+    // samples past M are zero-filled in all three arrays (the buffer behind them is uninitialised).  Every thread commits one
+    // cp.async group per chunk slot, empty past the last chunk, so that wait_group DW_NS - 2 always means "chunk it has landed".
     auto load = [&](long long ch, int buf) {
+        if (ch >= nch) { asm volatile("cp.async.commit_group;" ::: "memory"); return; }
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const int f = tid + i * 256, r = f >> 5, c4 = (f & 31) * 4;   // 32 rows x 32 float4
             const long long s = ch * DW_KC + r;
             const bool v = s < M;
-            const size_t o = (size_t)(v ? s : 0) * WN;
-            cp_async16(smem_u32(&As[buf][r][c4]), dh2 + o + j0 + c4, v);
-            cp_async16(smem_u32(&Bs[buf][r][c4]), h1 + o + k0 + c4, v);
+            cp_async16(smem_u32(&Hs[buf][r][c4]), h1 + (size_t)(v ? s : 0) * WN + k0 + c4, v);
+        }
+        if (tid < 2 * DW_KC) {                                              // 32 rows x 2 x 16 B of mask
+            const long long s = ch * DW_KC + (tid >> 1);
+            const bool v = s < M;
+            cp_async16(smem_u32(&Ms[buf][tid >> 1][4 * (tid & 1)]), m2 + (size_t)(v ? s : 0) * 8 + 4 * (tid & 1), v);
+        } else if (tid < 3 * DW_KC) {
+            const int r = tid - 2 * DW_KC;
+            const long long s = ch * DW_KC + r;
+            const bool v = s < M;
+            cp_async4(smem_u32(&Ds[buf][r]), dsdf + (v ? s : 0), v);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
-    int buf = 0;
-    if (split < nch) load(split, 0);
-    for (long long ch = split; ch < nch; ch += nsplit, buf ^= 1) {
-        if (ch + nsplit < nch) {
-            load(ch + nsplit, buf ^ 1);
-            asm volatile("cp.async.wait_group 1;" ::: "memory");
-        } else {
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
-        }
-        __syncthreads();
+#pragma unroll
+    for (int i = 0; i < DW_NS - 1; ++i) load(split + (long long)i * nsplit, i);
+    for (long long ch = split, it = 0; ch < nch; ch += nsplit, ++it) {
+        const int buf = (int)(it % DW_NS);
+        asm volatile("cp.async.wait_group %0;" ::"n"(DW_NS - 2) : "memory");
+        __syncthreads();   // chunk `it` is visible to all threads, and all of them are done with the slot the next load refills
+        load(ch + (long long)(DW_NS - 1) * nsplit, (int)((it + DW_NS - 1) % DW_NS));
+        float part[4][4][4];
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) part[a][b][c] = 0.f;
 #pragma unroll
         for (int ks = 0; ks < DW_KC / 8; ++ks) {
             const int s0 = ks * 8 + t;
-            uint32_t ah[4][4], al[4][4], bh[4][2], bl[4][2];
+            const uint32_t w0 = Ms[buf][s0][mw], w1 = Ms[buf][s0 + 4][mw];
+            const float d0 = Ds[buf][s0], d1 = Ds[buf][s0 + 4];
+            uint32_t a[4][4], bh[4][2], bl[4][2];
 #pragma unroll
             for (int mi = 0; mi < 4; ++mi) {
-                const int j = wj + mi * 16 + g;
-                const float v[4] = {As[buf][s0][j], As[buf][s0][j + 8], As[buf][s0 + 4][j], As[buf][s0 + 4][j + 8]};
-#pragma unroll
-                for (int i = 0; i < 4; ++i) { ah[mi][i] = tf32_rna(v[i]); al[mi][i] = tf32_rna(v[i] - __uint_as_float(ah[mi][i])); }
+                const int sh = m2_bit(wj + mi * 16 + g);
+                a[mi][0] = ((w0 >> sh) & 1u) ? 0x3f800000u : 0u;
+                a[mi][1] = ((w0 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
+                a[mi][2] = ((w1 >> sh) & 1u) ? 0x3f800000u : 0u;
+                a[mi][3] = ((w1 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
             }
 #pragma unroll
             for (int ni = 0; ni < 4; ++ni) {
                 const int n = wk + ni * 8 + g;
-                const float v[2] = {Bs[buf][s0][n], Bs[buf][s0 + 4][n]};
+                const float v[2] = {d0 * Hs[buf][s0][n], d1 * Hs[buf][s0 + 4][n]};
 #pragma unroll
                 for (int i = 0; i < 2; ++i) { bh[ni][i] = tf32_rna(v[i]); bl[ni][i] = tf32_rna(v[i] - __uint_as_float(bh[ni][i])); }
             }
@@ -556,56 +591,73 @@ __global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t 
             for (int mi = 0; mi < 4; ++mi)
 #pragma unroll
                 for (int ni = 0; ni < 4; ++ni) {
-                    mma_tf32(acc[mi][ni], ah[mi], bh[ni][0], bh[ni][1]);
-                    mma_tf32(acc[mi][ni], ah[mi], bl[ni][0], bl[ni][1]);
-                    mma_tf32(acc[mi][ni], al[mi], bh[ni][0], bh[ni][1]);
+                    mma_tf32(part[mi][ni], a[mi], bh[ni][0], bh[ni][1]);
+                    mma_tf32(part[mi][ni], a[mi], bl[ni][0], bl[ni][1]);
                 }
         }
-        __syncthreads();
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) acc[a][b][c] += part[a][b][c];
     }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (split >= nch) return;
 #pragma unroll
     for (int mi = 0; mi < 4; ++mi)
 #pragma unroll
-        for (int ni = 0; ni < 4; ++ni) {
-            const int j = j0 + wj + mi * 16 + g, k = k0 + wk + ni * 8 + 2 * t;
-            atomicAdd(gW1 + (size_t)j * WN + k, acc[mi][ni][0]);
-            atomicAdd(gW1 + (size_t)j * WN + k + 1, acc[mi][ni][1]);
-            atomicAdd(gW1 + (size_t)(j + 8) * WN + k, acc[mi][ni][2]);
-            atomicAdd(gW1 + (size_t)(j + 8) * WN + k + 1, acc[mi][ni][3]);
+        for (int h = 0; h < 2; ++h) {
+            const int j = j0 + wj + mi * 16 + 8 * h + g;
+            const float s = w2[j];
+            float r = 0.f;
+#pragma unroll
+            for (int ni = 0; ni < 4; ++ni) {
+                const int k = k0 + wk + ni * 8 + 2 * t;
+                const float2 w = *reinterpret_cast<const float2 *>(W1 + (size_t)j * WN + k);
+                const float c0 = acc[mi][ni][2 * h], c1 = acc[mi][ni][2 * h + 1];
+                atomicAdd(gW1 + (size_t)j * WN + k, s * c0);
+                atomicAdd(gW1 + (size_t)j * WN + k + 1, s * c1);
+                r = fmaf(w.x, c0, fmaf(w.y, c1, r));
+            }
+            r += __shfl_xor_sync(0xffffffffu, r, 1);
+            r += __shfl_xor_sync(0xffffffffu, r, 2);
+            if (t == 0) red[warp >> 1][wj + mi * 16 + 8 * h + g] = r;
         }
+    __syncthreads();
+    if (tid < 128) atomicAdd(gW2 + j0 + tid, red[0][tid] + red[1][tid] + red[2][tid] + red[3][tid]);
 }
 
-// Column sums of the stored activations, thread = column k, one contiguous range of samples per CTA:
-//   gW0[k][e] += sum_s dh1[s][k] x[s][e]   gb0[k] += sum_s dh1[s][k]   gW2[k] += sum_s d[s] h2[s][k]
-//   gb1[k]    += sum_s dh2[s][k]           gb2    += sum_s d[s]
+// Column sums, thread = column k, one contiguous range of samples per CTA:
+//   gW0[k][e] += sum_s dh1[s][k] x[s][e]   gb0[k] += sum_s dh1[s][k]   gb2 += sum_s d[s]
+//   c[k] = sum_s relu'(h2[s][k]) d[s]:     gb1[k] += w2[k] c[k]        gW2[k] += b1[k] c[k]
 constexpr int COLS_CHUNK = 64;
 __global__ void __launch_bounds__(WN) k_wg_cols(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ feats,
-                                                const float *__restrict__ dh1, const float *__restrict__ h2, const float *__restrict__ dh2,
-                                                const float *__restrict__ d, nl_mlp_grads g) {
+                                                const float *__restrict__ dh1, const uint32_t *__restrict__ m2, const float *__restrict__ d,
+                                                const float *__restrict__ w2, const float *__restrict__ b1, nl_mlp_grads g) {
     __shared__ float xs[COLS_CHUNK][16];
     __shared__ float ds[COLS_CHUNK];
+    __shared__ uint32_t ms[COLS_CHUNK][8];
     const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
     const long long per = ((M + gridDim.x - 1) / gridDim.x + COLS_CHUNK - 1) / COLS_CHUNK * COLS_CHUNK;
     const long long s0 = (long long)blockIdx.x * per, s1 = min(M, s0 + per);
-    const int k = threadIdx.x;
-    float gw0[16], gb0 = 0.f, gw2 = 0.f, gb1 = 0.f, gb2 = 0.f;
+    const int k = threadIdx.x, mw = m2_word(k), mb = m2_bit(k);
+    float gw0[16], gb0 = 0.f, c = 0.f, gb2 = 0.f;
 #pragma unroll
     for (int e = 0; e < 16; ++e) gw0[e] = 0.f;
     for (long long c0 = s0; c0 < s1; c0 += COLS_CHUNK) {
         const int n = (int)min((long long)COLS_CHUNK, s1 - c0);
         __syncthreads();
         for (int i = k; i < n * 16; i += WN) xs[i >> 4][i & 15] = feats[(size_t)c0 * 16 + i];
+        for (int i = k; i < n * 8; i += WN) ms[i >> 3][i & 7] = m2[(size_t)c0 * 8 + i];
         if (k < n) ds[k] = d[c0 + k];
         __syncthreads();
         for (int i = 0; i < n; ++i) {
-            const size_t o = (size_t)(c0 + i) * WN + k;
-            const float a = dh1[o];
+            const float a = dh1[(size_t)(c0 + i) * WN + k];
 #pragma unroll
             for (int e = 0; e < 16; ++e) gw0[e] = fmaf(a, xs[i][e], gw0[e]);
             gb0 += a;
-            gw2 = fmaf(ds[i], h2[o], gw2);
-            gb1 += dh2[o];
+            if ((ms[i][mw] >> mb) & 1u) c += ds[i];
             if (k == 0) gb2 += ds[i];
         }
     }
@@ -613,8 +665,8 @@ __global__ void __launch_bounds__(WN) k_wg_cols(long long M_host, const int32_t 
 #pragma unroll
     for (int e = 0; e < 16; ++e) atomicAdd(g.gW0 + k * 16 + e, gw0[e]);
     atomicAdd(g.gb0 + k, gb0);
-    atomicAdd(g.gW2 + k, gw2);
-    atomicAdd(g.gb1 + k, gb1);
+    atomicAdd(g.gb1 + k, w2[k] * c);
+    atomicAdd(g.gW2 + k, b1[k] * c);
     if (k == 0) atomicAdd(g.gb2, gb2);
 }
 
@@ -654,8 +706,8 @@ extern "C" int nl_mlp_tc_forward(int64_t M, const int32_t *d_M_dev, const float 
     return NL_OK;
 }
 
-// h1, h2, dh2, dh1 [cap][256] and d loss / d sdf [cap], cap = M rounded up to whole tiles
-extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * (4 * tc::WN + 1); }
+// h1, dh1 [cap][256], relu'(h2) bits [cap][8 words] and d loss / d sdf [cap], cap = M rounded up to whole tiles
+extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * (2 * tc::WN + 8 + 1); }
 
 extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *feats, const void *panels, const float *W1, const float *b0,
                                const float *b1, const float *w2, const float *b2, const uint8_t *s_flag, const float *s_depth,
@@ -681,10 +733,10 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
         return NL_OK;
     }
     const size_t cap = (size_t)((M + tc::TM - 1) / tc::TM) * tc::TM, plane = cap * tc::WN;
-    p.act_h1 = act; p.act_h2 = act + plane; p.act_dh2 = act + 2 * plane; p.act_dh1 = act + 3 * plane; p.act_d = act + 4 * plane;
+    p.act_h1 = act; p.act_dh1 = act + plane; p.act_m2 = reinterpret_cast<uint32_t *>(act + 2 * plane); p.act_d = act + 2 * plane + cap * 8;
     if (int rc = tc::launch<true, true>(p, stream)) return rc;
-    // The weight-gradient kernels only need what the kernel above wrote; on a second stream they overlap with whatever the
-    // caller enqueues next on `stream` (the embedding scatter).
+    // The weight-gradient kernels only need what the kernel above wrote and W1 / b1 / w2; on a second stream they overlap with
+    // whatever the caller enqueues next on `stream` (the embedding scatter).
     cudaStream_t ws = wgrad_stream_ ? (cudaStream_t)wgrad_stream_ : stream;
     if (ws != stream) {
         constexpr int NL_MAX_DEV = 64;
@@ -698,12 +750,9 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
         if (cudaEventRecord(ev, stream) != cudaSuccess || cudaStreamWaitEvent(ws, ev, 0) != cudaSuccess)
             return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not order the weight-gradient stream behind the decoder kernel");
     }
-    static NlPerDevice dw_configured;
-    const cudaError_t e = dw_configured.once([] { return cudaFuncSetAttribute(tc::k_dw1_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::DW_SMEM); });
-    if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
     const int nsplit = nl_num_sms() / 4 > 0 ? nl_num_sms() / 4 : 1;
-    tc::k_dw1_tc<<<4 * nsplit, 256, tc::DW_SMEM, ws>>>(M, d_M_dev, p.act_dh2, p.act_h1, grads->gW1, nsplit);
-    tc::k_wg_cols<<<nl_num_sms() * 4, tc::WN, 0, ws>>>(M, d_M_dev, feats, p.act_dh1, p.act_h2, p.act_dh2, p.act_d, *grads);
+    tc::k_dw1_tc<<<4 * nsplit, 256, tc::DW_SMEM, ws>>>(M, d_M_dev, p.act_m2, p.act_d, p.act_h1, W1, w2, grads->gW1, grads->gW2, nsplit);
+    tc::k_wg_cols<<<nl_num_sms() * 4, tc::WN, 0, ws>>>(M, d_M_dev, feats, p.act_dh1, p.act_m2, p.act_d, w2, b1, *grads);
     NL_CHECK_LAUNCH("nl_mlp_tc_train");
     return NL_OK;
 }
