@@ -14,13 +14,13 @@
 // Per 128-sample training tile the ring carries 42 items: layer 1 (2 halves), layer 2 (2 halves x 8 K-blocks of 32),
 // backward layer 2 (2 x 8) and backward layer 1 (8 K-blocks, N = 16).
 //
-// Decoder weight gradients (nl_mlp_tc_train with grads): the training kernel stores h1, dh1 [cap][256], the relu'(h2) bits
+// Decoder weight gradients (nl_mlp_tc_train with grads): the training kernel stores dh1 [cap][256], the relu'(h2) bits
 // (32 B per sample) and d loss / d sdf.  The output layer has one unit, so dh2 = dsdf * w2 * m2 (m2 = relu'(h2)) and everything
 // that would read h2 or dh2 follows from G = m2^T (dsdf * h1) and c = m2^T dsdf:
 //   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c
-// G (K = samples) is a split-K 2-term TF32 tensor-core GEMM whose A operand is the exact 0/1 mask (k_dw1_tc, mma.sync
-// m16n8k8: both operands are sample-major, which wgmma's tf32 forms cannot read); every CTA scales and contracts its partial G
-// before its atomics.  c, gb0, gb2 and gW0 = dh1^T x (K = 16) come from one streaming pass (k_wg_cols).
+// h1 = relu(x W0^T + b0) is not stored: its input x (K = 16, 64 B per sample) is, and recomputing h1 costs a tenth of G.  One
+// split-K kernel (k_wgrad_tc, mma.sync m16n8k8: the reduction index is the sample, so both operands are sample-major, which
+// wgmma's tf32 forms cannot read) recomputes h1, forms G with the exact 0/1 mask as A operand, gW0 = dh1^T x and the column sums.
 #include <mutex>
 
 #include "nl_cuda.cuh"
@@ -188,7 +188,7 @@ struct Params {
     nl_render_stats *stats;
     float truncation;
     const float *dsdf_ext;
-    float *act_h1, *act_dh1, *act_d;   // WGRAD: [cap][256] x 2, [cap]
+    float *act_dh1, *act_d;            // WGRAD: [cap][256], [cap]
     uint32_t *act_m2;                  // WGRAD: relu'(h2) rows, [cap][8] (see m2_word)
 };
 
@@ -326,13 +326,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 h[4 * j + x] = on ? v : 0.f;
                 if (on) mask1[j >> 3] |= 1u << ((j & 7) * 4 + x);
             }
-        if (WGRAD) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                if (live0) *reinterpret_cast<float2 *>(p.act_h1 + (size_t)m0 * WN + 8 * j + 2 * t) = make_float2(h[4 * j], h[4 * j + 1]);
-                if (live1) *reinterpret_cast<float2 *>(p.act_h1 + (size_t)m1 * WN + 8 * j + 2 * t) = make_float2(h[4 * j + 2], h[4 * j + 3]);
-            }
-        }
 
         // ---- layer 2 (two N halves) + output layer partial sums ----
         float ps0 = 0.f, ps1 = 0.f;
@@ -483,20 +476,37 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
     }
 }
 
-// G = m2^T (dsdf * h1), i.e. G[j][k] = sum_s relu'(h2[s][j]) dsdf[s] h1[s][k]: CTA = 128 x 128 tile of G, split-K over samples
-// (grid = 4 tiles x nsplit, one CTA per SM).  Chunks of 32 samples of h1, the mask rows and dsdf stream through a DW_NS-slot
-// shared-memory ring filled by cp.async DW_NS - 1 chunks ahead (h1 rows padded to 136 floats: the fragment loads (sample t / t+4,
-// column g) hit 32 distinct banks); warp w owns rows 64 (w & 1) .. +63 and columns 32 (w >> 1) .. +31 of the tile, 4 x 4 m16n8
-// accumulators.  The A operand is the mask itself (1.0f / 0, exact in tf32), so only B = dsdf * h1 is split into hi + lo: 2 MMAs
-// per fragment pair.  A thread's A rows j0 + wj + 16 mi + g (+8) all sit in word m2_word(g) + j0 / 128 of a mask row, at bit
-// m2_bit(wj + 16 mi + g) (+2).
+// Every decoder weight gradient from dh1, x = feats, the relu'(h2) bits and dsdf; h1 is recomputed from x instead of stored.
+// With G = m2^T (dsdf * h1) and c = m2^T dsdf (section at the top of the file):
+//   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c   gb2 = sum_s dsdf
+//   gW0 = dh1^T x      gb0 = sum_s dh1
+// Grid = 4 tiles x nsplit (one CTA per SM), split-K over samples.  CTA (tile, split) owns the 128 x 128 tile (j0, k0) of G and the
+// 64-column quarter 64 * tile of dh1, so dh1 is read exactly once.  Chunks of 32 samples of x, the mask rows, dsdf and the dh1
+// quarter stream through a WG_NS-slot shared-memory ring filled by cp.async WG_NS - 1 chunks ahead.  Per chunk the CTA
+//   1. recomputes dsdf * h1 for its 128 k columns, h1 = relu(x W0^T + b0), with 3xTF32 mma.sync m16n8k8 (K = 16) from the tf32
+//      hi / lo parts of W0 that the training kernel multiplies (the layer-1 panel), into the tile the G MMAs read.  Warp w owns
+//      samples 16 (w & 1) .. +15 and columns 32 (w >> 1) .. +31;
+//   2. accumulates G.  Warp w owns rows 64 (w & 1) .. +63 and columns 32 (w >> 1) .. +31 of the tile, 4 x 4 m16n8 accumulators.
+//      The A operand is the mask itself (1.0f / 0, exact in tf32), so only B = dsdf * h1 is split into hi + lo: 2 MMAs per
+//      fragment pair.  A thread's A rows j0 + wj + 16 mi + g (+8) all sit in word m2_word(g) + j0 / 128 of a mask row, at bit
+//      m2_bit(wj + 16 mi + g) (+2);
+//   3. accumulates gW0^T (16 x 64) = x^T dh1 with 3 terms (neither operand is exact); warp w owns dh1 columns 8w .. 8w + 7 of the
+//      quarter;
+//   4. sums gb0 over the quarter, c over the tile's rows (the k0 = 0 tiles) and gb2 (tile 0).
 // The tensor core truncates the sums it accumulates, a bias that grows with the number of MMAs into one accumulator; so every
-// chunk's MMAs start from zero and the chunk sums are added up in fp32 (rounded to nearest) over the ~2e4 samples of a split.
+// chunk's MMAs start from zero and the chunk sums are added up in fp32 (G) or fp64 (the rest) over the ~2e4 samples of a split.
+// Samples at or past the device-side count are zero-filled in every streamed array (the feature array behind them holds stale
+// values, possibly non-finite): x = dh1 = dsdf = 0 and an empty mask, so they add exact zeros everywhere.
 // The partial G is folded into the gradients it determines before the atomics:
-//   gW1[j][k] += w2[j] G[j][k]      gW2[j] += sum_k W1[j][k] G[j][k]   (the b1 * c part of gW2 comes from k_wg_cols)
-constexpr int DW_KC = 32, DW_LD = 136, DW_NS = 2;
-constexpr int DW_SMEM = DW_NS * DW_KC * (DW_LD + 8 + 1) * 4;   // 37 KB: DW_NS slots of h1, mask rows, dsdf
-static_assert(DW_SMEM + 4 * 128 * 4 <= 48 * 1024, "k_dw1_tc is launched without a shared-memory opt-in");
+//   gW1[j][k] += w2[j] G[j][k]      gW2[j] += sum_k W1[j][k] G[j][k] (+ b1[j] c[j] from the k0 = 0 tiles)
+constexpr int WG_KC = 32, WG_NS = 2;
+constexpr int WG_LDX = 20;     // x and W0 rows: fragment loads (row g, column t) hit 32 distinct banks
+constexpr int WG_LDQ = 72;     // dh1 quarter rows: fragment loads (sample t / t+4, column g) hit 32 distinct banks
+constexpr int WG_LDH = 136;    // dsdf * h1 rows: likewise
+constexpr int WG_OM = WG_KC * WG_LDX, WG_OD = WG_OM + WG_KC * 8, WG_OQ = WG_OD + WG_KC;   // slot: x | mask rows | dsdf | dh1 quarter
+constexpr int WG_SLOT = WG_OQ + WG_KC * WG_LDQ;                                            // floats
+constexpr int WG_SMEM = (WG_NS * WG_SLOT + WG_KC * WG_LDH + 2 * 128 * WG_LDX + 128) * 4;   // 63 KB: ring, h1 tile, W0 hi / lo, b0
+static_assert(WG_OM % 4 == 0 && WG_OD % 4 == 0 && WG_OQ % 4 == 0 && WG_SLOT % 4 == 0, "cp.async 16-byte destinations");
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
@@ -507,20 +517,37 @@ __device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], 
     asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t *__restrict__ M_dev, const uint32_t *__restrict__ m2,
-                                                const float *__restrict__ dsdf, const float *__restrict__ h1, const float *__restrict__ W1,
-                                                const float *__restrict__ w2, float *__restrict__ gW1, float *__restrict__ gW2, int nsplit) {
-    extern __shared__ float4 dw_smem[];
-    auto Hs = reinterpret_cast<float(*)[DW_KC][DW_LD]>(dw_smem);
-    auto Ms = reinterpret_cast<uint32_t(*)[DW_KC][8]>(reinterpret_cast<float *>(dw_smem) + DW_NS * DW_KC * DW_LD);
-    auto Ds = reinterpret_cast<float(*)[DW_KC]>(reinterpret_cast<float *>(dw_smem) + DW_NS * DW_KC * (DW_LD + 8));
-    __shared__ float red[4][128];   // gW2 partials of the 4 warps that share a row range
+__device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { hi[i] = tf32_rna(v[i]); lo[i] = tf32_rna(v[i] - __uint_as_float(hi[i])); }
+}
+__global__ void __launch_bounds__(256) k_wgrad_tc(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ x,
+                                                  const float *__restrict__ dh1, const uint32_t *__restrict__ m2, const float *__restrict__ dsdf,
+                                                  const uint8_t *__restrict__ panels, const float *__restrict__ b0, const float *__restrict__ W1,
+                                                  const float *__restrict__ b1, const float *__restrict__ w2, nl_mlp_grads grads, int nsplit) {
+    extern __shared__ float4 wg_smem[];
+    float *ring = reinterpret_cast<float *>(wg_smem);
+    float *Hs = ring + WG_NS * WG_SLOT;                                  // [32][WG_LDH]: dsdf * h1, columns k0 ..
+    uint32_t *W0h = reinterpret_cast<uint32_t *>(Hs + WG_KC * WG_LDH);  // [128][WG_LDX]: W0[k0 + r][e], tf32 hi
+    uint32_t *W0l = W0h + 128 * WG_LDX;                                  //                                  lo
+    float *b0s = reinterpret_cast<float *>(W0l + 128 * WG_LDX);
+    __shared__ float red[4][128];     // gW2 partials of the 4 warps that share a row range
+    __shared__ double cred[2][128];   // c partials of the two sample halves
     const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
     const int tile = blockIdx.x & 3, split = blockIdx.x >> 2;
-    const int j0 = (tile >> 1) * 128, k0 = (tile & 1) * 128;
+    const int j0 = (tile >> 1) * 128, k0 = (tile & 1) * 128, q0 = tile * 64;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int wj = (warp & 1) * 64, wk = (warp >> 1) * 32;
     const int mw = m2_word(g) + (j0 >> 7);
+
+    // the layer-1 panel holds W0 row j at panel row j, logical column kperm(p) at position p (16 positions in 4 16-byte chunks)
+    for (int i = tid; i < 128 * 16; i += 256) {
+        const int r = i >> 4, pos = i & 15, off = panel_off(k0 + r, pos >> 2) + (pos & 3) * 4;
+        W0h[r * WG_LDX + kperm(pos)] = *reinterpret_cast<const uint32_t *>(panels + off);
+        W0l[r * WG_LDX + kperm(pos)] = *reinterpret_cast<const uint32_t *>(panels + PANEL_B + off);
+    }
+    if (tid < 128) b0s[tid] = b0[k0 + tid];
+
     float acc[4][4][4];
 #pragma unroll
     for (int a = 0; a < 4; ++a)
@@ -528,79 +555,166 @@ __global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t 
         for (int b = 0; b < 4; ++b)
 #pragma unroll
             for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
-    const long long nch = (M + DW_KC - 1) / DW_KC;
-    // samples past M are zero-filled in all three arrays (the buffer behind them is uninitialised).  Every thread commits one
-    // cp.async group per chunk slot, empty past the last chunk, so that wait_group DW_NS - 2 always means "chunk it has landed".
+    double gw0[4] = {0.0, 0.0, 0.0, 0.0}, gb0 = 0.0, c_acc = 0.0, gb2 = 0.0;
+    const long long nch = (M + WG_KC - 1) / WG_KC;
+    // Every thread commits one cp.async group per chunk slot, empty past the last chunk, so that wait_group WG_NS - 2 always means
+    // "chunk it has landed".
     auto load = [&](long long ch, int buf) {
         if (ch >= nch) { asm volatile("cp.async.commit_group;" ::: "memory"); return; }
+        float *sl = ring + buf * WG_SLOT;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int f = tid + i * 256, r = f >> 5, c4 = (f & 31) * 4;   // 32 rows x 32 float4
-            const long long s = ch * DW_KC + r;
+        for (int i = 0; i < 2; ++i) {                                    // dh1 quarter: 32 rows x 16 float4
+            const int f = tid + i * 256, r = f >> 4, c4 = (f & 15) * 4;
+            const long long s = ch * WG_KC + r;
             const bool v = s < M;
-            cp_async16(smem_u32(&Hs[buf][r][c4]), h1 + (size_t)(v ? s : 0) * WN + k0 + c4, v);
+            cp_async16(smem_u32(sl + WG_OQ + r * WG_LDQ + c4), dh1 + (size_t)(v ? s : 0) * WN + q0 + c4, v);
         }
-        if (tid < 2 * DW_KC) {                                              // 32 rows x 2 x 16 B of mask
-            const long long s = ch * DW_KC + (tid >> 1);
+        if (tid < 4 * WG_KC) {                                           // x: 32 rows x 4 float4
+            const int r = tid >> 2, c4 = (tid & 3) * 4;
+            const long long s = ch * WG_KC + r;
             const bool v = s < M;
-            cp_async16(smem_u32(&Ms[buf][tid >> 1][4 * (tid & 1)]), m2 + (size_t)(v ? s : 0) * 8 + 4 * (tid & 1), v);
-        } else if (tid < 3 * DW_KC) {
-            const int r = tid - 2 * DW_KC;
-            const long long s = ch * DW_KC + r;
+            cp_async16(smem_u32(sl + r * WG_LDX + c4), x + (size_t)(v ? s : 0) * 16 + c4, v);
+        } else if (tid < 6 * WG_KC) {                                    // mask: 32 rows x 2 x 16 B
+            const int r = (tid - 4 * WG_KC) >> 1, h = tid & 1;
+            const long long s = ch * WG_KC + r;
             const bool v = s < M;
-            cp_async4(smem_u32(&Ds[buf][r]), dsdf + (v ? s : 0), v);
+            cp_async16(smem_u32(sl + WG_OM + r * 8 + 4 * h), m2 + (size_t)(v ? s : 0) * 8 + 4 * h, v);
+        } else if (tid < 7 * WG_KC) {                                    // dsdf
+            const int r = tid - 6 * WG_KC;
+            const long long s = ch * WG_KC + r;
+            const bool v = s < M;
+            cp_async4(smem_u32(sl + WG_OD + r), dsdf + (v ? s : 0), v);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
 #pragma unroll
-    for (int i = 0; i < DW_NS - 1; ++i) load(split + (long long)i * nsplit, i);
+    for (int i = 0; i < WG_NS - 1; ++i) load(split + (long long)i * nsplit, i);
     for (long long ch = split, it = 0; ch < nch; ch += nsplit, ++it) {
-        const int buf = (int)(it % DW_NS);
-        asm volatile("cp.async.wait_group %0;" ::"n"(DW_NS - 2) : "memory");
-        __syncthreads();   // chunk `it` is visible to all threads, and all of them are done with the slot the next load refills
-        load(ch + (long long)(DW_NS - 1) * nsplit, (int)((it + DW_NS - 1) % DW_NS));
-        float part[4][4][4];
+        const int buf = (int)(it % WG_NS);
+        asm volatile("cp.async.wait_group %0;" ::"n"(WG_NS - 2) : "memory");
+        __syncthreads();   // chunk `it` is visible to all threads, and all of them are done with Hs and the slot the next load refills
+        load(ch + (long long)(WG_NS - 1) * nsplit, (int)((it + WG_NS - 1) % WG_NS));
+        const float *Xs = ring + buf * WG_SLOT, *Ds = Xs + WG_OD, *Qs = Xs + WG_OQ;
+        const uint32_t *Ms = reinterpret_cast<const uint32_t *>(Xs + WG_OM);
+
+        // ---- 1. Hs = dsdf * relu(x W0^T + b0), terms in the training kernel's order ----
+        {
+            const int sm0 = (warp & 1) * 16;
+            float d1[4][4];
 #pragma unroll
-        for (int a = 0; a < 4; ++a)
+            for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
-            for (int b = 0; b < 4; ++b)
+                for (int c = 0; c < 4; ++c) d1[ni][c] = 0.f;
 #pragma unroll
-                for (int c = 0; c < 4; ++c) part[a][b][c] = 0.f;
+            for (int ks = 0; ks < 2; ++ks) {
+                const float *xr = Xs + (sm0 + g) * WG_LDX + 8 * ks + t;
+                const float av[4] = {xr[0], xr[8 * WG_LDX], xr[4], xr[8 * WG_LDX + 4]};
+                uint32_t ah[4], al[4];
+                split4(av, ah, al);
 #pragma unroll
-        for (int ks = 0; ks < DW_KC / 8; ++ks) {
-            const int s0 = ks * 8 + t;
-            const uint32_t w0 = Ms[buf][s0][mw], w1 = Ms[buf][s0 + 4][mw];
-            const float d0 = Ds[buf][s0], d1 = Ds[buf][s0 + 4];
-            uint32_t a[4][4], bh[4][2], bl[4][2];
-#pragma unroll
-            for (int mi = 0; mi < 4; ++mi) {
-                const int sh = m2_bit(wj + mi * 16 + g);
-                a[mi][0] = ((w0 >> sh) & 1u) ? 0x3f800000u : 0u;
-                a[mi][1] = ((w0 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
-                a[mi][2] = ((w1 >> sh) & 1u) ? 0x3f800000u : 0u;
-                a[mi][3] = ((w1 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
+                for (int ni = 0; ni < 4; ++ni) {
+                    const int wr = (wk + 8 * ni + g) * WG_LDX + 8 * ks + t;
+                    mma_tf32(d1[ni], ah, W0h[wr], W0h[wr + 4]);
+                    mma_tf32(d1[ni], ah, W0l[wr], W0l[wr + 4]);
+                    mma_tf32(d1[ni], al, W0h[wr], W0h[wr + 4]);
+                }
             }
 #pragma unroll
             for (int ni = 0; ni < 4; ++ni) {
-                const int n = wk + ni * 8 + g;
-                const float v[2] = {d0 * Hs[buf][s0][n], d1 * Hs[buf][s0 + 4][n]};
+                const int n = wk + 8 * ni + 2 * t;
 #pragma unroll
-                for (int i = 0; i < 2; ++i) { bh[ni][i] = tf32_rna(v[i]); bl[ni][i] = tf32_rna(v[i] - __uint_as_float(bh[ni][i])); }
+                for (int h = 0; h < 2; ++h) {
+                    const int s = sm0 + g + 8 * h;
+                    const float v0 = d1[ni][2 * h] + b0s[n], v1 = d1[ni][2 * h + 1] + b0s[n + 1], d = Ds[s];
+                    *reinterpret_cast<float2 *>(Hs + s * WG_LDH + n) = make_float2(d * (v0 > 0.f ? v0 : 0.f), d * (v1 > 0.f ? v1 : 0.f));
+                }
             }
+        }
+        __syncthreads();
+
+        // ---- 2. G ----
+        {
+            float part[4][4][4];
 #pragma unroll
-            for (int mi = 0; mi < 4; ++mi)
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int b = 0; b < 4; ++b)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) part[a][b][c] = 0.f;
+#pragma unroll
+            for (int ks = 0; ks < WG_KC / 8; ++ks) {
+                const int s0 = ks * 8 + t;
+                const uint32_t w0 = Ms[s0 * 8 + mw], w1 = Ms[(s0 + 4) * 8 + mw];
+                uint32_t a[4][4], bh[4][2], bl[4][2];
+#pragma unroll
+                for (int mi = 0; mi < 4; ++mi) {
+                    const int sh = m2_bit(wj + mi * 16 + g);
+                    a[mi][0] = ((w0 >> sh) & 1u) ? 0x3f800000u : 0u;
+                    a[mi][1] = ((w0 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
+                    a[mi][2] = ((w1 >> sh) & 1u) ? 0x3f800000u : 0u;
+                    a[mi][3] = ((w1 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
+                }
 #pragma unroll
                 for (int ni = 0; ni < 4; ++ni) {
-                    mma_tf32(part[mi][ni], a[mi], bh[ni][0], bh[ni][1]);
-                    mma_tf32(part[mi][ni], a[mi], bl[ni][0], bl[ni][1]);
+                    const int n = wk + ni * 8 + g;
+                    const float v[2] = {Hs[s0 * WG_LDH + n], Hs[(s0 + 4) * WG_LDH + n]};
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) { bh[ni][i] = tf32_rna(v[i]); bl[ni][i] = tf32_rna(v[i] - __uint_as_float(bh[ni][i])); }
                 }
+#pragma unroll
+                for (int mi = 0; mi < 4; ++mi)
+#pragma unroll
+                    for (int ni = 0; ni < 4; ++ni) {
+                        mma_tf32(part[mi][ni], a[mi], bh[ni][0], bh[ni][1]);
+                        mma_tf32(part[mi][ni], a[mi], bl[ni][0], bl[ni][1]);
+                    }
+            }
+#pragma unroll
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int b = 0; b < 4; ++b)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) acc[a][b][c] += part[a][b][c];
         }
+
+        // ---- 3. gW0^T = x^T dh1: A[e][s] = x[s][e], B[s][n] = dh1[s][n] ----
+        {
+            float pw[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-        for (int a = 0; a < 4; ++a)
+            for (int ks = 0; ks < WG_KC / 8; ++ks) {
+                const float *xr = Xs + (8 * ks + t) * WG_LDX + g;
+                const float av[4] = {xr[0], xr[8], xr[4 * WG_LDX], xr[4 * WG_LDX + 8]};
+                const float *qr = Qs + (8 * ks + t) * WG_LDQ + 8 * warp + g;
+                uint32_t ah[4], al[4], bh[2], bl[2];
+                split4(av, ah, al);
+                const float bv[2] = {qr[0], qr[4 * WG_LDQ]};
 #pragma unroll
-            for (int b = 0; b < 4; ++b)
+                for (int i = 0; i < 2; ++i) { bh[i] = tf32_rna(bv[i]); bl[i] = tf32_rna(bv[i] - __uint_as_float(bh[i])); }
+                mma_tf32(pw, ah, bh[0], bh[1]);
+                mma_tf32(pw, ah, bl[0], bl[1]);
+                mma_tf32(pw, al, bh[0], bh[1]);
+            }
 #pragma unroll
-                for (int c = 0; c < 4; ++c) acc[a][b][c] += part[a][b][c];
+            for (int i = 0; i < 4; ++i) gw0[i] += pw[i];
+        }
+
+        // ---- 4. column sums ----
+        {
+            const int cc = tid & 63, sg = tid >> 6;   // gb0: 4 threads per column, 8 samples each
+            float sb = 0.f;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) sb += Qs[(8 * sg + i) * WG_LDQ + cc];
+            gb0 += sb;
+            if (k0 == 0) {                            // c: 2 threads per row, 16 samples each
+                const int col = j0 + (tid & 127), hs = (tid >> 7) * 16, w = m2_word(col), b = m2_bit(col);
+                float sc = 0.f;
+#pragma unroll
+                for (int i = 0; i < 16; ++i)
+                    if ((Ms[(hs + i) * 8 + w] >> b) & 1u) sc += Ds[hs + i];
+                c_acc += sc;
+            }
+            if (tile == 0 && tid < WG_KC) gb2 += Ds[tid];
+        }
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (split >= nch) return;
@@ -616,58 +730,34 @@ __global__ void __launch_bounds__(256) k_dw1_tc(long long M_host, const int32_t 
                 const int k = k0 + wk + ni * 8 + 2 * t;
                 const float2 w = *reinterpret_cast<const float2 *>(W1 + (size_t)j * WN + k);
                 const float c0 = acc[mi][ni][2 * h], c1 = acc[mi][ni][2 * h + 1];
-                atomicAdd(gW1 + (size_t)j * WN + k, s * c0);
-                atomicAdd(gW1 + (size_t)j * WN + k + 1, s * c1);
+                atomicAdd(grads.gW1 + (size_t)j * WN + k, s * c0);
+                atomicAdd(grads.gW1 + (size_t)j * WN + k + 1, s * c1);
                 r = fmaf(w.x, c0, fmaf(w.y, c1, r));
             }
             r += __shfl_xor_sync(0xffffffffu, r, 1);
             r += __shfl_xor_sync(0xffffffffu, r, 2);
             if (t == 0) red[warp >> 1][wj + mi * 16 + 8 * h + g] = r;
         }
-    __syncthreads();
-    if (tid < 128) atomicAdd(gW2 + j0 + tid, red[0][tid] + red[1][tid] + red[2][tid] + red[3][tid]);
-}
-
-// Column sums, thread = column k, one contiguous range of samples per CTA:
-//   gW0[k][e] += sum_s dh1[s][k] x[s][e]   gb0[k] += sum_s dh1[s][k]   gb2 += sum_s d[s]
-//   c[k] = sum_s relu'(h2[s][k]) d[s]:     gb1[k] += w2[k] c[k]        gW2[k] += b1[k] c[k]
-constexpr int COLS_CHUNK = 64;
-__global__ void __launch_bounds__(WN) k_wg_cols(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ feats,
-                                                const float *__restrict__ dh1, const uint32_t *__restrict__ m2, const float *__restrict__ d,
-                                                const float *__restrict__ w2, const float *__restrict__ b1, nl_mlp_grads g) {
-    __shared__ float xs[COLS_CHUNK][16];
-    __shared__ float ds[COLS_CHUNK];
-    __shared__ uint32_t ms[COLS_CHUNK][8];
-    const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
-    const long long per = ((M + gridDim.x - 1) / gridDim.x + COLS_CHUNK - 1) / COLS_CHUNK * COLS_CHUNK;
-    const long long s0 = (long long)blockIdx.x * per, s1 = min(M, s0 + per);
-    const int k = threadIdx.x, mw = m2_word(k), mb = m2_bit(k);
-    float gw0[16], gb0 = 0.f, c = 0.f, gb2 = 0.f;
+    if (k0 == 0) cred[tid >> 7][tid & 127] = c_acc;
+    // gW0^T fragment: rows (e) g and g + 8, columns (k) 2t and 2t + 1 of the warp's 8
 #pragma unroll
-    for (int e = 0; e < 16; ++e) gw0[e] = 0.f;
-    for (long long c0 = s0; c0 < s1; c0 += COLS_CHUNK) {
-        const int n = (int)min((long long)COLS_CHUNK, s1 - c0);
-        __syncthreads();
-        for (int i = k; i < n * 16; i += WN) xs[i >> 4][i & 15] = feats[(size_t)c0 * 16 + i];
-        for (int i = k; i < n * 8; i += WN) ms[i >> 3][i & 7] = m2[(size_t)c0 * 8 + i];
-        if (k < n) ds[k] = d[c0 + k];
-        __syncthreads();
-        for (int i = 0; i < n; ++i) {
-            const float a = dh1[(size_t)(c0 + i) * WN + k];
-#pragma unroll
-            for (int e = 0; e < 16; ++e) gw0[e] = fmaf(a, xs[i][e], gw0[e]);
-            gb0 += a;
-            if ((ms[i][mw] >> mb) & 1u) c += ds[i];
-            if (k == 0) gb2 += ds[i];
-        }
+    for (int i = 0; i < 4; ++i) atomicAdd(grads.gW0 + (size_t)(q0 + 8 * warp + 2 * t + (i & 1)) * 16 + g + 8 * (i >> 1), (float)gw0[i]);
+    atomicAdd(grads.gb0 + q0 + (tid & 63), (float)gb0);
+    if (tile == 0 && warp == 0) {
+        for (int off = 16; off > 0; off >>= 1) gb2 += __shfl_xor_sync(0xffffffffu, gb2, off);
+        if (lane == 0) atomicAdd(grads.gb2, (float)gb2);
     }
-    if (s0 >= s1) return;
-#pragma unroll
-    for (int e = 0; e < 16; ++e) atomicAdd(g.gW0 + k * 16 + e, gw0[e]);
-    atomicAdd(g.gb0 + k, gb0);
-    atomicAdd(g.gb1 + k, w2[k] * c);
-    atomicAdd(g.gW2 + k, b1[k] * c);
-    if (k == 0) atomicAdd(g.gb2, gb2);
+    __syncthreads();
+    if (tid < 128) {
+        const int j = j0 + tid;
+        float r = red[0][tid] + red[1][tid] + red[2][tid] + red[3][tid];
+        if (k0 == 0) {
+            const float c = (float)(cred[0][tid] + cred[1][tid]);
+            atomicAdd(grads.gb1 + j, w2[j] * c);
+            r += b1[j] * c;
+        }
+        atomicAdd(grads.gW2 + j, r);
+    }
 }
 
 template <bool TRAIN, bool WGRAD>
@@ -706,8 +796,8 @@ extern "C" int nl_mlp_tc_forward(int64_t M, const int32_t *d_M_dev, const float 
     return NL_OK;
 }
 
-// h1, dh1 [cap][256], relu'(h2) bits [cap][8 words] and d loss / d sdf [cap], cap = M rounded up to whole tiles
-extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * (2 * tc::WN + 8 + 1); }
+// dh1 [cap][256], relu'(h2) bits [cap][8 words] and d loss / d sdf [cap], cap = M rounded up to whole tiles
+extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * (tc::WN + 8 + 1); }
 
 extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *feats, const void *panels, const float *W1, const float *b0,
                                const float *b1, const float *w2, const float *b2, const uint8_t *s_flag, const float *s_depth,
@@ -733,10 +823,13 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
         return NL_OK;
     }
     const size_t cap = (size_t)((M + tc::TM - 1) / tc::TM) * tc::TM, plane = cap * tc::WN;
-    p.act_h1 = act; p.act_dh1 = act + plane; p.act_m2 = reinterpret_cast<uint32_t *>(act + 2 * plane); p.act_d = act + 2 * plane + cap * 8;
+    p.act_dh1 = act; p.act_m2 = reinterpret_cast<uint32_t *>(act + plane); p.act_d = act + plane + cap * 8;
     if (int rc = tc::launch<true, true>(p, stream)) return rc;
-    // The weight-gradient kernels only need what the kernel above wrote and W1 / b1 / w2; on a second stream they overlap with
-    // whatever the caller enqueues next on `stream` (the embedding scatter).
+    static NlPerDevice configured;
+    const cudaError_t e = configured.once([] { return cudaFuncSetAttribute(tc::k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::WG_SMEM); });
+    if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
+    // The weight-gradient kernel only needs what the kernel above wrote, the features, the layer-1 panel and b0 / W1 / b1 / w2; on a
+    // second stream it overlaps with whatever the caller enqueues next on `stream` (the embedding scatter).
     cudaStream_t ws = wgrad_stream_ ? (cudaStream_t)wgrad_stream_ : stream;
     if (ws != stream) {
         constexpr int NL_MAX_DEV = 64;
@@ -751,8 +844,8 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
             return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not order the weight-gradient stream behind the decoder kernel");
     }
     const int nsplit = nl_num_sms() / 4 > 0 ? nl_num_sms() / 4 : 1;
-    tc::k_dw1_tc<<<4 * nsplit, 256, tc::DW_SMEM, ws>>>(M, d_M_dev, p.act_m2, p.act_d, p.act_h1, W1, w2, grads->gW1, grads->gW2, nsplit);
-    tc::k_wg_cols<<<nl_num_sms() * 4, tc::WN, 0, ws>>>(M, d_M_dev, feats, p.act_dh1, p.act_m2, p.act_d, w2, b1, *grads);
+    tc::k_wgrad_tc<<<4 * nsplit, 256, tc::WG_SMEM, ws>>>(M, d_M_dev, feats, p.act_dh1, p.act_m2, p.act_d, p.panels, b0, W1, b1, w2, *grads,
+                                                          nsplit);
     NL_CHECK_LAUNCH("nl_mlp_tc_train");
     return NL_OK;
 }

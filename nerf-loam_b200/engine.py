@@ -52,7 +52,7 @@ def mlp_train(bufs, M_cap, M_dev, feats, sdf, dfeats, want_wgrad, act, s_flag=No
                                         _capi.ptr(dfeats), gp, _capi.ptr(act["buf"]) if want_wgrad else None, _capi.ptr(dsdf_ext),
                                         C.c_void_p(wgrad_stream.cuda_stream) if (want_wgrad and wgrad_stream is not None) else None, st),
                     "nl_mlp_tc_train")
-        _capi.LAUNCHES += 3 if want_wgrad else 1
+        _capi.LAUNCHES += 2 if want_wgrad else 1
     else:
         w = bufs.weights_struct()
         _capi.check(lib.nl_mlp_train(M_cap, M_dev, _capi.ptr(feats), C.byref(w), _capi.ptr(s_flag), _capi.ptr(s_depth), _capi.ptr(s_ray),
