@@ -19,8 +19,9 @@
 // that would read h2 or dh2 follows from G = m2^T (dsdf * h1) and c = m2^T dsdf:
 //   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c
 // h1 = relu(x W0^T + b0) is not stored: its input x (K = 16, 64 B per sample) is, and recomputing h1 costs a tenth of G.  One
-// split-K kernel (k_wgrad_tc, mma.sync m16n8k8: the reduction index is the sample, so both operands are sample-major, which
-// wgmma's tf32 forms cannot read) recomputes h1, forms G with the exact 0/1 mask as A operand, gW0 = dh1^T x and the column sums.
+// split-K kernel (k_wgrad_tc) recomputes h1 and forms G on wgmma, both transposed so that the sample is wgmma's K: h1^T = W0 x^T
+// with A = W0 from registers and B = x (K-major as stored), then G^T = (dsdf h1)^T m2 with A = the h1^T accumulator from
+// registers and B = the exact 0/1 mask expanded into a K-major tile.  gW0 = dh1^T x (mma.sync) and the column sums run beside it.
 #include <mutex>
 
 #include "nl_cuda.cuh"
@@ -109,6 +110,28 @@ __device__ __forceinline__ void wgmma_n16(float (&d)[8], uint32_t a0, uint32_t a
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1));
+}
+// D = A x B (scale-d = 0: the accumulator's previous contents are not read) and D += A x B, as used by k_wgrad_tc
+__device__ __forceinline__ void wgmma_n128_z(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31]), "=f"(d[32]), "=f"(d[33]), "=f"(d[34]), "=f"(d[35]), "=f"(d[36]), "=f"(d[37]), "=f"(d[38]), "=f"(d[39]), "=f"(d[40]), "=f"(d[41]), "=f"(d[42]), "=f"(d[43]), "=f"(d[44]), "=f"(d[45]), "=f"(d[46]), "=f"(d[47]), "=f"(d[48]), "=f"(d[49]), "=f"(d[50]), "=f"(d[51]), "=f"(d[52]), "=f"(d[53]), "=f"(d[54]), "=f"(d[55]), "=f"(d[56]), "=f"(d[57]), "=f"(d[58]), "=f"(d[59]), "=f"(d[60]), "=f"(d[61]), "=f"(d[62]), "=f"(d[63])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(0));
+}
+__device__ __forceinline__ void wgmma_n64_z(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(0));
+}
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1));
 }
 
@@ -480,33 +503,41 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
 // With G = m2^T (dsdf * h1) and c = m2^T dsdf (section at the top of the file):
 //   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c   gb2 = sum_s dsdf
 //   gW0 = dh1^T x      gb0 = sum_s dh1
-// Grid = 4 tiles x nsplit (one CTA per SM), split-K over samples.  CTA (tile, split) owns the 128 x 128 tile (j0, k0) of G and the
-// 64-column quarter 64 * tile of dh1, so dh1 is read exactly once.  Chunks of 32 samples of x, the mask rows, dsdf and the dh1
-// quarter stream through a WG_NS-slot shared-memory ring filled by cp.async WG_NS - 1 chunks ahead.  Per chunk the CTA
-//   1. recomputes dsdf * h1 for its 128 k columns, h1 = relu(x W0^T + b0), with 3xTF32 mma.sync m16n8k8 (K = 16) from the tf32
-//      hi / lo parts of W0 that the training kernel multiplies (the layer-1 panel), into the tile the G MMAs read.  Warp w owns
-//      samples 16 (w & 1) .. +15 and columns 32 (w >> 1) .. +31;
-//   2. accumulates G.  Warp w owns rows 64 (w & 1) .. +63 and columns 32 (w >> 1) .. +31 of the tile, 4 x 4 m16n8 accumulators.
-//      The A operand is the mask itself (1.0f / 0, exact in tf32), so only B = dsdf * h1 is split into hi + lo: 2 MMAs per
-//      fragment pair.  A thread's A rows j0 + wj + 16 mi + g (+8) all sit in word m2_word(g) + j0 / 128 of a mask row, at bit
-//      m2_bit(wj + 16 mi + g) (+2);
-//   3. accumulates gW0^T (16 x 64) = x^T dh1 with 3 terms (neither operand is exact); warp w owns dh1 columns 8w .. 8w + 7 of the
-//      quarter;
-//   4. sums gb0 over the quarter, c over the tile's rows (the k0 = 0 tiles) and gb2 (tile 0).
+// Grid = 4 tiles x nsplit (one CTA per SM), split-K over samples.  CTA (tile, split) owns the 128 x 128 tile (k0, j0) of G^T and the
+// 64-column quarter 64 * tile of dh1, so dh1 is read exactly once.  The reduction index is the sample, and wgmma's tf32 forms take
+// B only as K-major shared memory and A from registers or K-major shared memory, so G is formed transposed with K = samples,
+// G^T[k, j] = sum_s (dsdf * h1)^T[k, s] m2[s, j]: A comes from registers and B, the mask, is rebuilt per chunk as a K-major tile.
+// Warpgroup w owns rows k0 + 64 w .. +63 (wgmma M = 64) and all 128 columns j.  Per chunk of WG_KC = 64 samples it
+//   1. recomputes h1^T[k, s] = W0[k, :] x[s, :]^T (N = 64 samples, K = 16) with 3xTF32 wgmma, terms in the training kernel's
+//      order: A = the tf32 hi / lo parts of W0 that the training kernel multiplies (the layer-1 panel), held in 16 registers for
+//      the whole kernel; B = the chunk's x split into hi / lo tiles (x's own [s][e] rows are K-major);
+//   2. forms dsdf * relu(h1^T + b0) in the accumulator registers (b0 per row, dsdf per column) and splits it into hi / lo.  An
+//      accumulator fragment is the A fragment of the next GEMM once K is permuted inside every group of 8 (kperm), so the mask
+//      tile stores its samples in kperm order;
+//   3. accumulates G^T with 2 terms (the mask is exact in tf32): A from the registers of step 2, B = the mask expanded from its bits
+//      into a [128 j][64 s] tile of 0 / 1.0f (K-major, 128-byte swizzle, two K-blocks of 32 samples), shared by both warpgroups.
+// While the G wgmmas run, every warp forms its part of gW0^T (16 x 64) = x^T dh1 with 3xTF32 mma.sync m16n8k8 (warp w owns dh1
+// columns 8w .. 8w + 7 of the quarter), the column sums gb0, c (the k0 = 0 tiles) and gb2 (tile 0), and builds the next chunk's x
+// and mask tiles into the other of two tile buffers.  x, the mask rows, dsdf and the dh1 quarter stream through a WG_NS-slot
+// shared-memory ring filled by cp.async WG_NS - 1 chunks ahead; one __syncthreads per chunk publishes the next chunk's data and
+// tiles.
 // The tensor core truncates the sums it accumulates, a bias that grows with the number of MMAs into one accumulator; so every
-// chunk's MMAs start from zero and the chunk sums are added up in fp32 (G) or fp64 (the rest) over the ~2e4 samples of a split.
+// chunk's first wgmma starts from zero (scale-d = 0) and the chunk sums are added up in fp32 (G) or fp64 (the rest) over the ~2e4
+// samples of a split.
 // Samples at or past the device-side count are zero-filled in every streamed array (the feature array behind them holds stale
 // values, possibly non-finite): x = dh1 = dsdf = 0 and an empty mask, so they add exact zeros everywhere.
 // The partial G is folded into the gradients it determines before the atomics:
 //   gW1[j][k] += w2[j] G[j][k]      gW2[j] += sum_k W1[j][k] G[j][k] (+ b1[j] c[j] from the k0 = 0 tiles)
-constexpr int WG_KC = 32, WG_NS = 2;
-constexpr int WG_LDX = 20;     // x and W0 rows: fragment loads (row g, column t) hit 32 distinct banks
+constexpr int WG_KC = 64, WG_NS = 4;
+constexpr int WG_LDX = 20;     // x rows in the ring: fragment loads (row g, column t) hit 32 distinct banks
 constexpr int WG_LDQ = 72;     // dh1 quarter rows: fragment loads (sample t / t+4, column g) hit 32 distinct banks
-constexpr int WG_LDH = 136;    // dsdf * h1 rows: likewise
 constexpr int WG_OM = WG_KC * WG_LDX, WG_OD = WG_OM + WG_KC * 8, WG_OQ = WG_OD + WG_KC;   // slot: x | mask rows | dsdf | dh1 quarter
 constexpr int WG_SLOT = WG_OQ + WG_KC * WG_LDQ;                                            // floats
-constexpr int WG_SMEM = (WG_NS * WG_SLOT + WG_KC * WG_LDH + 2 * 128 * WG_LDX + 128) * 4;   // 63 KB: ring, h1 tile, W0 hi / lo, b0
+constexpr int WG_MT = (WG_KC / 32) * HALF;   // mask tile: K-blocks of 32 samples, 128 rows (j) x 128 B each
+constexpr int WG_XT = WG_KC * 128;           // x tile (hi or lo): a 128-byte row per sample, the 16 features in its first 64 B
+constexpr int WG_SMEM = 2 * (WG_MT + 2 * WG_XT) + WG_NS * WG_SLOT * 4 + 1024;   // 198 KB: 2 tile buffers, ring, alignment slack
 static_assert(WG_OM % 4 == 0 && WG_OD % 4 == 0 && WG_OQ % 4 == 0 && WG_SLOT % 4 == 0, "cp.async 16-byte destinations");
+static_assert(WG_KC == 64, "the loaders and the x-tile build assign one 16-byte piece of x per thread");
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
@@ -521,236 +552,246 @@ __device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&hi)[4], u
 #pragma unroll
     for (int i = 0; i < 4; ++i) { hi[i] = tf32_rna(v[i]); lo[i] = tf32_rna(v[i] - __uint_as_float(hi[i])); }
 }
-__global__ void __launch_bounds__(256) k_wgrad_tc(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ x,
-                                                  const float *__restrict__ dh1, const uint32_t *__restrict__ m2, const float *__restrict__ dsdf,
-                                                  const uint8_t *__restrict__ panels, const float *__restrict__ b0, const float *__restrict__ W1,
-                                                  const float *__restrict__ b1, const float *__restrict__ w2, nl_mlp_grads grads, int nsplit) {
-    extern __shared__ float4 wg_smem[];
-    float *ring = reinterpret_cast<float *>(wg_smem);
-    float *Hs = ring + WG_NS * WG_SLOT;                                  // [32][WG_LDH]: dsdf * h1, columns k0 ..
-    uint32_t *W0h = reinterpret_cast<uint32_t *>(Hs + WG_KC * WG_LDH);  // [128][WG_LDX]: W0[k0 + r][e], tf32 hi
-    uint32_t *W0l = W0h + 128 * WG_LDX;                                  //                                  lo
-    float *b0s = reinterpret_cast<float *>(W0l + 128 * WG_LDX);
-    __shared__ float red[4][128];     // gW2 partials of the 4 warps that share a row range
+// keeps the compiler from moving reads of wgmma accumulators above the wgmma.wait_group that completes them
+template <int N>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+__global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ x,
+                                                     const float *__restrict__ dh1, const uint32_t *__restrict__ m2, const float *__restrict__ dsdf,
+                                                     const uint8_t *__restrict__ panels, const float *__restrict__ b0, const float *__restrict__ W1,
+                                                     const float *__restrict__ b1, const float *__restrict__ w2, nl_mlp_grads grads, int nsplit) {
+    extern __shared__ uint8_t wg_smem[];
+    const uint32_t raw = smem_u32(wg_smem);
+    const uint32_t base = (raw + 1023u) & ~1023u;    // SWIZZLE_128B tiles need 1024-byte alignment
+    // tile buffer b: mask tile at b * WG_MT, x hi / lo at 2 WG_MT + (2b, 2b + 1) WG_XT; then the ring
+    uint8_t *tiles = wg_smem + (base - raw);
+    float *ring = reinterpret_cast<float *>(tiles + 2 * (WG_MT + 2 * WG_XT));
+    __shared__ float red[8][128];     // gW2 partials of the 8 warps
     __shared__ double cred[2][128];   // c partials of the two sample halves
     const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
     const int tile = blockIdx.x & 3, split = blockIdx.x >> 2;
     const int j0 = (tile >> 1) * 128, k0 = (tile & 1) * 128, q0 = tile * 64;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
-    const int wj = (warp & 1) * 64, wk = (warp >> 1) * 32;
-    const int mw = m2_word(g) + (j0 >> 7);
+    const int kr = k0 + 64 * (warp >> 2) + 16 * (warp & 3) + g;   // this thread's rows of h1^T and G^T: kr and kr + 8
 
-    // the layer-1 panel holds W0 row j at panel row j, logical column kperm(p) at position p (16 positions in 4 16-byte chunks)
-    for (int i = tid; i < 128 * 16; i += 256) {
-        const int r = i >> 4, pos = i & 15, off = panel_off(k0 + r, pos >> 2) + (pos & 3) * 4;
-        W0h[r * WG_LDX + kperm(pos)] = *reinterpret_cast<const uint32_t *>(panels + off);
-        W0l[r * WG_LDX + kperm(pos)] = *reinterpret_cast<const uint32_t *>(panels + PANEL_B + off);
-    }
-    if (tid < 128) b0s[tid] = b0[k0 + tid];
+    // W0 as A fragments of k-steps 0, 1 (K position q of k-step ks = feature 8 ks + q).  The layer-1 panel holds W0 row k at panel
+    // row k and feature kperm(p) at position p.
+    uint32_t w0h[2][4], w0l[2][4];
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {   // i: row kr + 8 (i & 1), feature 8 ks + t + 4 (i >> 1)
+            const int e = 8 * ks + t + 4 * (i >> 1), pos = (e & ~7) | ((e & 1) << 2) | ((e & 7) >> 1);
+            const int off = panel_off(kr + 8 * (i & 1), pos >> 2) + (pos & 3) * 4;
+            w0h[ks][i] = *reinterpret_cast<const uint32_t *>(panels + off);
+            w0l[ks][i] = *reinterpret_cast<const uint32_t *>(panels + PANEL_B + off);
+        }
+    const float b0a = b0[kr], b0b = b0[kr + 8];
 
-    float acc[4][4][4];
+    float tot[64];   // G^T: tot[4 jn + x] is row kr + 8 (x >> 1), column j0 + 8 jn + 2t + (x & 1)
 #pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int b = 0; b < 4; ++b)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
+    for (int i = 0; i < 64; ++i) tot[i] = 0.f;
     double gw0[4] = {0.0, 0.0, 0.0, 0.0}, gb0 = 0.0, c_acc = 0.0, gb2 = 0.0;
     const long long nch = (M + WG_KC - 1) / WG_KC;
-    // Every thread commits one cp.async group per chunk slot, empty past the last chunk, so that wait_group WG_NS - 2 always means
-    // "chunk it has landed".
+    // Every thread commits one cp.async group per chunk, empty past the last chunk, so that wait_group n always means "all but the
+    // n chunks issued last have landed".
     auto load = [&](long long ch, int buf) {
         if (ch >= nch) { asm volatile("cp.async.commit_group;" ::: "memory"); return; }
         float *sl = ring + buf * WG_SLOT;
+        const long long s0 = ch * WG_KC;
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {                                    // dh1 quarter: 32 rows x 16 float4
+        for (int i = 0; i < WG_KC / 16; ++i) {                           // dh1 quarter: 64 rows x 16 float4
             const int f = tid + i * 256, r = f >> 4, c4 = (f & 15) * 4;
-            const long long s = ch * WG_KC + r;
-            const bool v = s < M;
-            cp_async16(smem_u32(sl + WG_OQ + r * WG_LDQ + c4), dh1 + (size_t)(v ? s : 0) * WN + q0 + c4, v);
+            const bool v = s0 + r < M;
+            cp_async16(smem_u32(sl + WG_OQ + r * WG_LDQ + c4), dh1 + (size_t)(v ? s0 + r : 0) * WN + q0 + c4, v);
         }
-        if (tid < 4 * WG_KC) {                                           // x: 32 rows x 4 float4
+        {                                                                // x: 64 rows x 4 float4
             const int r = tid >> 2, c4 = (tid & 3) * 4;
-            const long long s = ch * WG_KC + r;
-            const bool v = s < M;
-            cp_async16(smem_u32(sl + r * WG_LDX + c4), x + (size_t)(v ? s : 0) * 16 + c4, v);
-        } else if (tid < 6 * WG_KC) {                                    // mask: 32 rows x 2 x 16 B
-            const int r = (tid - 4 * WG_KC) >> 1, h = tid & 1;
-            const long long s = ch * WG_KC + r;
-            const bool v = s < M;
-            cp_async16(smem_u32(sl + WG_OM + r * 8 + 4 * h), m2 + (size_t)(v ? s : 0) * 8 + 4 * h, v);
-        } else if (tid < 7 * WG_KC) {                                    // dsdf
-            const int r = tid - 6 * WG_KC;
-            const long long s = ch * WG_KC + r;
-            const bool v = s < M;
-            cp_async4(smem_u32(sl + WG_OD + r), dsdf + (v ? s : 0), v);
+            const bool v = s0 + r < M;
+            cp_async16(smem_u32(sl + r * WG_LDX + c4), x + (size_t)(v ? s0 + r : 0) * 16 + c4, v);
+        }
+        if (tid < 2 * WG_KC) {                                           // mask: 64 rows x 2 x 16 B
+            const int r = tid >> 1, h = tid & 1;
+            const bool v = s0 + r < M;
+            cp_async16(smem_u32(sl + WG_OM + r * 8 + 4 * h), m2 + (size_t)(v ? s0 + r : 0) * 8 + 4 * h, v);
+        } else if (tid < 3 * WG_KC) {                                    // dsdf
+            const int r = tid - 2 * WG_KC;
+            const bool v = s0 + r < M;
+            cp_async4(smem_u32(sl + WG_OD + r), dsdf + (v ? s0 + r : 0), v);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
+    // x hi / lo and mask tiles of the chunk in ring slot `sl` into tile buffer b.  Thread tid writes mask tile row bj for the
+    // samples of parity bh: positions 4 bh .. 4 bh + 3 of sample group q hold samples 8q + bh + 2i (kperm).  The k0 = 0 tiles also
+    // add those samples' dsdf into c[j0 + bj] here.
+    const int bj = tid & 127, bh = tid >> 7, bw = m2_word(bj) + (j0 >> 7), bb = m2_bit(bj);
+    auto build = [&](const float *sl, int b) {
+        {
+            const int r = tid >> 2, c = tid & 3;
+            const float4 v = *reinterpret_cast<const float4 *>(sl + r * WG_LDX + 4 * c);
+            const float a[4] = {v.x, v.y, v.z, v.w};
+            uint32_t hi[4], lo[4];
+            split4(a, hi, lo);
+            uint8_t *xt = tiles + 2 * WG_MT + 2 * b * WG_XT;
+            *reinterpret_cast<uint4 *>(xt + panel_off(r, c)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+            *reinterpret_cast<uint4 *>(xt + WG_XT + panel_off(r, c)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+        }
+        const uint32_t *Ms = reinterpret_cast<const uint32_t *>(sl + WG_OM);
+        const float *Ds = sl + WG_OD;
+        uint8_t *mt = tiles + b * WG_MT;
+        float sc = 0.f;
+#pragma unroll
+        for (int q = 0; q < WG_KC / 8; ++q) {
+            uint32_t f[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int s = 8 * q + 2 * i + bh;
+                const bool on = (Ms[s * 8 + bw] >> bb) & 1u;
+                f[i] = on ? 0x3f800000u : 0u;
+                if (k0 == 0) sc += on ? Ds[s] : 0.f;
+            }
+            *reinterpret_cast<uint4 *>(mt + (q >> 2) * HALF + panel_off(bj, 2 * (q & 3) + bh)) = make_uint4(f[0], f[1], f[2], f[3]);
+        }
+        c_acc += sc;
+    };
+
 #pragma unroll
     for (int i = 0; i < WG_NS - 1; ++i) load(split + (long long)i * nsplit, i);
+    asm volatile("cp.async.wait_group %0;" ::"n"(WG_NS - 2) : "memory");
+    __syncthreads();
+    if (split < nch) build(ring, 0);
     for (long long ch = split, it = 0; ch < nch; ch += nsplit, ++it) {
-        const int buf = (int)(it % WG_NS);
-        asm volatile("cp.async.wait_group %0;" ::"n"(WG_NS - 2) : "memory");
-        __syncthreads();   // chunk `it` is visible to all threads, and all of them are done with Hs and the slot the next load refills
-        load(ch + (long long)(WG_NS - 1) * nsplit, (int)((it + WG_NS - 1) % WG_NS));
-        const float *Xs = ring + buf * WG_SLOT, *Ds = Xs + WG_OD, *Qs = Xs + WG_OQ;
-        const uint32_t *Ms = reinterpret_cast<const uint32_t *>(Xs + WG_OM);
-
-        // ---- 1. Hs = dsdf * relu(x W0^T + b0), terms in the training kernel's order ----
-        {
-            const int sm0 = (warp & 1) * 16;
-            float d1[4][4];
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) d1[ni][c] = 0.f;
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-                const float *xr = Xs + (sm0 + g) * WG_LDX + 8 * ks + t;
-                const float av[4] = {xr[0], xr[8 * WG_LDX], xr[4], xr[8 * WG_LDX + 4]};
-                uint32_t ah[4], al[4];
-                split4(av, ah, al);
-#pragma unroll
-                for (int ni = 0; ni < 4; ++ni) {
-                    const int wr = (wk + 8 * ni + g) * WG_LDX + 8 * ks + t;
-                    mma_tf32(d1[ni], ah, W0h[wr], W0h[wr + 4]);
-                    mma_tf32(d1[ni], ah, W0l[wr], W0l[wr + 4]);
-                    mma_tf32(d1[ni], al, W0h[wr], W0h[wr + 4]);
-                }
-            }
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni) {
-                const int n = wk + 8 * ni + 2 * t;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int s = sm0 + g + 8 * h;
-                    const float v0 = d1[ni][2 * h] + b0s[n], v1 = d1[ni][2 * h + 1] + b0s[n + 1], d = Ds[s];
-                    *reinterpret_cast<float2 *>(Hs + s * WG_LDH + n) = make_float2(d * (v0 > 0.f ? v0 : 0.f), d * (v1 > 0.f ? v1 : 0.f));
-                }
-            }
-        }
+        asm volatile("cp.async.wait_group %0;" ::"n"(WG_NS - 3) : "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the tiles were written by ordinary stores, wgmma reads them
+        // chunk `it`'s tiles and chunk it + 1's data are visible; every thread is done with ring slot (it + WG_NS - 1) % WG_NS and
+        // its wgmmas on tile buffer (it + 1) & 1 have completed
         __syncthreads();
+        load(ch + (long long)(WG_NS - 1) * nsplit, (int)((it + WG_NS - 1) % WG_NS));
+        const float *sl = ring + (it % WG_NS) * WG_SLOT;
+        const int b = (int)(it & 1);
+        const uint64_t xd = make_desc(base + 2 * WG_MT + 2 * b * WG_XT), md = make_desc(base + b * WG_MT);
 
-        // ---- 2. G ----
+        // ---- gW0^T = x^T dh1 with mma.sync: A[e][s] = x[s][e], B[s][n] = dh1[s][n].  It runs before the wgmmas, where few registers
+        // are live, with an accumulator per term and per 32 samples, so that the MMAs do not wait on each other ----
         {
-            float part[4][4][4];
+            float pw[WG_KC / 32][3][4];
 #pragma unroll
-            for (int a = 0; a < 4; ++a)
+            for (int hk = 0; hk < WG_KC / 32; ++hk)
 #pragma unroll
-                for (int b = 0; b < 4; ++b)
+                for (int m = 0; m < 3; ++m)
 #pragma unroll
-                    for (int c = 0; c < 4; ++c) part[a][b][c] = 0.f;
+                    for (int i = 0; i < 4; ++i) pw[hk][m][i] = 0.f;
 #pragma unroll
             for (int ks = 0; ks < WG_KC / 8; ++ks) {
-                const int s0 = ks * 8 + t;
-                const uint32_t w0 = Ms[s0 * 8 + mw], w1 = Ms[(s0 + 4) * 8 + mw];
-                uint32_t a[4][4], bh[4][2], bl[4][2];
-#pragma unroll
-                for (int mi = 0; mi < 4; ++mi) {
-                    const int sh = m2_bit(wj + mi * 16 + g);
-                    a[mi][0] = ((w0 >> sh) & 1u) ? 0x3f800000u : 0u;
-                    a[mi][1] = ((w0 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
-                    a[mi][2] = ((w1 >> sh) & 1u) ? 0x3f800000u : 0u;
-                    a[mi][3] = ((w1 >> (sh + 2)) & 1u) ? 0x3f800000u : 0u;
-                }
-#pragma unroll
-                for (int ni = 0; ni < 4; ++ni) {
-                    const int n = wk + ni * 8 + g;
-                    const float v[2] = {Hs[s0 * WG_LDH + n], Hs[(s0 + 4) * WG_LDH + n]};
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) { bh[ni][i] = tf32_rna(v[i]); bl[ni][i] = tf32_rna(v[i] - __uint_as_float(bh[ni][i])); }
-                }
-#pragma unroll
-                for (int mi = 0; mi < 4; ++mi)
-#pragma unroll
-                    for (int ni = 0; ni < 4; ++ni) {
-                        mma_tf32(part[mi][ni], a[mi], bh[ni][0], bh[ni][1]);
-                        mma_tf32(part[mi][ni], a[mi], bl[ni][0], bl[ni][1]);
-                    }
-            }
-#pragma unroll
-            for (int a = 0; a < 4; ++a)
-#pragma unroll
-                for (int b = 0; b < 4; ++b)
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) acc[a][b][c] += part[a][b][c];
-        }
-
-        // ---- 3. gW0^T = x^T dh1: A[e][s] = x[s][e], B[s][n] = dh1[s][n] ----
-        {
-            float pw[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int ks = 0; ks < WG_KC / 8; ++ks) {
-                const float *xr = Xs + (8 * ks + t) * WG_LDX + g;
+                const float *xr = sl + (8 * ks + t) * WG_LDX + g;
                 const float av[4] = {xr[0], xr[8], xr[4 * WG_LDX], xr[4 * WG_LDX + 8]};
-                const float *qr = Qs + (8 * ks + t) * WG_LDQ + 8 * warp + g;
-                uint32_t ah[4], al[4], bh[2], bl[2];
-                split4(av, ah, al);
+                const float *qr = sl + WG_OQ + (8 * ks + t) * WG_LDQ + 8 * warp + g;
+                uint32_t xh[4], xl[4], bh[2], bl[2];
+                split4(av, xh, xl);
                 const float bv[2] = {qr[0], qr[4 * WG_LDQ]};
 #pragma unroll
                 for (int i = 0; i < 2; ++i) { bh[i] = tf32_rna(bv[i]); bl[i] = tf32_rna(bv[i] - __uint_as_float(bh[i])); }
-                mma_tf32(pw, ah, bh[0], bh[1]);
-                mma_tf32(pw, ah, bl[0], bl[1]);
-                mma_tf32(pw, al, bh[0], bh[1]);
+                mma_tf32(pw[ks >> 2][0], xh, bh[0], bh[1]);
+                mma_tf32(pw[ks >> 2][1], xh, bl[0], bl[1]);
+                mma_tf32(pw[ks >> 2][2], xl, bh[0], bh[1]);
             }
 #pragma unroll
-            for (int i = 0; i < 4; ++i) gw0[i] += pw[i];
+            for (int hk = 0; hk < WG_KC / 32; ++hk)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) gw0[i] += pw[hk][0][i] + pw[hk][1][i] + pw[hk][2][i];
         }
 
-        // ---- 4. column sums ----
-        {
-            const int cc = tid & 63, sg = tid >> 6;   // gb0: 4 threads per column, 8 samples each
-            float sb = 0.f;
+        // ---- 1. h1^T = W0 x^T ----
+        float d1[32];
+        wg_fence();
 #pragma unroll
-            for (int i = 0; i < 8; ++i) sb += Qs[(8 * sg + i) * WG_LDQ + cc];
-            gb0 += sb;
-            if (k0 == 0) {                            // c: 2 threads per row, 16 samples each
-                const int col = j0 + (tid & 127), hs = (tid >> 7) * 16, w = m2_word(col), b = m2_bit(col);
-                float sc = 0.f;
-#pragma unroll
-                for (int i = 0; i < 16; ++i)
-                    if ((Ms[(hs + i) * 8 + w] >> b) & 1u) sc += Ds[hs + i];
-                c_acc += sc;
-            }
-            if (tile == 0 && tid < WG_KC) gb2 += Ds[tid];
+        for (int ks = 0; ks < 2; ++ks) {
+            const uint64_t xh = xd + 2 * ks, xl = xh + (WG_XT >> 4);
+            if (ks == 0) wgmma_n64_z(d1, w0h[0][0], w0h[0][1], w0h[0][2], w0h[0][3], xh);
+            else wgmma_n64(d1, w0h[ks][0], w0h[ks][1], w0h[ks][2], w0h[ks][3], xh);
+            wgmma_n64(d1, w0l[ks][0], w0l[ks][1], w0l[ks][2], w0l[ks][3], xh);
+            wgmma_n64(d1, w0h[ks][0], w0h[ks][1], w0h[ks][2], w0h[ks][3], xl);
         }
+        wg_commit_wait();
+        wg_fence_acc(d1);
+
+        // ---- 2. A fragments of k-step kk (samples 8 kk .. +7; K position q <-> sample 8 kk + kperm(q)) of dsdf * relu(h1^T + b0) ----
+        uint32_t ah[WG_KC / 8][4], al[WG_KC / 8][4];
+        {
+            const float *Ds = sl + WG_OD;
+#pragma unroll
+            for (int kk = 0; kk < WG_KC / 8; ++kk) {
+                const float2 ds = *reinterpret_cast<const float2 *>(Ds + 8 * kk + 2 * t);
+                const float v0 = d1[4 * kk] + b0a, v1 = d1[4 * kk + 1] + b0a, v2 = d1[4 * kk + 2] + b0b, v3 = d1[4 * kk + 3] + b0b;
+                const float v[4] = {ds.x * (v0 > 0.f ? v0 : 0.f), ds.x * (v2 > 0.f ? v2 : 0.f), ds.y * (v1 > 0.f ? v1 : 0.f),
+                                    ds.y * (v3 > 0.f ? v3 : 0.f)};
+                split4(v, ah[kk], al[kk]);
+            }
+        }
+
+        // ---- 3. this chunk's G^T = (dsdf h1)^T m2, left running while the warps do the rest ----
+        float part[64];
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < WG_KC / 8; ++kk) {
+            const uint64_t bd = md + (kk >> 2) * (HALF >> 4) + 2 * (kk & 3);
+            if (kk == 0) wgmma_n128_z(part, ah[0][0], ah[0][1], ah[0][2], ah[0][3], bd);
+            else wgmma_n128(part, ah[kk][0], ah[kk][1], ah[kk][2], ah[kk][3], bd);
+            wgmma_n128(part, al[kk][0], al[kk][1], al[kk][2], al[kk][3], bd);
+        }
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+
+        // ---- column sums gb0 (4 threads per column, 16 samples each) and gb2 (tile 0); c is summed in build() ----
+        {
+            const float *Qs = sl + WG_OQ;
+            const int cc = tid & 63, sg = tid >> 6;
+            float sb[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+            for (int i = 0; i < WG_KC / 4; ++i) sb[i & 3] += Qs[(WG_KC / 4 * sg + i) * WG_LDQ + cc];
+            gb0 += (sb[0] + sb[1]) + (sb[2] + sb[3]);
+            if (tile == 0 && tid < WG_KC) gb2 += sl[WG_OD + tid];
+        }
+
+        // ---- the next chunk's tiles, into the buffer that the previous chunk's wgmmas read ----
+        if (ch + nsplit < nch) build(ring + ((it + 1) % WG_NS) * WG_SLOT, b ^ 1);
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        wg_fence_acc(part);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) tot[i] += part[i];
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (split >= nch) return;
 #pragma unroll
-    for (int mi = 0; mi < 4; ++mi)
+    for (int jn = 0; jn < 16; ++jn)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int j = j0 + wj + mi * 16 + 8 * h + g;
-            const float s = w2[j];
-            float r = 0.f;
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni) {
-                const int k = k0 + wk + ni * 8 + 2 * t;
-                const float2 w = *reinterpret_cast<const float2 *>(W1 + (size_t)j * WN + k);
-                const float c0 = acc[mi][ni][2 * h], c1 = acc[mi][ni][2 * h + 1];
-                atomicAdd(grads.gW1 + (size_t)j * WN + k, s * c0);
-                atomicAdd(grads.gW1 + (size_t)j * WN + k + 1, s * c1);
-                r = fmaf(w.x, c0, fmaf(w.y, c1, r));
-            }
-            r += __shfl_xor_sync(0xffffffffu, r, 1);
-            r += __shfl_xor_sync(0xffffffffu, r, 2);
-            if (t == 0) red[warp >> 1][wj + mi * 16 + 8 * h + g] = r;
+        for (int e = 0; e < 2; ++e) {
+            const int j = j0 + 8 * jn + 2 * t + e;
+            const float s = w2[j], ga = tot[4 * jn + e], gb = tot[4 * jn + 2 + e];
+            atomicAdd(grads.gW1 + (size_t)j * WN + kr, s * ga);
+            atomicAdd(grads.gW1 + (size_t)j * WN + kr + 8, s * gb);
+            float r = fmaf(W1[(size_t)j * WN + kr], ga, W1[(size_t)j * WN + kr + 8] * gb);
+            r += __shfl_xor_sync(0xffffffffu, r, 4);
+            r += __shfl_xor_sync(0xffffffffu, r, 8);
+            r += __shfl_xor_sync(0xffffffffu, r, 16);
+            if (g == 0) red[warp][8 * jn + 2 * t + e] = r;
         }
     if (k0 == 0) cred[tid >> 7][tid & 127] = c_acc;
     // gW0^T fragment: rows (e) g and g + 8, columns (k) 2t and 2t + 1 of the warp's 8
 #pragma unroll
     for (int i = 0; i < 4; ++i) atomicAdd(grads.gW0 + (size_t)(q0 + 8 * warp + 2 * t + (i & 1)) * 16 + g + 8 * (i >> 1), (float)gw0[i]);
     atomicAdd(grads.gb0 + q0 + (tid & 63), (float)gb0);
-    if (tile == 0 && warp == 0) {
+    if (tile == 0 && warp < WG_KC / 32) {
         for (int off = 16; off > 0; off >>= 1) gb2 += __shfl_xor_sync(0xffffffffu, gb2, off);
         if (lane == 0) atomicAdd(grads.gb2, (float)gb2);
     }
     __syncthreads();
     if (tid < 128) {
         const int j = j0 + tid;
-        float r = red[0][tid] + red[1][tid] + red[2][tid] + red[3][tid];
+        float r = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) r += red[w][tid];
         if (k0 == 0) {
             const float c = (float)(cred[0][tid] + cred[1][tid]);
             atomicAdd(grads.gb1 + j, w2[j] * c);

@@ -20,7 +20,7 @@ import torch  # noqa: E402
 
 import bench  # noqa: E402
 
-DECODER_KERNELS = ("k_mlp_wg", "k_wgrad_tc", "k_dw1_tc", "k_wg_cols", "k_tc_prepare")
+DECODER_KERNELS = ("k_mlp_wg", "k_wgrad_tc", "k_tc_prepare")
 
 
 def card(index):
