@@ -88,6 +88,55 @@ NL_API int64_t nl_assign_embedding_rows_subset(const int32_t *h_vertex_rows, int
                                         int64_t n_rows_before, int32_t *h_vox2row_rows);
 
 /* ============================================================================================
+ * 1b. Device octree -- section 1's insert and the map-update glue around it (Octree::insert octree.cpp:51-111,
+ *     Mapping.create_voxels / update_grid_features mapping.py:283-339) on the GPU, bit for bit: the same node ids, types,
+ *     dirty rows (ascending id) and embedding-row numbering as nl_octree_insert + nl_octree_export_dirty +
+ *     nl_assign_embedding_rows_subset (csrc/octree_dev.cu states the parallel restatement of the creation order).
+ *     The tree is capacity-sized device arrays owned by the caller, node id = row:
+ *       child i32[cap][8] (every child, FEATURE ones included; -1 = none), code u64[cap] (Morton code of the min corner truncated
+ *       to the node's level), type i8[cap] (-1 NONLEAF, 0 SURFACE, 1 FEATURE), level u8[cap] (side = grid_dim >> level),
+ *       scratch i32[cap] (resting value INT32_MAX), and a pending dirty list u32[] (resting value 0xffffffff).
+ *     The root (id 0: child -1, code 0, NONLEAF, level 0) is written by the caller.
+ *     d_counts i64[8]: [0] batch rejected, [1] new nodes, [2] dirty rows, [3] embedding rows after the update, [4] pending entries.
+ *     Workspace for n points with L = log2(grid_dim), P = 8n, T = sum_{d=1..L} min(P, 8^d) (bound on the new nodes):
+ *       bytes = max(42 P + 8 + 33 T + sort/scan scratch,  4 (P + 2n) + (T + P + 2n) + 68 n + 4 + sort/select/scan scratch), each array
+ *       256-byte aligned; the CUB scratch is queried for the current device, so only this call gives the exact figure.
+ *     Unlike nl_octree_insert, which inserts the points before a bad one and then fails, a batch with any coordinate outside
+ *     [0, grid_dim-2] is rejected as a whole: d_counts[0] = 1 and nothing is written to the tree by insert_count; the caller
+ *     then does not call insert_commit.
+ * ============================================================================================ */
+NL_API int64_t nl_devoctree_workspace_bytes(int64_t n_points, int64_t grid_dim);
+/* Octree::insert octree.cpp:51-111, step 1 (reads the tree only): validate the batch d_vox i32[n,3] (n <= 2^23), find the nodes
+ * it creates.  Writes d_counts[0..1]; the caller reads them back, grows the tree to n_nodes + d_counts[1] and commits. */
+NL_API int nl_devoctree_insert_count(int64_t grid_dim, const int32_t *d_child, const int32_t *d_vox, int64_t n, void *d_ws, int64_t ws_bytes,
+                              int64_t *d_counts, void *stream);
+/* Octree::insert octree.cpp:51-111, step 2 (same batch, same workspace, the tree unchanged since step 1): create the n_new nodes
+ * with ids n_nodes.., link them, promote FEATURE leaves visited by corner 0, and append the nodes below `base` (the node count at
+ * the last dirty export) whose rows change to the pending list, once each (it needs min(base, 10 n) free entries). */
+NL_API int nl_devoctree_insert_commit(int64_t grid_dim, int64_t n_nodes, int64_t n_new, int64_t base, int32_t *d_child, uint64_t *d_code,
+                               int8_t *d_type, uint8_t *d_level, int32_t *d_scratch, uint32_t *d_dirty_list, int64_t n, void *d_ws,
+                               int64_t ws_bytes, int64_t *d_counts, void *stream);
+/* nl_octree_export_dirty's id list (mapping.py:320-326 restricted to the changed rows): d_ids i32[n_list + n_nodes - base] =
+ * the pending list sorted, then base .. n_nodes-1; d_counts[2] = their number.  Clears the pending list.  n_points: points
+ * inserted since the last call (sizes the workspace). */
+NL_API int nl_devoctree_dirty_ids(int64_t grid_dim, int64_t n_nodes, int64_t base, int64_t n_list, uint32_t *d_dirty_list, int32_t *d_scratch,
+                           int32_t *d_ids, int64_t n_points, void *d_ws, int64_t ws_bytes, int64_t *d_counts, void *stream);
+/* nl_octree_export_map's rows (mapping.py:320-326, octree.cpp:293-342) from the device tree: rows o < n_rows (and o < *d_count if
+ * given) of node d_ids[o] (d_ids NULL: node o) into row o (compact != 0) or row = node id of centres f32[.,3], structure i32[.,9],
+ * vertex i32[.,8]. */
+NL_API int nl_devoctree_export(int64_t grid_dim, double voxel_size, int64_t n_rows, const int32_t *d_ids, const int64_t *d_count, int compact,
+                        const int32_t *d_child, const uint64_t *d_code, const int8_t *d_type, const uint8_t *d_level, float *d_centres,
+                        int32_t *d_structure, int32_t *d_vertex, void *stream);
+/* nl_assign_embedding_rows_subset (mapping.py:294-317) over the dirty rows d_ids[o < d_counts[2]] (n_rows: their bound) of the
+ * row = node id arrays written by nl_devoctree_export: numbers the new vertices from n_emb_rows on in d_vertex2row i32[cap],
+ * writes d_vox2row rows of those nodes and d_counts[3] = the new number of embedding rows. */
+NL_API int nl_devoctree_assign_rows(int64_t grid_dim, int64_t n_rows, const int32_t *d_ids, int64_t n_nodes, const int8_t *d_type,
+                             const int32_t *d_vertex, int32_t *d_vertex2row, int32_t *d_scratch, int64_t n_emb_rows, int32_t *d_vox2row,
+                             int64_t n_points, void *d_ws, int64_t ws_bytes, int64_t *d_counts, void *stream);
+/* find_octant (octree.cpp:151-171) for d_xyz i32[n,3]: leaf id or -1 into d_out i32[n] (has_voxel octree.cpp:173-206). */
+NL_API int nl_devoctree_find(int64_t grid_dim, const int32_t *d_child, const int32_t *d_xyz, int64_t n, int32_t *d_out, void *stream);
+
+/* ============================================================================================
  * 2. Drop-ins for the two live `grid` kernels (third_party/sparse_voxels/src/binding.cpp:12-20)
  * ============================================================================================ */
 /* grid.svo_intersect (intersect.cpp:83-112, intersect_gpu.cu:193-272).  ray_start/ray_dir f32[b,m,3],

@@ -68,6 +68,13 @@ _SIGNATURES = {
     "nl_octree_export_dirty": (C.c_int, [vp, vp, vp, vp, vp, C.c_int]),
     "nl_assign_embedding_rows_subset": (C.c_int64, [vp, C.c_int64, C.c_int64, vp, C.c_int64, vp]),
     "nl_octree_pack_children_rows": (C.c_int, [C.c_int32, vp, vp, vp, vp, vp]),
+    "nl_devoctree_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
+    "nl_devoctree_insert_count": (C.c_int, [C.c_int64, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
+    "nl_devoctree_insert_commit": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
+    "nl_devoctree_dirty_ids": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int64, vp, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
+    "nl_devoctree_export": (C.c_int, [C.c_int64, C.c_double, C.c_int64, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "nl_devoctree_assign_rows": (C.c_int, [C.c_int64, C.c_int64, vp, C.c_int64, vp, vp, vp, vp, C.c_int64, vp, C.c_int64, vp, C.c_int64, vp, vp]),
+    "nl_devoctree_find": (C.c_int, [C.c_int64, vp, vp, C.c_int64, vp, vp]),
     "nl_octree_get_voxels": (C.c_int64, [vp, vp, C.c_int64]),
     "nl_octree_get_leaf_voxels": (C.c_int64, [vp, vp, C.c_int64]),
     "nl_morton_encode": (C.c_uint64, [C.c_int, C.c_int, C.c_int]),

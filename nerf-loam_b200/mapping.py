@@ -9,6 +9,8 @@ What changes relative to the reference:
   * the octree export is already in hot-path layout (centres / structure / vertex) -- svo.Octree.export_map.
 `map_states` keeps the reference's dict keys so the reference's tracker/mesher can read it, plus
 "_mapstate" (engine.MapState) which the fused renderer uses directly.
+`octree="device"` keeps the octree itself on the GPU (svo.DeviceOctree): the voxels of a scan never leave the device, and the
+update patches the same buffers with the same ids and rows as the host tree.
 """
 import ctypes as C
 
@@ -17,7 +19,65 @@ import torch
 
 from . import _capi
 from .engine import MapState
-from .svo import Octree
+from .svo import DeviceOctree, Octree
+
+
+class _LazyMapStates(dict):
+    """The reference-format map_states dict of a device-octree update.  "_mapstate" and "voxel_vertex_emb" are device objects and
+    present at once; the CPU tensors (vertex / centres / structure / id table) are copied from the device the first time one of
+    them is read, so a loop that never reads them never pays the copy.  The dict belongs to one map version: read it before the
+    next update."""
+    _LAZY = ("voxel_vertex_idx", "voxel_center_xyz", "voxel_structure", "voxel_id2embedding_id")
+
+    def __init__(self, eager, build):
+        super().__init__(eager)
+        self._build = build
+
+    def _materialise(self):
+        if self._build is not None:
+            build, self._build = self._build, None
+            super().update(build())
+
+    def __getitem__(self, k):
+        if k in self._LAZY:
+            self._materialise()
+        return super().__getitem__(k)
+
+    def get(self, k, default=None):
+        if k in self._LAZY:
+            self._materialise()
+        return super().get(k, default)
+
+    def __contains__(self, k):
+        return k in self._LAZY or super().__contains__(k)
+
+    def __iter__(self):
+        self._materialise()
+        return super().__iter__()
+
+    def __len__(self):
+        self._materialise()
+        return super().__len__()
+
+    def keys(self):
+        self._materialise()
+        return super().keys()
+
+    def values(self):
+        self._materialise()
+        return super().values()
+
+    def items(self):
+        self._materialise()
+        return super().items()
+
+    def copy(self):
+        self._materialise()
+        return dict(super().items())
+
+    def __repr__(self):
+        self._materialise()
+        return super().__repr__()
 
 
 class MapUpdater:
@@ -29,15 +89,24 @@ class MapUpdater:
     in place, numbers the new vertices and re-packs the touched nodes; the reference re-exports the whole octree with a torch
     dispatcher call per node and re-uploads everything every frame (octree.cpp:293-342, mapping.py:309-337).  Stable addresses are
     also what lets the captured CUDA graphs of the optimisation loops (render_helpers._MapGraph / _TrackGraph) survive map updates.
-    `incremental=False` keeps the full-export path (used by the tests as the cross-check)."""
+    `incremental=False` keeps the full-export path (used by the tests as the cross-check).
+    `octree="device"` (CUDA, incremental only) inserts into svo.DeviceOctree instead: the scan's voxels stay on the device and the
+    update exports, numbers and re-packs the dirty rows there too, reading back only the new-node, dirty-row and embedding-row
+    counts (new rows drawn with init_std > 0 still come from the CPU generator, so their values equal the host path's)."""
 
     def __init__(self, voxel_size, embed_dim=16, grid_dim=256 * 256 * 4, device="cuda", init_std=0.0, seed=0, incremental=True,
-                 reserve_nodes=0, reserve_rows=0):
+                 reserve_nodes=0, reserve_rows=0, octree="host"):
         assert embed_dim == 16
+        if octree not in ("host", "device"):
+            raise ValueError(f"octree must be 'host' or 'device', not {octree!r}")
         self.voxel_size = float(voxel_size)
         self.device = torch.device(device)
-        self.svo = Octree()
+        self.on_device = octree == "device"
+        if self.on_device and (self.device.type != "cuda" or not incremental):
+            raise ValueError("octree='device' needs a CUDA device and the incremental update")
+        self.svo = DeviceOctree(self.device) if self.on_device else Octree()
         self.svo.init(grid_dim, embed_dim, voxel_size)     # mapping.py:81-82
+        self._vertex = self._v2r = None    # device tree only: vertex ids and the vertex -> row table, both indexed by node id
         self.vertex2row = np.full(0, -1, np.int32)
         self.n_rows = 0
         self.n_nodes = 0
@@ -63,13 +132,24 @@ class MapUpdater:
     def embeddings(self):
         return self._emb_buf[:self.n_rows]
 
+    @property
+    def vertex2row(self):
+        """i32 vertex (node id) -> embedding row, -1 = none (numpy; copied from the device with octree="device")."""
+        if self._v2r is not None:
+            return self._v2r[:self.n_nodes].cpu().numpy()
+        return self._vertex2row
+
+    @vertex2row.setter
+    def vertex2row(self, v):
+        self._vertex2row = v
+
     def create_voxels(self, points, pose):
         """mapping.py:283-291: sensor-frame points [N,3] + 4x4 pose -> voxel coordinates -> octree -> map_states."""
         pts = torch.as_tensor(points, dtype=torch.float32, device=self.device)
         T = torch.as_tensor(pose, dtype=torch.float32, device=self.device)
         world = pts @ T[:3, :3].transpose(-1, -2) + T[:3, 3]
         voxels = torch.div(world, self.voxel_size, rounding_mode="floor")
-        self.svo.insert(voxels.cpu().int())
+        self.svo.insert(voxels.int() if self.on_device else voxels.cpu().int())
         return self.update_grid_features()
 
     def insert_voxels(self, voxels_i32):
@@ -100,11 +180,46 @@ class MapUpdater:
             new[0][:k] = self._centres[:k]; new[1][:k] = self._structure[:k]; new[2][:k] = self._vox2row[:k]
             new[3][:k * 128] = self._packed[:k * 128]
         self._centres, self._structure, self._vox2row, self._packed = new
+        if self.on_device:
+            vx, v2r = torch.full((cap, 8), -1, dtype=torch.int32, device=d), torch.full((cap,), -1, dtype=torch.int32, device=d)
+            if self._cap:
+                vx[:self.n_nodes] = self._vertex[:self.n_nodes]; v2r[:self.n_nodes] = self._v2r[:self.n_nodes]
+            self._vertex, self._v2r = vx, v2r
         self._cap = cap
 
     def update_grid_features(self):
         """mapping.py:320-339.  Returns the engine.MapState (also stored, with the reference's dict keys, in self.map_states)."""
+        if self.on_device:
+            return self._update_device()
         return self._update_incremental() if self.incremental else self._update_full()
+
+    def _update_device(self):
+        n = self.svo.count_export_nodes()
+        self._grow_nodes(n)
+        if self.readers is not None:      # a tracker on another stream may still traverse the arrays that are patched below
+            for ev in self.readers.reader_events():
+                torch.cuda.current_stream(self.device).wait_event(ev)
+        ids, m, new_rows = self.svo.update_map(self._centres, self._structure, self._vertex, self._v2r, self._vox2row, self.n_rows)
+        self._grow_rows(new_rows)
+        if m:
+            _capi.check(_capi.lib().nl_octree_pack_children_rows(m, _capi.ptr(ids), _capi.ptr(self._centres), _capi.ptr(self._structure),
+                                                                 _capi.ptr(self._packed), _capi.stream_ptr()), "nl_octree_pack_children_rows")
+            _capi.LAUNCHES += 1
+        self.n_nodes = n
+        self.generation += 1
+        self.last_update = {"dirty_rows": int(m), "nodes": int(n), "embedding_rows": int(new_rows)}
+        ms = MapState.__new__(MapState)
+        ms.centres, ms.structure, ms.vox2row = self._centres[:n], self._structure[:n], self._vox2row[:n]
+        ms.emb = self.embeddings
+        ms.emb_full = self._emb_buf
+        ms.n_nodes = n
+        ms._packed = self._packed[:n * 128]
+        ms.stable = True
+        c, s, v, r = self._centres[:n], self._structure[:n], self._vertex[:n], self._v2r[:n]
+        build = lambda: {"voxel_vertex_idx": v.cpu(), "voxel_center_xyz": c.cpu(), "voxel_structure": s.cpu(),
+                         "voxel_id2embedding_id": r.cpu().view(-1, 1)}
+        self.map_states = _LazyMapStates({"voxel_vertex_emb": self.embeddings, "_mapstate": ms}, build)
+        return ms
 
     def _update_incremental(self):
         ids, c, s, v = self.svo.export_dirty()

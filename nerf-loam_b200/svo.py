@@ -162,3 +162,206 @@ class Octree:
                 self._h = None
         except Exception:
             pass
+
+
+_NONE_U32 = -1          # 0xffffffff as int32: an empty entry of the pending dirty list
+_REST = 2 ** 31 - 1     # resting value of the per-node scratch word
+
+
+def _at(t, byte_offset):
+    return C.c_void_p(t.data_ptr() + byte_offset)
+
+
+class DeviceOctree:
+    """`Octree` with the tree in device memory (csrc/octree_dev.cu, include/nerfloam_b200.h section 1b): the same node ids,
+    exports and counts as the host tree bit for bit, without copying the batch or the tree to the host.
+
+    `insert` accepts CPU or CUDA int32 [N,3] and reads back two counters (the rejection flag and the number of new nodes, to grow
+    the capacity-doubling node arrays).  Unlike the host tree, a batch with a coordinate outside [0, grid_dim-2] is rejected as a
+    whole (NerfLoamError) and leaves the tree unchanged.  `export_map` returns CPU tensors like `Octree.export_map`;
+    `export_dirty` (numpy, like the host) and `update_map` (straight into a MapUpdater's device buffers) export the rows changed
+    since the last dirty export.  try_insert, get_voxels, get_leaf_voxels, get_centres_and_children and pickling are not
+    implemented and raise."""
+
+    def __init__(self, device="cuda"):
+        self.device = torch.device(device)
+        self._init_args = None
+        self._counts = None
+
+    def init(self, grid_dim, feat_dim, voxel_size):
+        gd = int(grid_dim)
+        if gd < 2 or gd > (1 << 20) or gd & (gd - 1):
+            raise _capi.NerfLoamError("DeviceOctree.init: grid_dim must be a power of two in [2, 2^20]")
+        self._init_args = (gd, int(feat_dim), float(voxel_size))
+        self._cap = 0
+        self._n = 1                     # the root, id 0 (octree.cpp:41-43)
+        self._grow(4096)
+        self._base = 0                  # node count at the last dirty export: ids >= base are dirty
+        self._pending_points = 0        # points inserted since the last dirty export
+        self._list = torch.full((1024,), _NONE_U32, dtype=torch.int32, device=self.device)
+        self._list_used = 0
+        self._counts = torch.zeros(8, dtype=torch.int64, device=self.device)
+        self._ws = torch.empty(0, dtype=torch.uint8, device=self.device)
+        self._ids = torch.empty(1024, dtype=torch.int32, device=self.device)
+
+    def _check(self):
+        if self._init_args is None:
+            raise RuntimeError("Octree not initialized!")
+
+    @property
+    def grid_dim(self):
+        return self._init_args[0]
+
+    def _grow(self, n):
+        if n <= self._cap:
+            return
+        cap = max(n, 2 * self._cap, 4096)
+        d = self.device
+        new = (torch.full((cap, 8), -1, dtype=torch.int32, device=d), torch.zeros(cap, dtype=torch.int64, device=d),
+               torch.full((cap,), -1, dtype=torch.int8, device=d), torch.zeros(cap, dtype=torch.uint8, device=d),
+               torch.full((cap,), _REST, dtype=torch.int32, device=d))
+        if self._cap:
+            for a, b in zip(new, (self._child, self._code, self._type, self._level, self._scratch)):
+                a[:self._n] = b[:self._n]
+        self._child, self._code, self._type, self._level, self._scratch = new
+        self._cap = cap
+
+    def _workspace(self, n_points):
+        nb = int(_capi.lib().nl_devoctree_workspace_bytes(int(n_points), self.grid_dim))
+        if nb < 0:
+            raise _capi.NerfLoamError(_capi.lib().nl_last_error().decode())
+        if nb > self._ws.numel():
+            self._ws = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        return self._ws
+
+    def insert(self, vox):
+        self._check()
+        if not isinstance(vox, torch.Tensor):
+            vox = torch.from_numpy(np.ascontiguousarray(vox, dtype=np.int32))
+        if vox.dtype != torch.int32:
+            raise RuntimeError("expected an int32 tensor (the reference accessor<int,2> throws here)")
+        if vox.dim() != 2 or vox.shape[1] != 3:
+            print(f"Point dimensions mismatch: inputs are {vox.shape[-1]} expect 3")  # octree.cpp:62-66
+            return
+        v = vox.detach().to(self.device).contiguous()
+        n = v.shape[0]
+        if n == 0:
+            return
+        L = _capi.lib()
+        ws = self._workspace(n)
+        _capi.check(L.nl_devoctree_insert_count(self.grid_dim, _capi.ptr(self._child), _capi.ptr(v), n, _capi.ptr(ws), ws.numel(),
+                                                _capi.ptr(self._counts), _capi.stream_ptr()), "nl_devoctree_insert_count")
+        bad, n_new = self._counts[:2].tolist()                       # read-back 1: rejection flag, new nodes
+        if bad:
+            raise _capi.NerfLoamError("DeviceOctree.insert: voxel coordinate outside [0, grid_dim-2]; the batch was rejected "
+                                      "and the tree is unchanged")
+        n0 = self._n
+        self._grow(n0 + n_new)
+        need = self._list_used + min(self._base, 10 * n)            # pending-list entries this batch may append
+        if need > self._list.numel():
+            lst = torch.full((max(need, 2 * self._list.numel()),), _NONE_U32, dtype=torch.int32, device=self.device)
+            lst[:self._list_used] = self._list[:self._list_used]
+            self._list = lst
+        _capi.check(L.nl_devoctree_insert_commit(self.grid_dim, n0, n_new, self._base, _capi.ptr(self._child), _capi.ptr(self._code),
+                                                 _capi.ptr(self._type), _capi.ptr(self._level), _capi.ptr(self._scratch),
+                                                 _capi.ptr(self._list), n, _capi.ptr(ws), ws.numel(), _capi.ptr(self._counts),
+                                                 _capi.stream_ptr()), "nl_devoctree_insert_commit")
+        _capi.LAUNCHES += 2
+        self._list_used = need
+        self._n = n0 + n_new
+        self._pending_points += n
+
+    def count_nodes(self):
+        self._check()
+        return self._n
+
+    def count_export_nodes(self):
+        self._check()
+        return self._n
+
+    def count_leaf_nodes(self):
+        self._check()
+        return int((self._type[:self._n] == 0).sum())
+
+    def has_voxel(self, xyz):
+        self._check()
+        v = Octree._as_i32(xyz).reshape(-1)
+        if v.shape[0] != 3:
+            return False
+        out = torch.empty(1, dtype=torch.int32, device=self.device)
+        _capi.check(_capi.lib().nl_devoctree_find(self.grid_dim, _capi.ptr(self._child), _capi.ptr(torch.from_numpy(v).to(self.device)), 1,
+                                                  _capi.ptr(out), _capi.stream_ptr()), "nl_devoctree_find")
+        return bool(int(out[0]) >= 0)
+
+    def _export(self, rows, ids, count_ptr, compact, centres, structure, vertex):
+        _capi.check(_capi.lib().nl_devoctree_export(self.grid_dim, self._init_args[2], rows, _capi.ptr(ids), count_ptr, int(compact),
+                                                    _capi.ptr(self._child), _capi.ptr(self._code), _capi.ptr(self._type),
+                                                    _capi.ptr(self._level), _capi.ptr(centres), _capi.ptr(structure), _capi.ptr(vertex),
+                                                    _capi.stream_ptr()), "nl_devoctree_export")
+        _capi.LAUNCHES += 1
+
+    def export_map(self):
+        """(centres f32[n,3], structure i32[n,9], vertex i32[n,8]) on the CPU, equal to Octree.export_map()."""
+        self._check()
+        n, d = self._n, self.device
+        c = torch.empty((n, 3), dtype=torch.float32, device=d)
+        s = torch.empty((n, 9), dtype=torch.int32, device=d)
+        v = torch.empty((n, 8), dtype=torch.int32, device=d)
+        self._export(n, None, None, False, c, s, v)
+        return c.cpu(), s.cpu(), v.cpu()
+
+    def _dirty_ids(self):
+        """Sorted dirty ids into self._ids (device count in counts[2]); returns (their bound, points since the last export)."""
+        rows = self._list_used + self._n - self._base
+        if rows > self._ids.numel():
+            self._ids = torch.empty(max(rows, 2 * self._ids.numel()), dtype=torch.int32, device=self.device)
+        pts = self._pending_points
+        ws = self._workspace(pts)
+        _capi.check(_capi.lib().nl_devoctree_dirty_ids(self.grid_dim, self._n, self._base, self._list_used, _capi.ptr(self._list),
+                                                       _capi.ptr(self._scratch), _capi.ptr(self._ids), pts, _capi.ptr(ws), ws.numel(),
+                                                       _capi.ptr(self._counts), _capi.stream_ptr()), "nl_devoctree_dirty_ids")
+        _capi.LAUNCHES += 1
+        self._base, self._list_used, self._pending_points = self._n, 0, 0
+        return rows, pts
+
+    def export_dirty(self, clear=True):
+        """Octree.export_dirty(): (ids i32[m] ascending, centres f32[m,3], structure i32[m,9], vertex i32[m,8]) as numpy arrays."""
+        self._check()
+        if not clear:
+            raise NotImplementedError("DeviceOctree.export_dirty always clears the dirty rows")
+        rows, _ = self._dirty_ids()
+        d = self.device
+        c = torch.empty((rows, 3), dtype=torch.float32, device=d)
+        s = torch.empty((rows, 9), dtype=torch.int32, device=d)
+        v = torch.empty((rows, 8), dtype=torch.int32, device=d)
+        self._export(rows, self._ids, _at(self._counts, 16), True, c, s, v)
+        m = int(self._counts[2])
+        return (self._ids[:m].cpu().numpy(), c[:m].cpu().numpy(), s[:m].cpu().numpy(), v[:m].cpu().numpy())
+
+    def update_map(self, centres, structure, vertex, vertex2row, vox2row, n_emb_rows):
+        """The dirty export of a map update, on the device: the changed rows go to their node ids in the (capacity-sized, >= n
+        rows) centres / structure / vertex / vox2row buffers, new vertices get embedding rows n_emb_rows.. in vertex2row.
+        Reads back the dirty-row count and the new number of embedding rows; returns (ids, m, rows): the first m entries of
+        ids (device) are the dirty node ids."""
+        self._check()
+        rows, pts = self._dirty_ids()
+        self._export(rows, self._ids, _at(self._counts, 16), False, centres, structure, vertex)
+        ws = self._workspace(pts)
+        _capi.check(_capi.lib().nl_devoctree_assign_rows(self.grid_dim, rows, _capi.ptr(self._ids), self._n, _capi.ptr(self._type),
+                                                         _capi.ptr(vertex), _capi.ptr(vertex2row), _capi.ptr(self._scratch), int(n_emb_rows),
+                                                         _capi.ptr(vox2row), pts, _capi.ptr(ws), ws.numel(), _capi.ptr(self._counts),
+                                                         _capi.stream_ptr()), "nl_devoctree_assign_rows")
+        _capi.LAUNCHES += 1
+        m, n_rows = self._counts[2:4].tolist()                      # read-back 2: dirty rows, embedding rows
+        return self._ids, m, n_rows
+
+    def _unsupported(self, *a, **k):
+        raise NotImplementedError("DeviceOctree implements insert, the counts, has_voxel and the exports; use svo.Octree for this")
+
+    try_insert = get_voxels = get_leaf_voxels = get_centres_and_children = _unsupported
+
+    def get_features(self, pts):
+        return None
+
+    def __getstate__(self):
+        raise NotImplementedError("DeviceOctree cannot be pickled; use svo.Octree")

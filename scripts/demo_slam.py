@@ -4,7 +4,7 @@ map update (MapUpdater) -> publication to the tracker (share.SharedMap); at the 
 BASELINE.json config 2 ("KITTI seq 00 tracking+mapping incremental loop") / config 3 ("... + marching cubes") in spirit; prints a
 JSON summary (per-stage ms per scan, trajectory error against the synthetic ground truth).
 
-    python scripts/demo_slam.py [--scans 12] [--spacing 0.5] [--json out.json]
+    python scripts/demo_slam.py [--scans 12] [--spacing 0.5] [--octree host|device] [--json out.json]
 """
 import argparse, json, os, sys, time
 from types import SimpleNamespace
@@ -19,6 +19,7 @@ def main():
     ap.add_argument("--scans", type=int, default=12); ap.add_argument("--spacing", type=float, default=0.5)
     ap.add_argument("--init-calls", type=int, default=12); ap.add_argument("--json", default=None)
     ap.add_argument("--ray-selection", default="device", choices=["device", "host"])
+    ap.add_argument("--octree", default="host", choices=["host", "device"], help="where MapUpdater keeps the octree (the `update` stage)")
     a = ap.parse_args()
     dev = torch.device("cuda"); syn, rh = nl.synthetic, nl.render_helpers
     vs, md, trunc = 0.3, 40.0, 0.3
@@ -26,7 +27,7 @@ def main():
                                                   data_specs={"max_depth": md}))
     torch.manual_seed(777)
     dec = nl.lidar.Decoder(depth=2, width=256, in_dim=16, skips=[], embedder="none", multires=0).to(dev)
-    mu = nl.mapping.MapUpdater(vs, device=dev, reserve_nodes=400_000, reserve_rows=400_000)       # embeddings start at zero like the reference
+    mu = nl.mapping.MapUpdater(vs, device=dev, reserve_nodes=400_000, reserve_rows=400_000, octree=a.octree)   # embeddings start at zero like the reference
     shared = nl.share.SharedMap(lambda: nl.lidar.Decoder(depth=2, width=256, in_dim=16, skips=[], embedder="none", multires=0).to(dev))
     mu.readers = shared
     scans = [syn.make_scan(seed=1000 + i, sensor_xyz=(a.spacing * i, 0.05 * np.sin(0.7 * i), 0.0), yaw=0.01 * np.sin(0.5 * i)) for i in range(a.scans)]
@@ -41,7 +42,9 @@ def main():
                                                             ray_selection=a.ray_selection)
     # ---- first scan: map it, then train on it while "waiting for the tracker" (mapping.py:100-108) ----
     f0 = mk(0, nl.se3pose.OptimizablePose.from_matrix(gt[0].clone()))
+    t0 = tick()
     ms = mu.create_voxels(scans[0][0], gt[0])
+    t_update0 = (tick() - t0) * 1e3
     keyframes, est = [f0], [gt[0].clone()]
     t0 = tick()
     for _ in range(a.init_calls):
@@ -83,9 +86,9 @@ def main():
     t_mesh = (tick() - t0) * 1e3
     err = [float((e[:3, 3] - g[:3, 3]).norm()) for e, g in zip(est, gt)]
     rot = [float(torch.linalg.matrix_norm(e[:3, :3] - g[:3, :3])) for e, g in zip(est, gt)]
-    out = {"scans": a.scans, "spacing_m": a.spacing, "translation_error_m": {"mean": float(np.mean(err[1:])), "max": float(np.max(err[1:])), "last": err[-1]},
+    out = {"scans": a.scans, "spacing_m": a.spacing, "octree": a.octree, "translation_error_m": {"mean": float(np.mean(err[1:])), "max": float(np.max(err[1:])), "last": err[-1]},
            "rotation_error_fro": {"mean": float(np.mean(rot[1:])), "max": float(np.max(rot[1:]))},
-           "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "init_mapping_ms": t_init,
+           "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0, "init_mapping_ms": t_init,
            "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
            "map": {"nodes": ms.n_nodes, "embedding_rows": int(mu.n_rows), "last_update": mu.last_update},
            "per_scan_translation_error_m": [round(e, 4) for e in err]}
