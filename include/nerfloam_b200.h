@@ -136,6 +136,34 @@ NL_API int nl_devoctree_assign_rows(int64_t grid_dim, int64_t n_rows, const int3
 /* find_octant (octree.cpp:151-171) for d_xyz i32[n,3]: leaf id or -1 into d_out i32[n] (has_voxel octree.cpp:173-206). */
 NL_API int nl_devoctree_find(int64_t grid_dim, const int32_t *d_child, const int32_t *d_xyz, int64_t n, int32_t *d_out, void *stream);
 
+/* --------------------------------------------------------------------------------------------
+ * 1b, queries: the rest of section 1's method set on the device tree, equal to the host tree's results bit for bit.  None of
+ * them depends on the order in which atomics land, and none synchronises with the host between its launches.
+ *   Query workspace for n_nodes nodes and n points (n = 0 except for try_insert), N = n_nodes, P = 8n:
+ *     bytes = max(29 N, 16 P) + CUB sort/select scratch, each array 256-byte aligned; only this call gives the exact figure.
+ * -------------------------------------------------------------------------------------------- */
+NL_API int64_t nl_devoctree_query_workspace_bytes(int64_t n_nodes, int64_t n_points, int64_t grid_dim);
+/* nl_devoctree_export with every output of export_row (octree_host.cpp): get_centres_and_children (octree.cpp:293-342) is
+ * voxels4 f32[.,4] (xyz, side; zero for FEATURE nodes), children_f f32[.,8] (visited non-FEATURE children, else -1) and vertex
+ * i32[.,8]; centres / structure are nl_devoctree_export's.  Any output but d_vertex may be NULL (not written). */
+NL_API int nl_devoctree_export_nodes(int64_t grid_dim, double voxel_size, int64_t n_rows, const int32_t *d_ids, const int64_t *d_count,
+                              int compact, const int32_t *d_child, const uint64_t *d_code, const int8_t *d_type, const uint8_t *d_level,
+                              float *d_voxels4, float *d_children_f, float *d_centres, int32_t *d_structure, int32_t *d_vertex,
+                              void *stream);
+/* get_voxels (leaves_only = 0: d_out f32[n_nodes,4] = xyz, side of every node) and get_leaf_voxels (leaves_only = 1: d_out
+ * f32[m,3] of the SURFACE leaves, m <= n_nodes written to d_count i64[1]) in preorder (octree.cpp:212-252), without a tree walk:
+ * the children are visited in slot order and the slot is the Morton digit of its level, so preorder is the order of (code,
+ * level); equal codes are an ancestor chain, created root first, so one stable radix sort of the codes with the node ids as
+ * values is the preorder, and the leaves are its SURFACE subset. */
+NL_API int nl_devoctree_preorder(int64_t grid_dim, int64_t n_nodes, const uint64_t *d_code, const int8_t *d_type, const uint8_t *d_level,
+                          int leaves_only, float *d_out, int64_t *d_count, void *d_ws, int64_t ws_bytes, void *stream);
+/* try_insert (octree.cpp:113-149, nl_octree_try_insert) for d_vox i32[n,3], 1 <= n <= 2^23: d_out i64[2] = (number of distinct
+ * int32-truncated corner keys of the batch that are keys of the tree, number of distinct corner keys of the batch); the ratio
+ * is 1.0 * d_out[0] / d_out[1].  The tree's corner keys are the codes of its level-L nodes, so a key is one iff it decodes to
+ * in-grid coordinates whose leaf exists; keys are the host's (21 bits per axis), so negative and out-of-grid points alias alike. */
+NL_API int nl_devoctree_try_insert(int64_t grid_dim, const int32_t *d_child, const int32_t *d_vox, int64_t n, void *d_ws, int64_t ws_bytes,
+                            int64_t *d_out, void *stream);
+
 /* ============================================================================================
  * 2. Drop-ins for the two live `grid` kernels (third_party/sparse_voxels/src/binding.cpp:12-20)
  * ============================================================================================ */

@@ -75,6 +75,10 @@ _SIGNATURES = {
     "nl_devoctree_export": (C.c_int, [C.c_int64, C.c_double, C.c_int64, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]),
     "nl_devoctree_assign_rows": (C.c_int, [C.c_int64, C.c_int64, vp, C.c_int64, vp, vp, vp, vp, C.c_int64, vp, C.c_int64, vp, C.c_int64, vp, vp]),
     "nl_devoctree_find": (C.c_int, [C.c_int64, vp, vp, C.c_int64, vp, vp]),
+    "nl_devoctree_query_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
+    "nl_devoctree_export_nodes": (C.c_int, [C.c_int64, C.c_double, C.c_int64, vp, vp, C.c_int] + [vp] * 10),
+    "nl_devoctree_preorder": (C.c_int, [C.c_int64, C.c_int64, vp, vp, vp, C.c_int, vp, vp, vp, C.c_int64, vp]),
+    "nl_devoctree_try_insert": (C.c_int, [C.c_int64, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
     "nl_octree_get_voxels": (C.c_int64, [vp, vp, C.c_int64]),
     "nl_octree_get_leaf_voxels": (C.c_int64, [vp, vp, C.c_int64]),
     "nl_morton_encode": (C.c_uint64, [C.c_int, C.c_int, C.c_int]),

@@ -20,6 +20,10 @@
 //                      nl_octree_export_map's layout; k_first / k_rflag / scan / k_assign number the new embedding rows in
 //                      nl_assign_embedding_rows_subset's order, k_vox2row composes the rows of the dirty nodes.
 // No step depends on the order in which atomics land, so every run gives the same arrays.
+//
+// The queries (get_centres_and_children, get_voxels, get_leaf_voxels, try_insert) follow the insert path: k_export with the
+// host export_row's optional outputs, preorder as one stable sort of the node codes, try_insert as two sorts of the batch's
+// corner keys (see the comment above k_pre_init).
 #include <cub/cub.cuh>
 
 #include <climits>
@@ -348,9 +352,11 @@ __global__ void k_dirty_tail(int n_list, int64_t n_new, int64_t base, const uint
 
 __global__ void k_reset_pending(int64_t *counts) { counts[4] = 0; }
 
+// octree_host.cpp export_row: every output but vertex is optional (NULL = not written)
 __global__ void k_export(int64_t rows, const int32_t *__restrict__ ids, const int64_t *__restrict__ count, int compact, int L, int size, float vs,
                          const int32_t *__restrict__ child, const uint64_t *__restrict__ code, const int8_t *__restrict__ type,
-                         const uint8_t *__restrict__ level, float *centres, int32_t *structure, int32_t *vertex) {
+                         const uint8_t *__restrict__ level, float *voxels4, float *children_f, float *centres, int32_t *structure,
+                         int32_t *vertex) {
     const int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (o >= rows || (count && o >= *count)) return;
     const int64_t id = ids ? ids[o] : o;
@@ -365,13 +371,20 @@ __global__ void k_export(int64_t rows, const int32_t *__restrict__ ids, const in
         xyz[2] = (float)(int)squeeze3(c >> 2);
         sd = (float)((unsigned)size >> level[id]);
     }
+    if (voxels4) {
+        for (int a = 0; a < 3; ++a) voxels4[r * 4 + a] = xyz[a];
+        voxels4[r * 4 + 3] = sd;
+    }
     const float h = sd / 2.0f;
-    for (int a = 0; a < 3; ++a) centres[r * 3 + a] = __fmul_rn(__fadd_rn(xyz[a], h), vs);   // mapping.py:322, all fp32
+    if (centres)
+        for (int a = 0; a < 3; ++a) centres[r * 3 + a] = __fmul_rn(__fadd_rn(xyz[a], h), vs);   // mapping.py:322, all fp32
     for (int s = 0; s < 8; ++s) {
         const int32_t c = child[id * 8 + s];
-        structure[r * 9 + s] = (visited && c >= 0 && type[c] != kFeature) ? c : -1;
+        const int32_t v = (visited && c >= 0 && type[c] != kFeature) ? c : -1;
+        if (structure) structure[r * 9 + s] = v;
+        if (children_f) children_f[r * 8 + s] = (float)v;
     }
-    structure[r * 9 + 8] = (int32_t)sd;
+    if (structure) structure[r * 9 + 8] = (int32_t)sd;
     for (int k = 0; k < 8; ++k)
         vertex[r * 8 + k] = ty == kSurface ? find_node(child, L, size, (int)xyz[0] + (k >> 2), (int)xyz[1] + ((k >> 1) & 1), (int)xyz[2] + (k & 1)) : -1;
 }
@@ -434,6 +447,148 @@ __global__ void k_find(int64_t n, int L, int size, const int32_t *__restrict__ c
     if (i >= n) return;
     const int x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
     out[i] = (x < 0 || y < 0 || z < 0 || x >= size || y >= size || z >= size) ? -1 : find_node(child, L, size, x, y, z);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Queries.  Preorder (get_voxels / get_leaf_voxels, octree.cpp:212-252): children are visited in slot order and the slot is the
+// Morton digit of its level, so preorder is the order of (code, level); nodes with equal codes are an ancestor chain, created
+// root first, so a stable sort of the codes with the node ids as values (ascending) is the preorder.
+__global__ void k_pre_init(int N, const uint64_t *__restrict__ code, uint64_t *keys, uint32_t *vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    keys[i] = code[i];
+    vals[i] = (uint32_t)i;
+}
+
+__global__ void k_pre_rows(int N, int size, const uint32_t *__restrict__ order, const uint64_t *__restrict__ code,
+                           const uint8_t *__restrict__ level, float *out) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= N) return;
+    const uint32_t id = order[r];
+    const uint64_t c = code[id];
+    out[(size_t)r * 4 + 0] = (float)(int)squeeze3(c);
+    out[(size_t)r * 4 + 1] = (float)(int)squeeze3(c >> 1);
+    out[(size_t)r * 4 + 2] = (float)(int)squeeze3(c >> 2);
+    out[(size_t)r * 4 + 3] = (float)((unsigned)size >> level[id]);
+}
+
+__global__ void k_pre_flag(int N, const uint32_t *__restrict__ order, const int8_t *__restrict__ type, uint8_t *flag) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < N) flag[r] = type[order[r]] == kSurface;   // SURFACE nodes are leaves: the walk lists them and returns
+}
+
+__global__ void k_leaf_rows(int N, const uint32_t *__restrict__ sel, const int64_t *__restrict__ count, const uint64_t *__restrict__ code,
+                            float *out) {
+    const int o = blockIdx.x * blockDim.x + threadIdx.x;
+    if (o >= N || o >= *count) return;
+    const uint64_t c = code[sel[o]];
+    out[(size_t)o * 3 + 0] = (float)(int)squeeze3(c);
+    out[(size_t)o * 3 + 1] = (float)(int)squeeze3(c >> 1);
+    out[(size_t)o * 3 + 2] = (float)(int)squeeze3(c >> 2);
+}
+
+// try_insert (octree_host.cpp nl_octree_try_insert, octree.cpp:113-149): |{(int32) k : k in keys, k a corner key}| / |keys| over
+// the distinct corner keys of the batch.  The host's corner-key set is exactly the set of level-L node codes (every inserted
+// corner creates its leaf, whose code is the corner's full key), so a key is a corner key iff it decodes to in-grid coordinates
+// whose leaf exists.
+__global__ void k_try_keys(int P, const int32_t *__restrict__ vox, uint64_t *keys) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= P) return;
+    const int i = p >> 3, j = p & 7;
+    // morton() keeps the low 21 bits of each coordinate: negative and out-of-grid corners alias exactly as on the host
+    const uint64_t x = (uint32_t)vox[3 * i] + (uint32_t)(j >> 2), y = (uint32_t)vox[3 * i + 1] + (uint32_t)((j >> 1) & 1),
+                   z = (uint32_t)vox[3 * i + 2] + (uint32_t)(j & 1);
+    keys[p] = spread3(x) | (spread3(y) << 1) | (spread3(z) << 2);
+}
+
+// over the sorted keys: out[1] += distinct keys; low[k] = the low 32 bits of a distinct corner key, else bit 32 set
+__global__ void k_try_match(int P, int L, int size, const int32_t *__restrict__ child, const uint64_t *__restrict__ keys, uint64_t *low,
+                            int64_t *out) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    int first = 0;
+    if (k < P) {
+        const uint64_t key = keys[k];
+        uint64_t v = uint64_t(1) << 32;
+        first = k == 0 || keys[k - 1] != key;
+        if (first && (key >> (3 * L)) == 0 &&
+            find_node(child, L, size, (int)squeeze3(key), (int)squeeze3(key >> 1), (int)squeeze3(key >> 2)) >= 0)
+            v = key & 0xffffffffull;
+        low[k] = v;
+    }
+    const int c = __syncthreads_count(first);
+    if (threadIdx.x == 0 && c) atomicAdd((unsigned long long *)&out[1], (unsigned long long)c);
+}
+
+// over the sorted low words: out[0] += distinct low words of corner keys (octree.cpp:141-147 de-duplicates after truncation)
+__global__ void k_try_distinct(int P, const uint64_t *__restrict__ low, int64_t *out) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    int first = 0;
+    if (k < P) {
+        const uint64_t v = low[k];
+        first = (v >> 32) == 0 && (k == 0 || low[k - 1] != v);
+    }
+    const int c = __syncthreads_count(first);
+    if (threadIdx.x == 0 && c) atomicAdd((unsigned long long *)&out[0], (unsigned long long)c);
+}
+
+// Query workspace: the preorder of N nodes and try_insert of n points (P = 8n corner keys) each use it from offset 0; the CUB
+// scratch follows the larger of the two.  The arrays are pure arithmetic, so a short workspace is rejected before any CUDA call.
+struct QueryLayout {
+    int64_t N = 0, P = 0;
+    size_t pk_a = 0, pk_b = 0, pv_a = 0, pv_b = 0, pflag = 0, psel = 0;   // preorder
+    size_t tk_a = 0, tk_b = 0;                                           // try_insert
+    size_t tmp = 0, tmp_bytes = 0, total = 0;
+};
+
+void query_arrays(int64_t N, int64_t n, QueryLayout &l) {
+    l.N = N;
+    l.P = 8 * n;
+    size_t at = 0;
+    l.pk_a = take(at, 8 * (size_t)N); l.pk_b = take(at, 8 * (size_t)N);
+    l.pv_a = take(at, 4 * (size_t)N); l.pv_b = take(at, 4 * (size_t)N);
+    l.pflag = take(at, (size_t)N); l.psel = take(at, 4 * (size_t)N);
+    const size_t pre_end = at;
+    at = 0;
+    l.tk_a = take(at, 8 * (size_t)l.P); l.tk_b = take(at, 8 * (size_t)l.P);
+    l.tmp = (std::max(pre_end, at) + 255) & ~size_t(255);
+    l.total = l.tmp;
+}
+
+cudaError_t query_scratch(int L, QueryLayout &l) {
+    size_t a = 0, b = 0, c = 0, d = 0;
+    cudaError_t err;
+    cub::DoubleBuffer<uint64_t> k(nullptr, nullptr);
+    if (l.N > 0) {
+        cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
+        if ((err = cub::DeviceRadixSort::SortPairs(nullptr, a, k, v, (int)l.N, 0, 3 * L)) != cudaSuccess) return err;
+        if ((err = cub::DeviceSelect::Flagged(nullptr, b, (const uint32_t *)nullptr, (const uint8_t *)nullptr, (uint32_t *)nullptr,
+                                              (int64_t *)nullptr, (int)l.N)) != cudaSuccess)
+            return err;
+    }
+    if (l.P > 0) {
+        if ((err = cub::DeviceRadixSort::SortKeys(nullptr, c, k, (int)l.P, 0, 63)) != cudaSuccess) return err;
+        if ((err = cub::DeviceRadixSort::SortKeys(nullptr, d, k, (int)l.P, 0, 33)) != cudaSuccess) return err;
+    }
+    l.tmp_bytes = std::max(std::max(a, b), std::max(c, d));
+    l.total = l.tmp + l.tmp_bytes;
+    return cudaSuccess;
+}
+
+int short_qws(const char *what, int64_t ws_bytes, size_t need) {
+    char buf[192];
+    std::snprintf(buf, sizeof(buf), "%s: workspace of %lld bytes, nl_devoctree_query_workspace_bytes asks for %lld", what, (long long)ws_bytes,
+                  (long long)need);
+    return nl_set_error(buf);
+}
+
+int check_qws(int64_t N, int64_t n, int L, const void *ws, int64_t ws_bytes, QueryLayout &l, const char *what) {
+    query_arrays(N, n, l);
+    if (ws_bytes < (int64_t)l.total) return short_qws(what, ws_bytes, l.total);            // the arrays alone do not fit
+    if (((uintptr_t)ws & 255u) != 0) return nl_set_error("nl_devoctree: the workspace must be 256-byte aligned");
+    const cudaError_t e = query_scratch(L, l);
+    if (e != cudaSuccess) return cuda_fail(what, e);
+    if (ws_bytes < (int64_t)l.total) return short_qws(what, ws_bytes, l.total);
+    return NL_OK;
 }
 
 int check_ws(int64_t n, int L, const void *ws, int64_t ws_bytes, Layout &l, const char *what) {
@@ -577,8 +732,102 @@ int nl_devoctree_export(int64_t grid_dim, double voxel_size, int64_t n_rows, con
     if (n_rows == 0) return NL_OK;
     if (!d_child || !d_code || !d_type || !d_level || !d_centres || !d_structure || !d_vertex) return nl_set_error("nl_devoctree_export: null pointer");
     k_export<<<nl_div_up(n_rows, kThreads), kThreads, 0, (cudaStream_t)stream>>>(n_rows, d_ids, d_count, compact, L, (int)grid_dim, (float)voxel_size,
-                                                                                d_child, d_code, d_type, d_level, d_centres, d_structure, d_vertex);
+                                                                                d_child, d_code, d_type, d_level, nullptr, nullptr, d_centres,
+                                                                                d_structure, d_vertex);
     NL_CHECK_LAUNCH("nl_devoctree_export");
+    return NL_OK;
+}
+
+int nl_devoctree_export_nodes(int64_t grid_dim, double voxel_size, int64_t n_rows, const int32_t *d_ids, const int64_t *d_count, int compact,
+                              const int32_t *d_child, const uint64_t *d_code, const int8_t *d_type, const uint8_t *d_level, float *d_voxels4,
+                              float *d_children_f, float *d_centres, int32_t *d_structure, int32_t *d_vertex, void *stream) {
+    const int L = levels_of(grid_dim);
+    if (L < 0) return nl_set_error("nl_devoctree_export_nodes: grid_dim must be a power of two in [2, 2^20]");
+    if (n_rows < 0) return nl_set_error("nl_devoctree_export_nodes: negative n_rows");
+    if (n_rows == 0) return NL_OK;
+    if (!d_child || !d_code || !d_type || !d_level || !d_vertex) return nl_set_error("nl_devoctree_export_nodes: null pointer");
+    k_export<<<nl_div_up(n_rows, kThreads), kThreads, 0, (cudaStream_t)stream>>>(n_rows, d_ids, d_count, compact, L, (int)grid_dim, (float)voxel_size,
+                                                                                d_child, d_code, d_type, d_level, d_voxels4, d_children_f,
+                                                                                d_centres, d_structure, d_vertex);
+    NL_CHECK_LAUNCH("nl_devoctree_export_nodes");
+    return NL_OK;
+}
+
+int64_t nl_devoctree_query_workspace_bytes(int64_t n_nodes, int64_t n_points, int64_t grid_dim) {
+    const int L = levels_of(grid_dim);
+    if (L < 0 || n_nodes < 0 || n_nodes > INT32_MAX || n_points < 0 || n_points > kMaxPoints)
+        return nl_set_error("nl_devoctree_query_workspace_bytes: bad n_nodes, n_points or grid_dim");
+    QueryLayout l;
+    query_arrays(n_nodes, n_points, l);
+    const cudaError_t e = query_scratch(L, l);
+    if (e != cudaSuccess) return cuda_fail("nl_devoctree_query_workspace_bytes", e);
+    return (int64_t)l.total;
+}
+
+int nl_devoctree_preorder(int64_t grid_dim, int64_t n_nodes, const uint64_t *d_code, const int8_t *d_type, const uint8_t *d_level, int leaves_only,
+                          float *d_out, int64_t *d_count, void *d_ws, int64_t ws_bytes, void *stream) {
+    const int L = levels_of(grid_dim);
+    if (L < 0) return nl_set_error("nl_devoctree_preorder: grid_dim must be a power of two in [2, 2^20]");
+    if (n_nodes < 1 || n_nodes > INT32_MAX || (leaves_only != 0 && leaves_only != 1)) return nl_set_error("nl_devoctree_preorder: bad sizes");
+    if (!d_code || !d_type || !d_level || !d_out || !d_ws || (leaves_only && !d_count)) return nl_set_error("nl_devoctree_preorder: null pointer");
+    QueryLayout l;
+    if (int rc = check_qws(n_nodes, 0, L, d_ws, ws_bytes, l, "nl_devoctree_preorder")) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int N = (int)n_nodes;
+    uint64_t *ka = at<uint64_t>(d_ws, l.pk_a), *kb = at<uint64_t>(d_ws, l.pk_b);
+    uint32_t *va = at<uint32_t>(d_ws, l.pv_a), *vb = at<uint32_t>(d_ws, l.pv_b);
+    k_pre_init<<<nl_div_up(N, kThreads), kThreads, 0, s>>>(N, d_code, ka, va);
+    NL_CHECK_LAUNCH("nl_devoctree_preorder");
+    cub::DoubleBuffer<uint64_t> dk(ka, kb);
+    cub::DoubleBuffer<uint32_t> dv(va, vb);
+    size_t tb = l.tmp_bytes;
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(at<void>(d_ws, l.tmp), tb, dk, dv, N, 0, 3 * L, s);   // stable: equal codes keep id order
+    if (e != cudaSuccess) return cuda_fail("nl_devoctree_preorder: sort", e);
+    const uint32_t *order = dv.Current();
+    if (!leaves_only) {
+        k_pre_rows<<<nl_div_up(N, kThreads), kThreads, 0, s>>>(N, (int)grid_dim, order, d_code, d_level, d_out);
+        NL_CHECK_LAUNCH("nl_devoctree_preorder");
+        return NL_OK;
+    }
+    uint8_t *flag = at<uint8_t>(d_ws, l.pflag);
+    uint32_t *sel = at<uint32_t>(d_ws, l.psel);
+    k_pre_flag<<<nl_div_up(N, kThreads), kThreads, 0, s>>>(N, order, d_type, flag);
+    NL_CHECK_LAUNCH("nl_devoctree_preorder");
+    tb = l.tmp_bytes;
+    if ((e = cub::DeviceSelect::Flagged(at<void>(d_ws, l.tmp), tb, order, flag, sel, d_count, N, s)) != cudaSuccess)   // keeps the order
+        return cuda_fail("nl_devoctree_preorder: select", e);
+    k_leaf_rows<<<nl_div_up(N, kThreads), kThreads, 0, s>>>(N, sel, d_count, d_code, d_out);
+    NL_CHECK_LAUNCH("nl_devoctree_preorder");
+    return NL_OK;
+}
+
+int nl_devoctree_try_insert(int64_t grid_dim, const int32_t *d_child, const int32_t *d_vox, int64_t n, void *d_ws, int64_t ws_bytes,
+                            int64_t *d_out, void *stream) {
+    const int L = levels_of(grid_dim);
+    if (L < 0) return nl_set_error("nl_devoctree_try_insert: grid_dim must be a power of two in [2, 2^20]");
+    if (n < 1 || n > kMaxPoints) return nl_set_error("nl_devoctree_try_insert: n must be in [1, 2^23]");
+    if (!d_child || !d_vox || !d_ws || !d_out) return nl_set_error("nl_devoctree_try_insert: null pointer");
+    QueryLayout l;
+    if (int rc = check_qws(0, n, L, d_ws, ws_bytes, l, "nl_devoctree_try_insert")) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int P = (int)(8 * n);
+    cudaError_t e = cudaMemsetAsync(d_out, 0, 2 * sizeof(int64_t), s);
+    if (e != cudaSuccess) return cuda_fail("nl_devoctree_try_insert", e);
+    uint64_t *ka = at<uint64_t>(d_ws, l.tk_a), *kb = at<uint64_t>(d_ws, l.tk_b);
+    k_try_keys<<<nl_div_up(P, kThreads), kThreads, 0, s>>>(P, d_vox, ka);
+    NL_CHECK_LAUNCH("nl_devoctree_try_insert");
+    cub::DoubleBuffer<uint64_t> dk(ka, kb);
+    size_t tb = l.tmp_bytes;
+    if ((e = cub::DeviceRadixSort::SortKeys(at<void>(d_ws, l.tmp), tb, dk, P, 0, 63, s)) != cudaSuccess)
+        return cuda_fail("nl_devoctree_try_insert: sort", e);
+    k_try_match<<<nl_div_up(P, kThreads), kThreads, 0, s>>>(P, L, (int)grid_dim, d_child, dk.Current(), dk.Alternate(), d_out);
+    NL_CHECK_LAUNCH("nl_devoctree_try_insert");
+    dk.selector ^= 1;                                // sort the matched keys' low words (bit 32 set = no match)
+    tb = l.tmp_bytes;
+    if ((e = cub::DeviceRadixSort::SortKeys(at<void>(d_ws, l.tmp), tb, dk, P, 0, 33, s)) != cudaSuccess)
+        return cuda_fail("nl_devoctree_try_insert: sort", e);
+    k_try_distinct<<<nl_div_up(P, kThreads), kThreads, 0, s>>>(P, dk.Current(), d_out);
+    NL_CHECK_LAUNCH("nl_devoctree_try_insert");
     return NL_OK;
 }
 

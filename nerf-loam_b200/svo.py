@@ -180,19 +180,26 @@ class DeviceOctree:
     the capacity-doubling node arrays).  Unlike the host tree, a batch with a coordinate outside [0, grid_dim-2] is rejected as a
     whole (NerfLoamError) and leaves the tree unchanged.  `export_map` returns CPU tensors like `Octree.export_map`;
     `export_dirty` (numpy, like the host) and `update_map` (straight into a MapUpdater's device buffers) export the rows changed
-    since the last dirty export.  try_insert, get_voxels, get_leaf_voxels, get_centres_and_children and pickling are not
-    implemented and raise."""
+    since the last dirty export.  `get_centres_and_children`, `get_voxels` and `get_leaf_voxels` return the host tree's CPU
+    tensors; `try_insert` takes CPU or CUDA input and reads back 16 bytes.
+
+    Pickling (and so deepcopy and torch.save) stores the init arguments and the node arrays as CPU arrays, 42 bytes per node, not
+    the inserted points, and restores onto the current CUDA device.  A restored tree is in the state of a restored host tree:
+    every row is dirty, so the next `export_dirty` returns all of them, and later inserts and exports equal the host tree's.  It
+    has no embedding-row state, so `update_map` refuses it (a MapUpdater builds its own tree)."""
 
     def __init__(self, device="cuda"):
         self.device = torch.device(device)
         self._init_args = None
         self._counts = None
+        self._restored = False
 
     def init(self, grid_dim, feat_dim, voxel_size):
         gd = int(grid_dim)
         if gd < 2 or gd > (1 << 20) or gd & (gd - 1):
             raise _capi.NerfLoamError("DeviceOctree.init: grid_dim must be a power of two in [2, 2^20]")
         self._init_args = (gd, int(feat_dim), float(voxel_size))
+        self._restored = False
         self._cap = 0
         self._n = 1                     # the root, id 0 (octree.cpp:41-43)
         self._grow(4096)
@@ -201,6 +208,7 @@ class DeviceOctree:
         self._list = torch.full((1024,), _NONE_U32, dtype=torch.int32, device=self.device)
         self._list_used = 0
         self._counts = torch.zeros(8, dtype=torch.int64, device=self.device)
+        self._qcounts = torch.zeros(2, dtype=torch.int64, device=self.device)   # the queries' read-back block
         self._ws = torch.empty(0, dtype=torch.uint8, device=self.device)
         self._ids = torch.empty(1024, dtype=torch.int32, device=self.device)
 
@@ -226,13 +234,23 @@ class DeviceOctree:
         self._child, self._code, self._type, self._level, self._scratch = new
         self._cap = cap
 
-    def _workspace(self, n_points):
-        nb = int(_capi.lib().nl_devoctree_workspace_bytes(int(n_points), self.grid_dim))
+    def _workspace(self, n_points, query_nodes=None):
+        """The workspace of an insert / export of n_points, or with query_nodes given, of a query over that many nodes."""
+        L = _capi.lib()
+        if query_nodes is None:
+            nb = int(L.nl_devoctree_workspace_bytes(int(n_points), self.grid_dim))
+        else:
+            nb = int(L.nl_devoctree_query_workspace_bytes(int(query_nodes), int(n_points), self.grid_dim))
         if nb < 0:
-            raise _capi.NerfLoamError(_capi.lib().nl_last_error().decode())
+            raise _capi.NerfLoamError(L.nl_last_error().decode())
         if nb > self._ws.numel():
             self._ws = torch.empty(nb, dtype=torch.uint8, device=self.device)
         return self._ws
+
+    def _check_query(self):
+        if self.device.type != "cuda":
+            raise NotImplementedError("DeviceOctree's queries run on a CUDA device; use svo.Octree on the CPU")
+        self._check()
 
     def insert(self, vox):
         self._check()
@@ -344,6 +362,9 @@ class DeviceOctree:
         Reads back the dirty-row count and the new number of embedding rows; returns (ids, m, rows): the first m entries of
         ids (device) are the dirty node ids."""
         self._check()
+        if self._restored:
+            raise _capi.NerfLoamError("DeviceOctree.update_map: an unpickled tree has no embedding-row state to continue from; "
+                                      "a MapUpdater builds its own tree")
         rows, pts = self._dirty_ids()
         self._export(rows, self._ids, _at(self._counts, 16), False, centres, structure, vertex)
         ws = self._workspace(pts)
@@ -355,13 +376,83 @@ class DeviceOctree:
         m, n_rows = self._counts[2:4].tolist()                      # read-back 2: dirty rows, embedding rows
         return self._ids, m, n_rows
 
-    def _unsupported(self, *a, **k):
-        raise NotImplementedError("DeviceOctree implements insert, the counts, has_voxel and the exports; use svo.Octree for this")
+    def try_insert(self, vox):
+        """Octree.try_insert: the share of the batch's distinct corner keys that are already in the tree (-1.0 for an empty or
+        malformed batch)."""
+        self._check_query()
+        if not isinstance(vox, torch.Tensor):
+            vox = torch.from_numpy(np.ascontiguousarray(vox, dtype=np.int32))
+        if vox.dtype != torch.int32:
+            raise RuntimeError("expected an int32 tensor (the reference accessor<int,2> throws here)")
+        if vox.dim() != 2 or vox.shape[1] != 3 or vox.shape[0] == 0:
+            return -1.0
+        v = vox.detach().to(self.device).contiguous()
+        n = v.shape[0]
+        ws = self._workspace(n, query_nodes=0)
+        _capi.check(_capi.lib().nl_devoctree_try_insert(self.grid_dim, _capi.ptr(self._child), _capi.ptr(v), n, _capi.ptr(ws), ws.numel(),
+                                                        _capi.ptr(self._qcounts), _capi.stream_ptr()), "nl_devoctree_try_insert")
+        _capi.LAUNCHES += 1
+        hits, keys = self._qcounts.tolist()
+        return 1.0 * hits / keys
 
-    try_insert = get_voxels = get_leaf_voxels = get_centres_and_children = _unsupported
+    def _preorder(self, out, leaves_only):
+        ws = self._workspace(0, query_nodes=self._n)
+        _capi.check(_capi.lib().nl_devoctree_preorder(self.grid_dim, self._n, _capi.ptr(self._code), _capi.ptr(self._type),
+                                                      _capi.ptr(self._level), int(leaves_only), _capi.ptr(out), _capi.ptr(self._qcounts),
+                                                      _capi.ptr(ws), ws.numel(), _capi.stream_ptr()), "nl_devoctree_preorder")
+        _capi.LAUNCHES += 1
+
+    def get_voxels(self):
+        """Octree.get_voxels: f32[n,4] (xyz, side) of every node in preorder, on the CPU."""
+        self._check_query()
+        out = torch.empty((self._n, 4), dtype=torch.float32, device=self.device)
+        self._preorder(out, False)
+        return out.cpu()
+
+    def get_leaf_voxels(self):
+        """Octree.get_leaf_voxels: f32[m,3] of the SURFACE leaves in preorder, on the CPU."""
+        self._check_query()
+        out = torch.empty((self._n, 3), dtype=torch.float32, device=self.device)
+        self._preorder(out, True)
+        return out[:int(self._qcounts[0])].cpu()
+
+    def get_centres_and_children(self):
+        """Octree.get_centres_and_children: (voxels f32[n,4], children f32[n,8], features i32[n,8]) on the CPU."""
+        self._check_query()
+        n, d = self._n, self.device
+        voxels = torch.empty((n, 4), dtype=torch.float32, device=d)
+        children = torch.empty((n, 8), dtype=torch.float32, device=d)
+        features = torch.empty((n, 8), dtype=torch.int32, device=d)
+        _capi.check(_capi.lib().nl_devoctree_export_nodes(self.grid_dim, self._init_args[2], n, None, None, 0, _capi.ptr(self._child),
+                                                          _capi.ptr(self._code), _capi.ptr(self._type), _capi.ptr(self._level),
+                                                          _capi.ptr(voxels), _capi.ptr(children), None, None, _capi.ptr(features),
+                                                          _capi.stream_ptr()), "nl_devoctree_export_nodes")
+        _capi.LAUNCHES += 1
+        return voxels.cpu(), children.cpu(), features.cpu()
 
     def get_features(self, pts):
         return None
 
+    _STATE = ("child", "code", "type", "level")
+
     def __getstate__(self):
-        raise NotImplementedError("DeviceOctree cannot be pickled; use svo.Octree")
+        if self._init_args is None:
+            return {"init": None}
+        n = self._n
+        arrays = (self._child, self._code, self._type, self._level)
+        return {"init": self._init_args, **{k: a[:n].cpu().numpy() for k, a in zip(self._STATE, arrays)}}
+
+    def __setstate__(self, state):
+        self.device = torch.device("cuda", torch.cuda.current_device())
+        self._init_args = None
+        self._counts = None
+        self._restored = False
+        if state["init"] is None:
+            return
+        self.init(*state["init"])
+        n = len(state["type"])
+        self._grow(n)
+        for k, a in zip(self._STATE, (self._child, self._code, self._type, self._level)):
+            a[:n].copy_(torch.from_numpy(state[k]))
+        self._n = n                     # _base = 0, no pending entries, scratch at rest: every row is dirty, as after a host replay
+        self._restored = True
