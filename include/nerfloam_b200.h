@@ -87,6 +87,32 @@ NL_API int64_t nl_assign_embedding_rows(const int32_t *h_vertex, int64_t n_nodes
 NL_API int64_t nl_assign_embedding_rows_subset(const int32_t *h_vertex_rows, int64_t n_rows_in, int64_t n_nodes, int32_t *h_vertex2row,
                                         int64_t n_rows_before, int32_t *h_vox2row_rows);
 
+/* Node arrays: the state of a tree, and the layout of a map checkpoint (nerf-loam_b200/mapping.py MapUpdater.state_dict) and of
+ * the device tree (section 1b).  child i32[n][8] (every child, FEATURE ones included; -1 = none), code u64[n] (Morton code of the
+ * min corner truncated to the node's level), type i8[n] (-1 NONLEAF, 0 SURFACE, 1 FEATURE), level u8[n] (side = grid_dim >> level).
+ * Node arrays read from outside the program are checked before any walk of them.  The checks, L = log2(grid_dim), and the bit each
+ * one sets when it fails: */
+#define NL_TREE_ROOT 1       /* n >= 1; node 0 has level 0, code 0 and is NONLEAF                                                    */
+#define NL_TREE_RANGE 2      /* type in {-1, 0, 1}; level <= L; every child id c of node i has i < c < n (parents are created first)  */
+#define NL_TREE_LINK 4       /* level[c] = level[i] + 1 and code[c] = code[i] | s << 3 (L - level[c]) for the child c in slot s;
+                              * no code bits below a node's level                                                                       */
+#define NL_TREE_PARENTS 8    /* every node but the root is the child of exactly one node                                             */
+#define NL_TREE_SHAPE 16     /* NONLEAF <=> level < L; every NONLEAF node has a child                                                 */
+#define NL_TREE_ROWS 32      /* vertex2row in [-1, n_rows); rows only on level-L nodes; every row in [0, n_rows) used exactly once      */
+#define NL_TREE_VERTICES 64  /* the 8 corner leaves of every SURFACE leaf exist; vertex2row[v] >= 0 <=> v is such a corner             */
+/* ROWS and VERTICES walk the tree, so they are evaluated only on a tree that passes the first five checks (otherwise they are 0).
+ * nl_octree_validate returns the OR of the failed checks' bits (0 = well-formed), or < 0 for bad arguments; vertex2row i32[n] may
+ * be NULL (no row checks).  Validation reads every array in O(n) and never follows an id it has not range-checked. */
+NL_API int64_t nl_octree_validate(int64_t grid_dim, int64_t n, const int32_t *h_child, const uint64_t *h_code, const int8_t *h_type,
+                                  const uint8_t *h_level, const int32_t *h_vertex2row, int64_t n_rows);
+/* Copies the tree's node arrays out (n = nl_octree_count_nodes). */
+NL_API int nl_octree_nodes(const nl_octree *t, int32_t *h_child, uint64_t *h_code, int8_t *h_type, uint8_t *h_level);
+/* Replaces the tree of an initialised handle by node arrays in O(n), without replaying points: runs nl_octree_validate (no rows)
+ * first and returns its bits (> 0) without touching the tree if any is set, else NL_OK.  The restored tree has an empty dirty
+ * list and an empty set of seen points (a cache: a repeated point only visits existing nodes and changes nothing). */
+NL_API int nl_octree_restore(nl_octree *t, const int32_t *h_child, const uint64_t *h_code, const int8_t *h_type, const uint8_t *h_level,
+                             int64_t n);
+
 /* ============================================================================================
  * 1b. Device octree -- section 1's insert and the map-update glue around it (Octree::insert octree.cpp:51-111,
  *     Mapping.create_voxels / update_grid_features mapping.py:283-339) on the GPU, bit for bit: the same node ids, types,
@@ -163,6 +189,15 @@ NL_API int nl_devoctree_preorder(int64_t grid_dim, int64_t n_nodes, const uint64
  * in-grid coordinates whose leaf exists; keys are the host's (21 bits per axis), so negative and out-of-grid points alias alike. */
 NL_API int nl_devoctree_try_insert(int64_t grid_dim, const int32_t *d_child, const int32_t *d_vox, int64_t n, void *d_ws, int64_t ws_bytes,
                             int64_t *d_out, void *stream);
+/* nl_octree_validate on the device, for node arrays uploaded from outside the program (a checkpoint, a pickle): d_out i64[2] =
+ * (bits of the first five checks, bits of ROWS / VERTICES); their OR equals nl_octree_validate's result.  A structural pass (one
+ * thread per node and slot; parent counts in the workspace) and a sweep of the parent counts, then, with d_vertex2row i32[n_nodes]
+ * given, a row pass that returns at once unless the structural word is 0, so it never walks a malformed tree, and a sweep of its
+ * counts.  No result depends on the order in which atomics land; no host synchronisation.  Workspace: three arrays of 4 n_nodes bytes, each 256-byte
+ * aligned (nl_devoctree_query_workspace_bytes(n_nodes, 0, grid_dim) covers it). */
+NL_API int nl_devoctree_validate(int64_t grid_dim, int64_t n_nodes, const int32_t *d_child, const uint64_t *d_code, const int8_t *d_type,
+                                 const uint8_t *d_level, const int32_t *d_vertex2row, int64_t n_rows, void *d_ws, int64_t ws_bytes,
+                                 int64_t *d_out, void *stream);
 
 /* ============================================================================================
  * 2. Drop-ins for the two live `grid` kernels (third_party/sparse_voxels/src/binding.cpp:12-20)

@@ -68,6 +68,10 @@ _SIGNATURES = {
     "nl_octree_export_dirty": (C.c_int, [vp, vp, vp, vp, vp, C.c_int]),
     "nl_assign_embedding_rows_subset": (C.c_int64, [vp, C.c_int64, C.c_int64, vp, C.c_int64, vp]),
     "nl_octree_pack_children_rows": (C.c_int, [C.c_int32, vp, vp, vp, vp, vp]),
+    "nl_octree_validate": (C.c_int64, [C.c_int64, C.c_int64, vp, vp, vp, vp, vp, C.c_int64]),
+    "nl_octree_nodes": (C.c_int, [vp, vp, vp, vp, vp]),
+    "nl_octree_restore": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64]),
+    "nl_devoctree_validate": (C.c_int, [C.c_int64, C.c_int64, vp, vp, vp, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
     "nl_devoctree_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
     "nl_devoctree_insert_count": (C.c_int, [C.c_int64, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
     "nl_devoctree_insert_commit": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int64, vp, C.c_int64, vp, vp]),
@@ -130,6 +134,13 @@ _SIGNATURES = {
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)
 CTL_ERROR, CTL_SKIPPED, CTL_SKIP_NOW, CTL_ADAM_STEP, CTL_MIN_HIT, CTL_ITERS, CTL_MAX_SAMPLES, CTL_WORDS = 0, 1, 2, 3, 4, 5, 6, 8
 STATS_PACK_FIXED = 10
+# node-array checks, bit i = 1 << i (NL_TREE_* in include/nerfloam_b200.h section 1)
+TREE_CHECKS = ("ROOT", "RANGE", "LINK", "PARENTS", "SHAPE", "ROWS", "VERTICES")
+
+
+def tree_checks_failed(bits):
+    """The names of the NL_TREE_* checks whose bits are set."""
+    return [name for i, name in enumerate(TREE_CHECKS) if bits >> i & 1]
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))
 

@@ -531,6 +531,107 @@ __global__ void k_try_distinct(int P, const uint64_t *__restrict__ low, int64_t 
     if (threadIdx.x == 0 && c) atomicAdd((unsigned long long *)&out[0], (unsigned long long)c);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Validation of uploaded node arrays (nl_octree_validate in octree_host.cpp, check for check).  Every block ORs its bits into one
+// word, so the verdict is independent of the order in which blocks and atomics land.
+__device__ __forceinline__ void or_bits(int bits, unsigned long long *word) {
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    __shared__ int block_bits;
+    if (threadIdx.x == 0) block_bits = 0;
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0 && bits) atomicOr(&block_bits, bits);
+    __syncthreads();
+    if (threadIdx.x == 0 && block_bits) atomicOr(word, (unsigned long long)block_bits);
+}
+
+// one thread per (node i, slot s): the child id's range before anything is read at it, the link to the child, its parent count;
+// slot 0 also checks the node's own fields
+__global__ void k_val_tree(int64_t N, int L, const int32_t *__restrict__ child, const uint64_t *__restrict__ code, const int8_t *__restrict__ type,
+                           const uint8_t *__restrict__ level, int32_t *parents, int64_t *out) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = t < 8 * N;
+    const int64_t i = t >> 3;
+    const int s = (int)(t & 7);
+    int bits = 0;
+    bool has = false;
+    if (live) {
+        const int64_t c = child[t];
+        has = c != -1;
+        if (has) {
+            if (c <= i || c >= N) {
+                bits |= NL_TREE_RANGE;
+            } else {
+                atomicAdd(&parents[c], 1);
+                const int lc = level[c], lv = level[i];
+                if (lc != lv + 1 || lc > L) bits |= NL_TREE_LINK;
+                else if (code[c] != (code[i] | (uint64_t)s << (3 * (L - lc)))) bits |= NL_TREE_LINK;
+            }
+        }
+    }
+    const unsigned any = __ballot_sync(0xffffffffu, has);            // blockDim % 32 == 0: a node's 8 slots share a warp
+    if (live && s == 0) {
+        const int ty = type[i], lv = level[i];
+        if (i == 0 && (lv != 0 || code[0] != 0 || ty != kNonLeaf)) bits |= NL_TREE_ROOT;
+        if (ty < kNonLeaf || ty > kFeature || lv > L) {
+            bits |= NL_TREE_RANGE;
+        } else {
+            const bool has_child = (any >> (threadIdx.x & 24)) & 0xffu;
+            if (code[i] & ((uint64_t(1) << (3 * (L - lv))) - 1)) bits |= NL_TREE_LINK;
+            if ((ty == kNonLeaf) != (lv < L) || (ty == kNonLeaf && !has_child)) bits |= NL_TREE_SHAPE;
+        }
+    }
+    if (t == 0 && N < 1) bits |= NL_TREE_ROOT;
+    or_bits(bits, (unsigned long long *)&out[0]);
+}
+
+__global__ void k_val_parents(int64_t N, const int32_t *__restrict__ parents, int64_t *out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    or_bits(i >= 1 && i < N && parents[i] != 1 ? NL_TREE_PARENTS : 0, (unsigned long long *)&out[0]);
+}
+
+// rows and vertices, on a tree the structural pass found well-formed: a SURFACE node is then a level-L leaf with in-grid
+// coordinates, and find_node's walk is bounded by L levels of range-checked ids
+__global__ void k_val_rows(int64_t N, int L, int size, const int32_t *__restrict__ child, const uint64_t *__restrict__ code,
+                           const int8_t *__restrict__ type, const uint8_t *__restrict__ level, const int32_t *__restrict__ v2r, int64_t n_rows,
+                           int32_t *uses, int32_t *referenced, int64_t *out) {
+    if (*(volatile int64_t *)&out[0] != 0) return;                // the structural verdict: never walk a malformed tree
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int bits = 0;
+    if (i < N) {
+        const int32_t r = v2r[i];
+        if (r < -1 || r >= n_rows) {
+            bits |= NL_TREE_ROWS;
+        } else if (r >= 0) {
+            if (level[i] != L) bits |= NL_TREE_ROWS;
+            if (r < N) atomicAdd(&uses[r], 1);
+        }
+        if (type[i] == kSurface) {
+            const uint64_t c = code[i];
+            const int x = (int)squeeze3(c), y = (int)squeeze3(c >> 1), z = (int)squeeze3(c >> 2);
+            for (int k = 0; k < 8; ++k) {
+                const int cx = x + (k >> 2), cy = y + ((k >> 1) & 1), cz = z + (k & 1);
+                const int v = (cx < size && cy < size && cz < size) ? find_node(child, L, size, cx, cy, cz) : -1;
+                if (v < 0) bits |= NL_TREE_VERTICES;
+                else referenced[v] = 1;                                 // idempotent store
+            }
+        }
+    }
+    if (i == 0 && n_rows > N) bits |= NL_TREE_ROWS;                  // a row per node at most
+    or_bits(bits, (unsigned long long *)&out[1]);
+}
+
+__global__ void k_val_rows_sweep(int64_t N, const int32_t *__restrict__ v2r, int64_t n_rows, const int32_t *__restrict__ uses,
+                                 const int32_t *__restrict__ referenced, int64_t *out) {
+    if (*(volatile int64_t *)&out[0] != 0) return;
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int bits = 0;
+    if (i < N) {
+        if (i < n_rows && uses[i] != 1) bits |= NL_TREE_ROWS;
+        if ((v2r[i] >= 0) != (referenced[i] != 0)) bits |= NL_TREE_VERTICES;
+    }
+    or_bits(bits, (unsigned long long *)&out[1]);
+}
+
 // Query workspace: the preorder of N nodes and try_insert of n points (P = 8n corner keys) each use it from offset 0; the CUB
 // scratch follows the larger of the two.  The arrays are pure arithmetic, so a short workspace is rejected before any CUDA call.
 struct QueryLayout {
@@ -828,6 +929,40 @@ int nl_devoctree_try_insert(int64_t grid_dim, const int32_t *d_child, const int3
         return cuda_fail("nl_devoctree_try_insert: sort", e);
     k_try_distinct<<<nl_div_up(P, kThreads), kThreads, 0, s>>>(P, dk.Current(), d_out);
     NL_CHECK_LAUNCH("nl_devoctree_try_insert");
+    return NL_OK;
+}
+
+int nl_devoctree_validate(int64_t grid_dim, int64_t n_nodes, const int32_t *d_child, const uint64_t *d_code, const int8_t *d_type,
+                          const uint8_t *d_level, const int32_t *d_vertex2row, int64_t n_rows, void *d_ws, int64_t ws_bytes, int64_t *d_out,
+                          void *stream) {
+    const int L = levels_of(grid_dim);
+    if (L < 0) return nl_set_error("nl_devoctree_validate: grid_dim must be a power of two in [2, 2^20]");
+    if (n_nodes < 0 || n_nodes > INT32_MAX || n_rows < 0) return nl_set_error("nl_devoctree_validate: bad sizes");
+    if (!d_out || (n_nodes > 0 && (!d_child || !d_code || !d_type || !d_level || !d_ws))) return nl_set_error("nl_devoctree_validate: null pointer");
+    size_t need = 0;
+    const size_t parents = take(need, 4 * (size_t)n_nodes), uses = take(need, 4 * (size_t)n_nodes), referenced = take(need, 4 * (size_t)n_nodes);
+    if (n_nodes > 0 && ws_bytes < (int64_t)need) {
+        char buf[160];
+        std::snprintf(buf, sizeof(buf), "nl_devoctree_validate: workspace of %lld bytes, needs %lld", (long long)ws_bytes, (long long)need);
+        return nl_set_error(buf);
+    }
+    if (((uintptr_t)d_ws & 255u) != 0) return nl_set_error("nl_devoctree: the workspace must be 256-byte aligned");
+    cudaStream_t s = (cudaStream_t)stream;
+    cudaError_t e = cudaMemsetAsync(d_out, 0, 2 * sizeof(int64_t), s);
+    if (e == cudaSuccess && n_nodes > 0) e = cudaMemsetAsync(d_ws, 0, need, s);
+    if (e != cudaSuccess) return cuda_fail("nl_devoctree_validate", e);
+    const int64_t nb = nl_div_up(std::max<int64_t>(8 * n_nodes, 1), kThreads);
+    k_val_tree<<<nb, kThreads, 0, s>>>(n_nodes, L, d_child, d_code, d_type, d_level, at<int32_t>(d_ws, parents), d_out);
+    if (n_nodes > 0) {
+        const int64_t blocks = nl_div_up(n_nodes, kThreads);
+        k_val_parents<<<blocks, kThreads, 0, s>>>(n_nodes, at<int32_t>(d_ws, parents), d_out);
+        if (d_vertex2row) {
+            k_val_rows<<<blocks, kThreads, 0, s>>>(n_nodes, L, (int)grid_dim, d_child, d_code, d_type, d_level, d_vertex2row, n_rows,
+                                                   at<int32_t>(d_ws, uses), at<int32_t>(d_ws, referenced), d_out);
+            k_val_rows_sweep<<<blocks, kThreads, 0, s>>>(n_nodes, d_vertex2row, n_rows, at<int32_t>(d_ws, uses), at<int32_t>(d_ws, referenced), d_out);
+        }
+    }
+    NL_CHECK_LAUNCH("nl_devoctree_validate");
     return NL_OK;
 }
 

@@ -10,6 +10,7 @@
 // the reference's get_centres_and_children().  Duplicate points are skipped through a hash set: a
 // repeated point can neither create a node nor change a type, so skipping it is exact.
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -89,6 +90,18 @@ struct KeySet {
     }
 };
 
+int32_t find_in(const int32_t *child, int size, int max_level, int x, int y, int z) {  // find_octant, octree.cpp:151-171
+    int32_t n = 0;
+    unsigned edge = (unsigned)size / 2;
+    for (int d = 1; d <= max_level; edge /= 2, ++d) {
+        int slot = ((x & edge) > 0) + 2 * ((y & edge) > 0) + 4 * ((z & edge) > 0);
+        int32_t c = child[(size_t)n * 8 + slot];
+        if (c < 0) return -1;
+        n = c;
+    }
+    return n;
+}
+
 }  // namespace
 
 struct nl_octree {
@@ -120,17 +133,7 @@ struct nl_octree {
         mark(id);
         return id;
     }
-    int32_t find(int x, int y, int z) const {  // find_octant, octree.cpp:151-171
-        int32_t n = 0;
-        unsigned edge = (unsigned)size / 2;
-        for (int d = 1; d <= max_level; edge /= 2, ++d) {
-            int slot = ((x & edge) > 0) + 2 * ((y & edge) > 0) + 4 * ((z & edge) > 0);
-            int32_t c = child[(size_t)n * 8 + slot];
-            if (c < 0) return -1;
-            n = c;
-        }
-        return n;
-    }
+    int32_t find(int x, int y, int z) const { return find_in(child.data(), size, max_level, x, y, z); }
 };
 
 extern "C" {
@@ -340,6 +343,99 @@ int64_t nl_assign_embedding_rows_subset(const int32_t *vertex_rows, int64_t n_ro
         vox2row_rows[i] = (v >= 0 && v < n_nodes) ? vertex2row[v] : -1;
     }
     return n_rows;
+}
+
+// Node-array validation (header section 1, NL_TREE_*).  csrc/octree_dev.cu nl_devoctree_validate restates it check for check; the
+// two must set the same bits for every input.
+int64_t nl_octree_validate(int64_t grid_dim, int64_t n, const int32_t *child, const uint64_t *code, const int8_t *type, const uint8_t *level,
+                           const int32_t *vertex2row, int64_t n_rows) {
+    if (grid_dim < 2 || grid_dim > (1 << 20) || (grid_dim & (grid_dim - 1))) return nl_set_error("nl_octree_validate: grid_dim must be a power of two in [2, 2^20]");
+    if (n < 0 || n > INT32_MAX || n_rows < 0) return nl_set_error("nl_octree_validate: bad sizes");
+    if (n > 0 && (!child || !code || !type || !level)) return nl_set_error("nl_octree_validate: null pointer");
+    if (n == 0) return NL_TREE_ROOT;
+    int L = 0;
+    while ((int64_t(1) << L) < grid_dim) ++L;
+    int64_t bits = 0;
+    if (level[0] != 0 || code[0] != 0 || type[0] != kNonLeaf) bits |= NL_TREE_ROOT;
+    std::vector<int32_t> parents((size_t)n, 0);
+    for (int64_t i = 0; i < n; ++i) {
+        const int t = type[i], lv = level[i];
+        bool has_child = false;
+        for (int s = 0; s < 8; ++s) {
+            const int64_t c = child[i * 8 + s];
+            if (c == -1) continue;
+            has_child = true;
+            if (c <= i || c >= n) { bits |= NL_TREE_RANGE; continue; }   // never read at an unchecked id
+            ++parents[(size_t)c];
+            const int lc = level[c];
+            if (lc != lv + 1 || lc > L) bits |= NL_TREE_LINK;
+            else if (code[c] != (code[i] | (uint64_t)s << (3 * (L - lc)))) bits |= NL_TREE_LINK;
+        }
+        const bool t_ok = t >= kNonLeaf && t <= kFeature;
+        if (!t_ok || lv > L) { bits |= NL_TREE_RANGE; continue; }
+        if (code[i] & ((uint64_t(1) << (3 * (L - lv))) - 1)) bits |= NL_TREE_LINK;
+        if ((t == kNonLeaf) != (lv < L) || (t == kNonLeaf && !has_child)) bits |= NL_TREE_SHAPE;
+    }
+    for (int64_t i = 1; i < n; ++i)
+        if (parents[(size_t)i] != 1) bits |= NL_TREE_PARENTS;
+    if (bits || !vertex2row) return bits;
+    // rows: the tree is well-formed, so a SURFACE node is a level-L leaf with in-grid coordinates and find() stays in the tree
+    const int size = (int)grid_dim;
+    std::vector<int32_t> uses((size_t)std::min(n_rows, n), 0);
+    std::vector<uint8_t> referenced((size_t)n, 0);
+    if (n_rows > n) bits |= NL_TREE_ROWS;                          // a row per node at most
+    for (int64_t i = 0; i < n; ++i) {
+        const int32_t r = vertex2row[i];
+        if (r < -1 || r >= n_rows) bits |= NL_TREE_ROWS;
+        else if (r >= 0) {
+            if (level[i] != L) bits |= NL_TREE_ROWS;
+            if (r < n) ++uses[(size_t)r];
+        }
+        if (type[i] != kSurface) continue;
+        const int x = (int)squeeze3(code[i]), y = (int)squeeze3(code[i] >> 1), z = (int)squeeze3(code[i] >> 2);
+        for (int k = 0; k < 8; ++k) {
+            const int cx = x + kIncX[k], cy = y + kIncY[k], cz = z + kIncZ[k];
+            const int32_t v = (cx < size && cy < size && cz < size) ? find_in(child, size, L, cx, cy, cz) : -1;
+            if (v < 0) bits |= NL_TREE_VERTICES;
+            else referenced[(size_t)v] = 1;
+        }
+    }
+    for (size_t r = 0; r < uses.size(); ++r)
+        if (uses[r] != 1) bits |= NL_TREE_ROWS;
+    for (int64_t i = 0; i < n; ++i)
+        if ((vertex2row[i] >= 0) != (referenced[(size_t)i] != 0)) bits |= NL_TREE_VERTICES;
+    return bits;
+}
+
+int nl_octree_nodes(const nl_octree *t, int32_t *child, uint64_t *code, int8_t *type, uint8_t *level) {
+    if (!t || !child || !code || !type || !level) return nl_set_error("nl_octree_nodes: null argument");
+    const size_t n = t->type.size();
+    std::memcpy(child, t->child.data(), n * 8 * sizeof(int32_t));
+    std::memcpy(code, t->code.data(), n * sizeof(uint64_t));
+    std::memcpy(type, t->type.data(), n);
+    for (size_t i = 0; i < n; ++i) level[i] = (uint8_t)(t->max_level - __builtin_ctz(t->side[i]));   // side = grid_dim >> level
+    return NL_OK;
+}
+
+int nl_octree_restore(nl_octree *t, const int32_t *child, const uint64_t *code, const int8_t *type, const uint8_t *level, int64_t n) {
+    if (!t || n < 0) return nl_set_error("nl_octree_restore: bad arguments");
+    const int64_t bits = nl_octree_validate(t->size, n, child, code, type, level, nullptr, 0);
+    if (bits != 0) return (int)bits;                              // < 0: bad arguments; > 0: the failed checks, tree untouched
+    t->child.assign(child, child + n * 8);
+    t->code.assign(code, code + n);
+    t->type.assign(type, type + n);
+    t->side.resize((size_t)n);
+    t->corner_keys = KeySet();
+    for (int64_t i = 0; i < n; ++i) {
+        t->side[(size_t)i] = (uint32_t)t->size >> level[i];
+        if (level[i] == t->max_level) t->corner_keys.insert(code[i]);   // the corner keys are exactly the level-L codes
+    }
+    t->dirty.clear();
+    t->dirty_flag.assign((size_t)n, 0);
+    // seen_points is a cache of inserted points: a repeated point only visits existing nodes and changes nothing, so the restored
+    // tree starts with an empty one and inserts exactly like the tree it was saved from.
+    t->seen_points = KeySet();
+    return NL_OK;
 }
 
 }  // extern "C"

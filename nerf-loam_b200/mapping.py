@@ -19,7 +19,7 @@ import torch
 
 from . import _capi
 from .engine import MapState
-from .svo import DeviceOctree, Octree
+from .svo import DeviceOctree, Octree, malformed_tree, validate_nodes
 
 
 class _LazyMapStates(dict):
@@ -143,6 +143,101 @@ class MapUpdater:
     def vertex2row(self, v):
         self._vertex2row = v
 
+    # -- checkpoints ------------------------------------------------------------------------------------------------------------
+    FORMAT = 1
+
+    def state_dict(self):
+        """The map as a plain dict of CPU tensors and Python scalars (loads with torch.load(..., weights_only=True)):
+        format, grid_dim, embed_dim, voxel_size, init_std, generation; generator (the CPU generator's state, so rows drawn with
+        init_std > 0 continue the same stream); the tree as node arrays child i32[n,8], code i64[n] (u64 bit pattern), type i8[n],
+        level u8[n]; vertex2row i32[n] and embeddings bf16[n_rows,16] (the current, trained values).  Host and device trees give
+        equal dicts for the same insert history.  Raises NerfLoamError if the tree holds inserts not yet applied to the map
+        (svo.insert without update_grid_features): such a map could not continue bit for bit."""
+        n = self.n_nodes
+        if self.svo.is_dirty() or self.svo.count_nodes() != n:
+            raise _capi.NerfLoamError("MapUpdater.state_dict: the octree has inserts that were not applied to the map yet; "
+                                      "call update_grid_features() first")
+        child, code, type_, level = self.svo.export_nodes()
+        gd, _, _ = self.svo._init_args
+        return {"format": self.FORMAT, "grid_dim": int(gd), "embed_dim": int(self._emb_buf.shape[1]), "voxel_size": self.voxel_size,
+                "init_std": float(self.init_std), "generation": int(self.generation), "generator": self._gen.get_state(),
+                "child": child, "code": code, "type": type_, "level": level,
+                "vertex2row": torch.from_numpy(np.array(self.vertex2row[:n], dtype=np.int32)),
+                "embeddings": self.embeddings.detach().to("cpu", copy=True)}
+
+    _STATE_DTYPES = {"child": torch.int32, "code": torch.int64, "type": torch.int8, "level": torch.uint8, "vertex2row": torch.int32,
+                     "embeddings": torch.bfloat16, "generator": torch.uint8}
+
+    @classmethod
+    def _check_state(cls, sd):
+        """The checks of a checkpoint that need no tree walk; the names of the failed ones."""
+        if not isinstance(sd, dict):
+            return ["a dict"]
+        missing = [k for k in ("format", "grid_dim", "embed_dim", "voxel_size", "init_std", "generation", *cls._STATE_DTYPES) if k not in sd]
+        if missing:
+            return ["keys " + ", ".join(missing)]
+        bad = []
+        if sd["format"] != cls.FORMAT:
+            bad.append(f"format {sd['format']!r} (this version reads {cls.FORMAT})")
+        gd = sd["grid_dim"]
+        if not isinstance(gd, int) or gd < 2 or gd > 1 << 20 or gd & (gd - 1):
+            bad.append("grid_dim a power of two in [2, 2^20]")
+        if sd["embed_dim"] != 16:
+            bad.append("embed_dim 16")
+        for k, dt in cls._STATE_DTYPES.items():
+            if not isinstance(sd[k], torch.Tensor) or sd[k].dtype != dt or sd[k].device.type != "cpu":
+                bad.append(f"{k} a CPU {dt} tensor")
+        if bad:
+            return bad
+        n = sd["type"].shape[0]
+        shapes = {"child": (n, 8), "code": (n,), "type": (n,), "level": (n,), "vertex2row": (n,)}
+        bad += [f"{k} of shape {list(s)}" for k, s in shapes.items() if tuple(sd[k].shape) != s]
+        if sd["embeddings"].dim() != 2 or sd["embeddings"].shape[1] != 16:
+            bad.append("embeddings of shape [n_rows, 16]")
+        return bad
+
+    @classmethod
+    def from_state_dict(cls, sd, device="cuda", octree="host", incremental=True, reserve_nodes=0, reserve_rows=0):
+        """A new MapUpdater holding the map of `sd` (state_dict()), on either octree whichever tree saved it.  The node arrays and
+        the row table are checked (the NL_TREE_* checks of include/nerfloam_b200.h) before anything walks them: a malformed
+        checkpoint raises NerfLoamError naming the failed checks.  The buffers, host mirrors, vertex2row, embeddings and map_states
+        equal the saved updater's, the tree is clean, and every later create_voxels gives what the saved updater would have given.
+        With octree="device" each checkpoint array is copied to the device once and 16 bytes come back."""
+        bad = cls._check_state(sd)
+        if bad:
+            raise _capi.NerfLoamError("MapUpdater.from_state_dict: malformed checkpoint, failed checks: " + "; ".join(bad))
+        n, n_rows = sd["type"].shape[0], sd["embeddings"].shape[0]
+        nodes = tuple(sd[k].contiguous() for k in ("child", "code", "type", "level"))
+        v2r = sd["vertex2row"].contiguous()
+        mu = cls(sd["voxel_size"], sd["embed_dim"], sd["grid_dim"], device=device, init_std=sd["init_std"], incremental=incremental,
+                 reserve_nodes=max(int(reserve_nodes), n), reserve_rows=max(int(reserve_rows), n_rows), octree=octree)
+        mu._gen.set_state(sd["generator"])
+        mu._emb_buf[:n_rows].copy_(sd["embeddings"])
+        mu.n_rows = n_rows
+        if mu.on_device:
+            mu._v2r[:n].copy_(v2r)
+            mu.svo.load_nodes(*nodes, vertex2row=mu._v2r, n_rows=n_rows)
+            mu.svo.rebuild_map(mu._centres, mu._structure, mu._vertex, mu._v2r, mu._vox2row, n_rows)
+            _capi.check(_capi.lib().nl_octree_pack_children(n, _capi.ptr(mu._centres), _capi.ptr(mu._structure), _capi.ptr(mu._packed),
+                                                            _capi.stream_ptr()), "nl_octree_pack_children")
+            _capi.LAUNCHES += 1
+            mu.n_nodes = n
+            mu._publish_device()
+        else:
+            bits = validate_nodes(sd["grid_dim"], *nodes, v2r, n_rows)
+            if bits:
+                raise malformed_tree("MapUpdater.from_state_dict", bits)
+            mu.svo.load_nodes(*nodes)
+            mu.vertex2row = v2r.numpy().copy()
+            if mu.incremental:
+                c, s, v = (t.numpy() for t in mu.svo.export_map())
+                mu._apply_rows(np.arange(n, dtype=np.int32), c, s, v)
+                mu._publish_host()
+            else:
+                mu._update_full()
+        mu.generation = sd["generation"]
+        return mu
+
     def create_voxels(self, points, pose):
         """mapping.py:283-291: sensor-frame points [N,3] + 4x4 pose -> voxel coordinates -> octree -> map_states."""
         pts = torch.as_tensor(points, dtype=torch.float32, device=self.device)
@@ -208,6 +303,10 @@ class MapUpdater:
         self.n_nodes = n
         self.generation += 1
         self.last_update = {"dirty_rows": int(m), "nodes": int(n), "embedding_rows": int(new_rows)}
+        return self._publish_device()
+
+    def _publish_device(self):
+        n = self.n_nodes
         ms = MapState.__new__(MapState)
         ms.centres, ms.structure, ms.vox2row = self._centres[:n], self._structure[:n], self._vox2row[:n]
         ms.emb = self.embeddings
@@ -223,6 +322,14 @@ class MapUpdater:
 
     def _update_incremental(self):
         ids, c, s, v = self.svo.export_dirty()
+        new_rows = self._apply_rows(ids, c, s, v)
+        self.generation += 1
+        self.last_update = {"dirty_rows": int(ids.shape[0]), "nodes": int(self.n_nodes), "embedding_rows": int(new_rows)}
+        return self._publish_host()
+
+    def _apply_rows(self, ids, c, s, v):
+        """Patches the exported rows ids (ascending) into the device buffers and host mirrors, numbering their new vertices;
+        returns the new number of embedding rows."""
         n = self.svo.count_export_nodes()
         m = ids.shape[0]
         if self.vertex2row.shape[0] < n:
@@ -257,8 +364,10 @@ class MapUpdater:
             self._host = (hc, hs, hv)
         self._host[0][ids], self._host[1][ids], self._host[2][ids] = c, s, v
         self.n_nodes = n
-        self.generation += 1
-        self.last_update = {"dirty_rows": int(m), "nodes": int(n), "embedding_rows": int(new_rows)}
+        return new_rows
+
+    def _publish_host(self):
+        n = self.n_nodes
         ms = MapState.__new__(MapState)
         ms.centres, ms.structure, ms.vox2row = self._centres[:n], self._structure[:n], self._vox2row[:n]
         ms.emb = self.embeddings

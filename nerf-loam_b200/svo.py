@@ -7,7 +7,8 @@ Differences from the reference class, all deliberate:
     instance corrupts its exports);
   * `get_centres_and_children()` is a direct array pass (no per-node torch dispatch);
   * `export_map()` returns the arrays already in the layout the hot path consumes (mapping.py:320-326);
-  * pickling replays the inserted point tensors like the reference (bindings.cpp:23-31) and is wired.
+  * pickling replays the inserted point tensors like the reference (bindings.cpp:23-31) and is wired; a tree restored from node
+    arrays (`load_nodes`), which has no point history, pickles as its node arrays instead.
 """
 import ctypes as C
 
@@ -15,6 +16,26 @@ import numpy as np
 import torch
 
 from . import _capi
+
+
+def _np_ptr(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
+def validate_nodes(grid_dim, child, code, type_, level, vertex2row=None, n_rows=0):
+    """nl_octree_validate on CPU node arrays (child i32[n,8], code i64[n], type i8[n], level u8[n], vertex2row i32[n] or None):
+    the OR of the failed NL_TREE_* checks' bits, 0 for a well-formed tree (_capi.tree_checks_failed names them)."""
+    a = [np.ascontiguousarray(t.numpy() if isinstance(t, torch.Tensor) else t) for t in (child, code, type_, level)]
+    v = None if vertex2row is None else np.ascontiguousarray(vertex2row.numpy() if isinstance(vertex2row, torch.Tensor) else vertex2row)
+    n = a[2].shape[0]
+    bits = int(_capi.lib().nl_octree_validate(int(grid_dim), n, *(_np_ptr(x) for x in a), None if v is None else _np_ptr(v), int(n_rows)))
+    if bits < 0:
+        raise _capi.NerfLoamError(_capi.lib().nl_last_error().decode())
+    return bits
+
+
+def malformed_tree(what, bits):
+    return _capi.NerfLoamError(f"{what}: malformed octree state, failed checks: {', '.join(_capi.tree_checks_failed(bits))}")
 
 
 def encode(x, y, z):
@@ -25,7 +46,7 @@ def encode(x, y, z):
 class Octree:
     def __init__(self):
         self._h = None
-        self._all_pts = []
+        self._all_pts = []              # None: restored from node arrays, no point history
         self._init_args = None
 
     # -- bindings.cpp:14 init(grid_dim, feat_dim, voxel_size)
@@ -59,7 +80,8 @@ class Octree:
             print(f"Point dimensions mismatch: inputs are {v.shape[-1]} expect 3")  # octree.cpp:62-66
             return
         _capi.check(_capi.lib().nl_octree_insert(self._h, v.ctypes.data_as(C.c_void_p), v.shape[0]), "nl_octree_insert")
-        self._all_pts.append(torch.from_numpy(v.copy()))
+        if self._all_pts is not None:
+            self._all_pts.append(torch.from_numpy(v.copy()))
 
     def try_insert(self, vox):
         self._check()
@@ -142,8 +164,44 @@ class Octree:
         self._check()
         return int(_capi.lib().nl_octree_count_export_nodes(self._h))
 
-    # -- pickle (bindings.cpp:23-31): state = (size, feat_dim, voxel_size, all inserted tensors), replayed on load
+    def is_dirty(self):
+        """True if rows changed since the last clearing export_dirty (inserts a map update has not applied yet)."""
+        self._check()
+        return int(_capi.lib().nl_octree_dirty_count(self._h)) > 0
+
+    def export_nodes(self):
+        """The tree's node arrays as CPU tensors: child i32[n,8], code i64[n] (the u64 bit pattern), type i8[n], level u8[n]
+        (side = grid_dim >> level), the layout of DeviceOctree's arrays and of MapUpdater.state_dict()."""
+        self._check()
+        n = self.count_nodes()
+        a = (np.empty((n, 8), np.int32), np.empty(n, np.uint64), np.empty(n, np.int8), np.empty(n, np.uint8))
+        _capi.check(_capi.lib().nl_octree_nodes(self._h, *(_np_ptr(x) for x in a)), "nl_octree_nodes")
+        return torch.from_numpy(a[0]), torch.from_numpy(a[1].view(np.int64)), torch.from_numpy(a[2]), torch.from_numpy(a[3])
+
+    def load_nodes(self, child, code, type_, level):
+        """Replace the tree by node arrays (export_nodes' layout) in O(n), without replaying points.  Malformed arrays raise
+        NerfLoamError naming the failed checks and leave the tree as it was.  The restored tree has nothing dirty; having no point
+        history, it pickles as its node arrays from now on."""
+        self._check()
+        a = [np.ascontiguousarray(t.numpy() if isinstance(t, torch.Tensor) else t) for t in (child, code, type_, level)]
+        for x, dt in zip(a, (np.int32, np.int64, np.int8, np.uint8)):
+            if x.dtype != dt and not (dt == np.int64 and x.dtype == np.uint64):
+                raise _capi.NerfLoamError(f"Octree.load_nodes: expected {np.dtype(dt).name} node arrays, got {x.dtype}")
+        n = a[2].shape[0]
+        if a[0].shape != (n, 8) or a[1].shape != (n,) or a[3].shape != (n,):
+            raise _capi.NerfLoamError("Octree.load_nodes: node arrays of mismatched shapes")
+        rc = int(_capi.lib().nl_octree_restore(self._h, *(_np_ptr(x) for x in a), n))
+        if rc < 0:
+            raise _capi.NerfLoamError(_capi.lib().nl_last_error().decode())
+        if rc > 0:
+            raise malformed_tree("Octree.load_nodes", rc)
+        self._all_pts = None
+
+    # -- pickle (bindings.cpp:23-31): state = (size, feat_dim, voxel_size, all inserted tensors), replayed on load.  A tree restored
+    # from node arrays has no inserted tensors to replay and pickles as its node arrays.
     def __getstate__(self):
+        if self._all_pts is None and self._init_args is not None:
+            return {"init": self._init_args, "nodes": tuple(t.numpy() for t in self.export_nodes())}
         return {"init": self._init_args, "all_pts": self._all_pts}
 
     def __setstate__(self, state):
@@ -152,8 +210,11 @@ class Octree:
         self._init_args = None
         if state["init"] is not None:
             self.init(*state["init"])
-            for p in state["all_pts"]:
-                self.insert(p)
+            if "nodes" in state:
+                self.load_nodes(*state["nodes"])
+            else:
+                for p in state["all_pts"]:
+                    self.insert(p)
 
     def __del__(self):
         try:
@@ -184,9 +245,10 @@ class DeviceOctree:
     tensors; `try_insert` takes CPU or CUDA input and reads back 16 bytes.
 
     Pickling (and so deepcopy and torch.save) stores the init arguments and the node arrays as CPU arrays, 42 bytes per node, not
-    the inserted points, and restores onto the current CUDA device.  A restored tree is in the state of a restored host tree:
-    every row is dirty, so the next `export_dirty` returns all of them, and later inserts and exports equal the host tree's.  It
-    has no embedding-row state, so `update_map` refuses it (a MapUpdater builds its own tree)."""
+    the inserted points, and restores onto the current CUDA device.  The arrays are checked on the device before anything walks
+    them; a malformed state raises NerfLoamError.  A restored tree is in the state of a restored host tree: every row is dirty, so
+    the next `export_dirty` returns all of them, and later inserts and exports equal the host tree's.  It has no embedding-row
+    state, so `update_map` refuses it (MapUpdater.from_state_dict restores a tree together with its rows)."""
 
     def __init__(self, device="cuda"):
         self.device = torch.device(device)
@@ -301,6 +363,11 @@ class DeviceOctree:
         self._check()
         return int((self._type[:self._n] == 0).sum())
 
+    def is_dirty(self):
+        """Octree.is_dirty: nodes, pending dirty rows or points since the last dirty export."""
+        self._check()
+        return self._base != self._n or self._list_used > 0 or self._pending_points > 0
+
     def has_voxel(self, xyz):
         self._check()
         v = Octree._as_i32(xyz).reshape(-1)
@@ -376,6 +443,22 @@ class DeviceOctree:
         m, n_rows = self._counts[2:4].tolist()                      # read-back 2: dirty rows, embedding rows
         return self._ids, m, n_rows
 
+    def rebuild_map(self, centres, structure, vertex, vertex2row, vox2row, n_emb_rows):
+        """The full export of a tree loaded together with its embedding rows (MapUpdater.from_state_dict): every row into the
+        row = node id buffers of update_map, and vox2row composed from vertex2row.  Every vertex already has its row (the load
+        validated it), so no row is numbered and nothing is read back."""
+        self._check()
+        n = self._n
+        self._export(n, None, None, False, centres, structure, vertex)
+        ids = torch.arange(n, dtype=torch.int32, device=self.device)
+        self._counts[2].fill_(n)                                        # the id list's device-side length
+        ws = self._workspace(0, query_nodes=n)
+        _capi.check(_capi.lib().nl_devoctree_assign_rows(self.grid_dim, n, _capi.ptr(ids), n, _capi.ptr(self._type), _capi.ptr(vertex),
+                                                         _capi.ptr(vertex2row), _capi.ptr(self._scratch), int(n_emb_rows), _capi.ptr(vox2row),
+                                                         0, _capi.ptr(ws), ws.numel(), _capi.ptr(self._counts), _capi.stream_ptr()),
+                    "nl_devoctree_assign_rows")
+        _capi.LAUNCHES += 1
+
     def try_insert(self, vox):
         """Octree.try_insert: the share of the batch's distinct corner keys that are already in the tree (-1.0 for an empty or
         malformed batch)."""
@@ -433,14 +516,48 @@ class DeviceOctree:
     def get_features(self, pts):
         return None
 
+    def export_nodes(self):
+        """Octree.export_nodes: child i32[n,8], code i64[n], type i8[n], level u8[n] as CPU tensors."""
+        self._check()
+        n = self._n
+        return self._child[:n].cpu(), self._code[:n].cpu(), self._type[:n].cpu(), self._level[:n].cpu()
+
+    def validate(self, vertex2row=None, n_rows=0):
+        """nl_devoctree_validate over the tree's n nodes (with vertex2row, a device i32 tensor of >= n entries, the row checks too):
+        the OR of the failed NL_TREE_* checks' bits, 0 for a well-formed tree.  Reads back 16 bytes."""
+        self._check()
+        ws = self._workspace(0, query_nodes=self._n)
+        _capi.check(_capi.lib().nl_devoctree_validate(self.grid_dim, self._n, _capi.ptr(self._child), _capi.ptr(self._code), _capi.ptr(self._type),
+                                                      _capi.ptr(self._level), _capi.ptr(vertex2row), int(n_rows), _capi.ptr(ws), ws.numel(),
+                                                      _capi.ptr(self._qcounts), _capi.stream_ptr()), "nl_devoctree_validate")
+        _capi.LAUNCHES += 1
+        structural, rows = self._qcounts.tolist()
+        return structural | rows
+
+    def load_nodes(self, child, code, type_, level, vertex2row=None, n_rows=0):
+        """Replace the tree by node arrays (CPU tensors in export_nodes' layout, dtypes and shapes checked by the caller): one
+        host-to-device copy per array, then `validate` (with vertex2row / n_rows: the caller's device table, already uploaded).
+        On success the tree is clean, nothing dirty; malformed arrays raise NerfLoamError naming the failed checks and leave the
+        tree uninitialised."""
+        self._check()
+        n = type_.shape[0]
+        self._grow(n)
+        for src, dst in zip((child, code, type_, level), (self._child, self._code, self._type, self._level)):
+            dst[:n].copy_(src)
+        self._n = n
+        self._base, self._list_used, self._pending_points = n, 0, 0
+        self._restored = False
+        bits = self.validate(vertex2row, n_rows)
+        if bits:
+            self._init_args = None
+            raise malformed_tree("DeviceOctree.load_nodes", bits)
+
     _STATE = ("child", "code", "type", "level")
 
     def __getstate__(self):
         if self._init_args is None:
             return {"init": None}
-        n = self._n
-        arrays = (self._child, self._code, self._type, self._level)
-        return {"init": self._init_args, **{k: a[:n].cpu().numpy() for k, a in zip(self._STATE, arrays)}}
+        return {"init": self._init_args, **{k: a.numpy() for k, a in zip(self._STATE, self.export_nodes())}}
 
     def __setstate__(self, state):
         self.device = torch.device("cuda", torch.cuda.current_device())
@@ -450,9 +567,6 @@ class DeviceOctree:
         if state["init"] is None:
             return
         self.init(*state["init"])
-        n = len(state["type"])
-        self._grow(n)
-        for k, a in zip(self._STATE, (self._child, self._code, self._type, self._level)):
-            a[:n].copy_(torch.from_numpy(state[k]))
-        self._n = n                     # _base = 0, no pending entries, scratch at rest: every row is dirty, as after a host replay
+        self.load_nodes(*(torch.from_numpy(np.ascontiguousarray(state[k])) for k in self._STATE))
+        self._base = 0                  # no pending entries, scratch at rest: every row is dirty, as after a host replay
         self._restored = True
