@@ -222,7 +222,11 @@ typedef struct {
     int32_t n_hit_rays;    /* R_hit  = hits.sum()                        render_helpers.py:216   */
     int32_t max_hits;      /* P      = max valid hits per ray            voxel_helpers.py:555    */
     int32_t max_samples;   /* S_max  = max valid samples per ray         voxel_helpers.py:332    */
-    int32_t n_samples;     /* M      = sample_mask.sum()                 render_helpers.py:242   */
+    int32_t n_samples;     /* M      = sample_mask.sum()                 render_helpers.py:242
+                              summed in 64 bits, stored saturated at INT32_MAX; bit1 of error is set whenever the 64-bit total
+                              exceeds sample_capacity, so a call that needs 2^31 samples or more reports INT32_MAX with bit1 set.
+                              d_ray_offset saturates the same way and no sample at or past sample_capacity is written.  One ray's
+                              stratum count ceil(steps) saturates at INT32_MAX as well. */
     int32_t error;         /* bit0: sum(dists) > 10*MAX_DEPTH (ray_sample returns None, voxel_helpers.py:579)
                               bit1: sample capacity exceeded, bit2: DFS stack overflow                  */
     int32_t max_steps_ceil;/* ceil(steps).max(); the reference's noise width is this + P (voxel_helpers.py:294) */

@@ -15,6 +15,7 @@
 //   k_sample<true>  : 1 thread/hit ray  sampler again, writes the compact sample list
 // The reference keeps every intermediate as a padded dense tensor and syncs the host 6 times to size them.
 #include <cstdlib>
+#include <type_traits>
 
 #include "loss.cuh"
 #include "sampler.cuh"
@@ -28,7 +29,7 @@ struct Workspace {
     float *h_max;     // [20][R]
     int32_t *nvalid;  // [R]
     int32_t *hitray;  // [R] ray index of the q-th hit ray
-    unsigned long long *scan;   // [2][SCAN_SCRATCH]: tile ticket + per-tile (ready << 32 | total) of the two chained scans; zeroed per call
+    unsigned long long *scan;   // [2][SCAN_SCRATCH]: tile ticket + per-tile (ready << 63 | 63-bit total) of the two chained scans; zeroed per call
 };
 constexpr int SCAN_MAX_TILES = 1024;                 // tiles of 4096 elements: up to 4 M rays per call in one wave of look-back
 constexpr int SCAN_SCRATCH = SCAN_MAX_TILES + 8;     // words per scan: [0] = ticket counter, [8 + tile] = published tile total
@@ -274,8 +275,29 @@ __global__ void k_pack_children(int n_nodes, const int32_t *__restrict__ ids, co
 // k_scan: single-block exclusive scan over n <= 2^31 ints (n is ~1e5..1e6; ~10 us).
 //   HITS:    in = nvalid (flag = nvalid > 0) -> hit_rank[r] (or -1), hitray[rank] = r, total -> n_hit_rays
 //   SAMPLES: in = ray_nsamp                  -> ray_offset[r],                         total -> n_samples
+// The sample scan adds in 64 bits: a call may ask for 2^31 samples or more (many rays, small step).  Its offsets and total are
+// stored saturated at INT32_MAX (sat_i32), which no sample capacity exceeds, so the writing pass then stores nothing for them.
 // ------------------------------------------------------------------------------------------------
 enum { SCAN_HITS = 0, SCAN_SAMPLES = 1 };
+
+template <int MODE>
+using scan_t = typename std::conditional<MODE == SCAN_SAMPLES, long long, int>::type;
+
+__device__ __forceinline__ int sat_i32(long long x) { return x < (long long)INT32_MAX ? (int)x : INT32_MAX; }
+__device__ __forceinline__ int sat_i32(int x) { return x; }
+
+// the published total of a tile in the chained scans' scratch: bit 63 = ready, bits 0..62 = total
+constexpr unsigned long long SCAN_READY = 1ULL << 63;
+
+template <int MODE>
+__device__ __forceinline__ void scan_finish(long long total, nl_render_stats *stats, int sample_capacity) {
+    if (MODE == SCAN_HITS) {
+        stats->n_hit_rays = (int)total;
+    } else {
+        stats->n_samples = sat_i32(total);
+        if (total > sample_capacity) atomicOr(&stats->error, 2);
+    }
+}
 
 template <int MODE, bool STAGE = true>   // STAGE = false: no shared-memory staging of the compacted ray list (the block then needs 256 B of
                                           // shared memory and can share an SM with the persistent weight-gradient CTAs of the previous iteration)
@@ -284,7 +306,8 @@ __global__ void __launch_bounds__(1024) k_scan(int n, const int32_t *__restrict_
     // tiles of 4096 elements: every thread owns 4 consecutive ones (one 16-byte load, issued one tile ahead so that its
     // latency hides behind the previous tile), warp shuffle scan, then every warp scans the 32 warp totals redundantly:
     // one __syncthreads per tile (the totals are double-buffered) and the running carry stays in registers
-    __shared__ int wsum[2][32];
+    using T = scan_t<MODE>;
+    __shared__ T wsum[2][32];
     __shared__ int compact[(MODE == SCAN_HITS && STAGE) ? 4096 : 1];
     const int t = threadIdx.x, lane = t & 31, w = t >> 5;
     auto load4 = [&](int i0) {
@@ -298,7 +321,7 @@ __global__ void __launch_bounds__(1024) k_scan(int n, const int32_t *__restrict_
         }
         return x;
     };
-    int carry = 0;
+    T carry = 0;
     int4 nxt = load4(t * 4);
     for (int base = 0, par = 0; base < n; base += 4096, par ^= 1) {
         const int i0 = base + t * 4;
@@ -309,25 +332,25 @@ __global__ void __launch_bounds__(1024) k_scan(int n, const int32_t *__restrict_
 #pragma unroll
             for (int k = 0; k < 4; ++k) v[k] = v[k] > 0;
         }
-        const int mine = v[0] + v[1] + v[2] + v[3];
-        int incl = mine;
+        const T mine = (T)v[0] + v[1] + v[2] + v[3];
+        T incl = mine;
 #pragma unroll
         for (int off = 1; off < 32; off <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, incl, off);
+            const T y = __shfl_up_sync(0xffffffffu, incl, off);
             if (lane >= off) incl += y;
         }
         if (lane == 31) wsum[par][w] = incl;
         __syncthreads();
-        const int ws = wsum[par][lane];
-        int wi = ws;
+        const T ws = wsum[par][lane];
+        T wi = ws;
 #pragma unroll
         for (int off = 1; off < 32; off <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, wi, off);
+            const T y = __shfl_up_sync(0xffffffffu, wi, off);
             if (lane >= off) wi += y;
         }
-        const int wexcl = __shfl_sync(0xffffffffu, wi - ws, w);      // exclusive prefix of this warp's total
-        const int tile_total = __shfl_sync(0xffffffffu, wi, 31);
-        int run = carry + wexcl + incl - mine;
+        const T wexcl = __shfl_sync(0xffffffffu, wi - ws, w);      // exclusive prefix of this warp's total
+        const T tile_total = __shfl_sync(0xffffffffu, wi, 31);
+        T run = carry + wexcl + incl - mine;
         if (MODE == SCAN_HITS) {
             // ranks as one 16-byte store; the compacted ray list of this tile is contiguous in the output, so it is staged in
             // shared memory and written back coalesced
@@ -344,7 +367,7 @@ __global__ void __launch_bounds__(1024) k_scan(int n, const int32_t *__restrict_
                 if (i0 + 2 < n) out[i0 + 2] = o.z;
             }
             if (STAGE) {
-                int loc = run - carry;
+                int loc = (int)(run - carry);
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
                     if (v[k]) compact[loc] = i0 + k;     // v[k] is 0 for i0 + k >= n
@@ -363,7 +386,7 @@ __global__ void __launch_bounds__(1024) k_scan(int n, const int32_t *__restrict_
                 }
             }
         } else {
-            const int4 o = make_int4(run, run + v[0], run + v[0] + v[1], run + v[0] + v[1] + v[2]);
+            const int4 o = make_int4(sat_i32(run), sat_i32(run + v[0]), sat_i32(run + v[0] + v[1]), sat_i32(run + v[0] + v[1] + v[2]));
             if (i0 + 3 < n) {
                 *reinterpret_cast<int4 *>(out + i0) = o;
             } else {
@@ -374,15 +397,7 @@ __global__ void __launch_bounds__(1024) k_scan(int n, const int32_t *__restrict_
         }
         carry += tile_total;
     }
-    if (t == 0) {
-        const int total = carry;
-        if (MODE == SCAN_HITS) {
-            stats->n_hit_rays = total;
-        } else {
-            stats->n_samples = total;
-            if (total > sample_capacity) atomicOr(&stats->error, 2);
-        }
-    }
+    if (t == 0) scan_finish<MODE>(carry, stats, sample_capacity);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -390,14 +405,16 @@ __global__ void __launch_bounds__(1024) k_scan(int n, const int32_t *__restrict_
 // (so that every tile it may have to wait for belongs to a block that is already running), scans its tile, publishes the tile
 // total, and adds up the totals of the tiles before it -- one thread per predecessor, spinning until that total is published.
 // At 83 k rays that is 21 blocks and ~5 us instead of 17-30 us for the single-block loop above (which stays as the fallback for
-// more than 4 M rays).  scratch: [0] ticket, [8 + tile] (1 << 32 | total); zeroed by nl_render_samples before the chain starts.
+// more than 4 M rays).  scratch: [0] ticket, [8 + tile] (SCAN_READY | total); zeroed by nl_render_samples before the chain starts.
 // ------------------------------------------------------------------------------------------------
 template <int MODE>
 __global__ void __launch_bounds__(1024) k_scan_chained(int n, const int32_t *__restrict__ in, int32_t *__restrict__ out,
                                                         int32_t *__restrict__ hitray, nl_render_stats *stats, int sample_capacity,
                                                         unsigned long long *scratch) {
-    __shared__ int s_warp[32];
-    __shared__ int s_tile, s_carry;
+    using T = scan_t<MODE>;
+    __shared__ T s_warp[32];
+    __shared__ T s_carry;
+    __shared__ int s_tile;
     const int t = threadIdx.x, lane = t & 31, w = t >> 5;
     if (t == 0) s_tile = (int)atomicAdd(&scratch[0], 1ULL);
     __syncthreads();
@@ -416,34 +433,34 @@ __global__ void __launch_bounds__(1024) k_scan_chained(int n, const int32_t *__r
 #pragma unroll
         for (int k = 0; k < 4; ++k) v[k] = v[k] > 0;
     }
-    const int mine = v[0] + v[1] + v[2] + v[3];
-    int incl = mine;
+    const T mine = (T)v[0] + v[1] + v[2] + v[3];
+    T incl = mine;
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, incl, off);
+        const T y = __shfl_up_sync(0xffffffffu, incl, off);
         if (lane >= off) incl += y;
     }
     if (lane == 31) s_warp[w] = incl;
     __syncthreads();
-    const int ws_ = s_warp[lane];
-    int wi = ws_;
+    const T ws_ = s_warp[lane];
+    T wi = ws_;
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, wi, off);
+        const T y = __shfl_up_sync(0xffffffffu, wi, off);
         if (lane >= off) wi += y;
     }
-    const int wexcl = __shfl_sync(0xffffffffu, wi - ws_, w);
-    const int tile_total = __shfl_sync(0xffffffffu, wi, 31);
+    const T wexcl = __shfl_sync(0xffffffffu, wi - ws_, w);
+    const T tile_total = __shfl_sync(0xffffffffu, wi, 31);
     if (t == 0) {
         __threadfence();
-        atomicExch(&scratch[8 + tile], (1ULL << 32) | (unsigned long long)(unsigned)tile_total);
+        atomicExch(&scratch[8 + tile], SCAN_READY | (unsigned long long)tile_total);
     }
     // totals of the tiles before this one (gridDim.x <= 1024 = one thread per predecessor)
-    int prev = 0;
+    T prev = 0;
     if (t < tile) {
         unsigned long long a;
-        do { a = *((volatile unsigned long long *)&scratch[8 + t]); } while ((a >> 32) == 0ULL);
-        prev = (int)(unsigned)(a & 0xffffffffULL);
+        do { a = *((volatile unsigned long long *)&scratch[8 + t]); } while (!(a & SCAN_READY));
+        prev = (T)(a & ~SCAN_READY);
     }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) prev += __shfl_down_sync(0xffffffffu, prev, off);
@@ -451,13 +468,13 @@ __global__ void __launch_bounds__(1024) k_scan_chained(int n, const int32_t *__r
     if (lane == 0) s_warp[w] = prev;
     __syncthreads();
     if (t == 0) {
-        int c = 0;
+        T c = 0;
         for (int k = 0; k < 32; ++k) c += s_warp[k];
         s_carry = c;
     }
     __syncthreads();
-    const int carry = s_carry;
-    const int run = carry + wexcl + incl - mine;
+    const T carry = s_carry;
+    const T run = carry + wexcl + incl - mine;
     if (MODE == SCAN_HITS) {
         int4 o;
         o.x = v[0] ? run : -1;
@@ -478,7 +495,7 @@ __global__ void __launch_bounds__(1024) k_scan_chained(int n, const int32_t *__r
             loc += v[k];
         }
     } else {
-        const int4 o = make_int4(run, run + v[0], run + v[0] + v[1], run + v[0] + v[1] + v[2]);
+        const int4 o = make_int4(sat_i32(run), sat_i32(run + v[0]), sat_i32(run + v[0] + v[1]), sat_i32(run + v[0] + v[1] + v[2]));
         if (i0 + 3 < n) {
             *reinterpret_cast<int4 *>(out + i0) = o;
         } else {
@@ -487,15 +504,7 @@ __global__ void __launch_bounds__(1024) k_scan_chained(int n, const int32_t *__r
             if (i0 + 2 < n) out[i0 + 2] = o.z;
         }
     }
-    if (tile == (int)gridDim.x - 1 && t == 0) {
-        const int total = carry + tile_total;
-        if (MODE == SCAN_HITS) {
-            stats->n_hit_rays = total;
-        } else {
-            stats->n_samples = total;
-            if (total > sample_capacity) atomicOr(&stats->error, 2);
-        }
-    }
+    if (tile == (int)gridDim.x - 1 && t == 0) scan_finish<MODE>(carry + tile_total, stats, sample_capacity);
 }
 
 // counter-based uniform noise in (0,1) for the stochastic sampler when no noise tensor is passed in
@@ -562,7 +571,7 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
         const float steps = __fdiv_rn(tot, p.step_size);                         // :577
         if (!FILL) {
             if (tot > 10.0f * NL_MAX_DEPTH_FILL) atomicOr(&stats->error, 1);      // :579
-            steps_ceil = (int)ceilf(steps);
+            steps_ceil = nl_strata_count(steps);
         }
         // position of this ray in the reference's [200, K', P] layout and 800-wide launches (voxel_helpers.py:274-316)
         const int Kp = (R_hit + NL_SAMPLE_G - 1) / NL_SAMPLE_G;
@@ -583,8 +592,8 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
             uint32_t fl = 0;
             if (with_loss) fl = loss_flags(__fmul_rn(depth, cosr), gd, p.truncation, p.max_depth);
             if (FILL) {
-                const int m = base + nsamp;
-                if (m < p.sample_capacity) {
+                const long long m = (long long)base + nsamp;    // base saturates at INT32_MAX (k_scan): nothing lands past the arrays
+                if (m >= 0 && m < p.sample_capacity) {
                     p.s_ray[m] = r;
                     p.s_vox[m] = vox;
                     p.s_depth[m] = depth;

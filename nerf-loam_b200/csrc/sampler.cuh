@@ -9,7 +9,16 @@
 // previous cut to the new one.  After the last stratum the open remainder of the current bin -- and, while `tail_allowed`, of
 // the bins after it -- is flushed.  A sample is reported as emit(voxel id, z_from, z_to); callers derive mid-point / length.
 #pragma once
+#include <cstdint>
+
 #include "nl_cuda.cuh"
+
+// ceil(steps) as a stratum count.  The float -> int conversion is undefined at 2^31 and above, so the count saturates at INT32_MAX
+// there (and is 0 for NaN); below that it is (int)ceilf(steps) exactly.
+__device__ __forceinline__ int nl_strata_count(float steps) {
+    const float c = ceilf(steps);
+    return c >= 2147483648.0f ? INT32_MAX : (c > 0.0f ? (int)c : 0);
+}
 
 template <class Bins, class Noise, class Emit, class TailAllowed, class TailNextIdx>
 __device__ __forceinline__ void nl_inverse_cdf_walk(int n_bins, const Bins &bins, float steps, float fixed_step, Noise noise, Emit emit,
@@ -19,7 +28,7 @@ __device__ __forceinline__ void nl_inverse_cdf_walk(int n_bins, const Bins &bins
     float mass_before = 0.f, mass_upto = bins.prob(0);                  // cumulative probability at the two ends of bin b
     const float dt = fixed_step > 0.0f ? fixed_step : __frcp_rn(steps);  // (float)(1.0 / (double)steps) is the correctly rounded reciprocal
     float cut = lo;                                                      // where the previous sample ended
-    const int n_strata = (int)ceilf(steps);
+    const int n_strata = nl_strata_count(steps);
     bool exhausted = false;                                              // ran past the ray's last valid bin
     for (int i = 0; i < n_strata; ++i) {
         const float t = __fmul_rn(__fadd_rn((float)i, noise(i)), dt);

@@ -57,6 +57,17 @@ def _cfg(step_size, voxel_size, max_distance, crit=None):
     return c
 
 
+# nl_render_stats.n_samples saturates here: the sample list of one call is int32-indexed, so no capacity can hold such a call
+SAMPLES_SATURATED = 2 ** 31 - 1
+
+
+def _check_sample_total(n_samples, what):
+    """A call whose sample count saturated (2^31 - 1 samples or more) cannot be redone with a larger capacity: raise instead."""
+    if n_samples >= SAMPLES_SATURATED:
+        raise _capi.NerfLoamError(f"{what}: one call needs 2^31 - 1 or more samples (too many rays or too small a step_size); "
+                                  "split the rays or raise step_size")
+
+
 def _run_with_capacity(fn, n_rays, device, samples_per_ray=40):
     """Run fn(engine) and grow the sample capacity if the kernels report it was exceeded."""
     cap = n_rays * samples_per_ray
@@ -67,6 +78,7 @@ def _run_with_capacity(fn, n_rays, device, samples_per_ray=40):
         if st.error & 4:
             _check_ctl([4], "render_rays")
         if st.error & 2:
+            _check_sample_total(st.n_samples, "render_rays")
             cap = max(cap * 2, st.n_samples + 1)
             continue
         return eng, st
@@ -341,7 +353,8 @@ def _check_ctl(ctl, what):
         raise _capi.NerfLoamError(f"{what}: octree traversal stack overflow (octree deeper than the 18 levels of octree.cpp:39?)")
 
 
-def _grown_capacity(cap, ctl):
+def _grown_capacity(cap, ctl, what):
+    _check_sample_total(ctl[_capi.CTL_MAX_SAMPLES], what)
     return max(2 * cap, int(ctl[_capi.CTL_MAX_SAMPLES] * 1.25) + 1024)
 
 
@@ -565,7 +578,7 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
         torch.set_rng_state(snap[3]); torch.cuda.set_rng_state(snap[4], dev)
         if loss_log is not None:
             del loss_log[n_log:]
-        cap = _grown_capacity(cap, ctl)
+        cap = _grown_capacity(cap, ctl, "bundle_adjust_frames")
     for _ in range(ctl[_capi.CTL_SKIPPED]):
         print("Encouter a bug while Mapping, currently not be fixed, Continue!!")  # render_helpers.py:407-409 (the step was skipped)
     with torch.no_grad():
@@ -691,7 +704,7 @@ def _track_frame_graph(frame_pose, curr_frame, map_states, sdf_network, loss_cri
         _check_ctl(ctl, "track_frame")
         if not (ctl[_capi.CTL_ERROR] & 2):
             break
-        spr = -(-_grown_capacity(N_rays * spr, ctl) // N_rays)       # sample capacity exceeded: re-capture with a larger engine, redo the scan
+        spr = -(-_grown_capacity(N_rays * spr, ctl, "track_frame") // N_rays)       # sample capacity exceeded: re-capture with a larger engine, redo the scan
     with torch.no_grad():
         init_pose.data.copy_(g.pose6.reshape(init_pose.data.shape))
     if ctl[_capi.CTL_SKIPPED] > 0 or st.n_samples == 0:
@@ -752,6 +765,7 @@ def track_frame(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, 
             if not (st.error & 2):
                 break
             # sample capacity exceeded: nothing has been applied yet (the optimiser step follows) -- redo this iteration on a larger engine
+            _check_sample_total(st.n_samples, "track_frame")
             cap = max(2 * cap, int(st.n_samples * 1.25) + 1024)
             eng = _engine(N_rays, cap, dev)
             if opt is not None:
