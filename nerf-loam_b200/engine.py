@@ -93,23 +93,44 @@ class MapState:
     and the D2H/H2D detour of get_features, render_helpers.py:88, on every chunk of every iteration)."""
 
     def __init__(self, centres, structure, vox2row, emb, device="cuda"):
-        self.centres = centres.detach().to(device=device, dtype=torch.float32).contiguous()
-        self.structure = structure.detach().to(device=device, dtype=torch.int32).contiguous()
-        self.vox2row = vox2row.detach().to(device=device, dtype=torch.int32).contiguous()
-        self.emb = emb if (emb.is_cuda and emb.dtype == torch.bfloat16 and emb.is_contiguous()) else \
-            emb.detach().to(device=device, dtype=torch.bfloat16).contiguous()
+        self._set(centres.detach().to(device=device, dtype=torch.float32).contiguous(),
+                  structure.detach().to(device=device, dtype=torch.int32).contiguous(),
+                  vox2row.detach().to(device=device, dtype=torch.int32).contiguous(),
+                  emb if (emb.is_cuda and emb.dtype == torch.bfloat16 and emb.is_contiguous()) else
+                  emb.detach().to(device=device, dtype=torch.bfloat16).contiguous())
         assert self.centres.shape[1] == 3 and self.structure.shape[1] == 9 and self.vox2row.shape[1] == 8
         assert self.emb.shape[1] == 16, "embedding dim must be 16 (decoder_specs.in_dim of every shipped config)"
-        self.n_nodes = self.centres.shape[0]
-        self._packed = None
+
+    def _set(self, centres, structure, vox2row, emb, emb_full=None, stable=False, packed=None, cache_ref=None):
+        self.centres, self.structure, self.vox2row, self.emb = centres, structure, vox2row, emb
+        self.n_nodes = centres.shape[0]
+        self.emb_full = emb_full        # the capacity-sized table that emb is the front of (a MapUpdater map), else None
+        self.stable = stable            # the arrays keep their addresses across map updates: captured graphs survive them
+        self._packed = packed           # traversal image, None until packed_children()
+        self._cache_ref = cache_ref     # from_map_states' cache entry, which packed_children() stores the image back into
+
+    @classmethod
+    def view(cls, centres, structure, vox2row, emb, emb_full=None, stable=False, packed=None, cache_ref=None):
+        """A MapState over device arrays already in hot-path layout (dtypes and devices as __init__ makes them): no copy, no
+        conversion, no check."""
+        m = object.__new__(cls)
+        m._set(centres, structure, vox2row, emb, emb_full, stable, packed, cache_ref)
+        return m
+
+    def replace(self, **fields):
+        """A MapState over the same arrays with the given fields (view's arguments) replaced."""
+        args = dict(centres=self.centres, structure=self.structure, vox2row=self.vox2row, emb=self.emb, emb_full=self.emb_full,
+                    stable=self.stable, packed=self._packed, cache_ref=self._cache_ref)
+        args.update(fields)
+        return MapState.view(**args)
 
     _cache = {}
 
     def packed_children(self):
         """Traversal image of the octree (nl_octree_pack_children), built once per map version."""
-        if getattr(self, "_packed", None) is None:
+        if self._packed is None:
             self._packed = pack_children(self.centres, self.structure)
-            if getattr(self, "_cache_ref", None) is not None:
+            if self._cache_ref is not None:
                 self._cache_ref["packed"] = self._packed
         return self._packed
 
@@ -153,15 +174,10 @@ class MapState:
                           "centres": map_states["voxel_center_xyz"].detach().to(device=device, dtype=torch.float32).contiguous(),
                           "structure": stru.detach().to(device=device, dtype=torch.int32).contiguous(), "packed": None}
         c = cls._cache
-        obj = cls.__new__(cls)
-        obj.centres, obj.structure, obj.vox2row = c["centres"], c["structure"], c["vox2row"]
-        obj._packed = c["packed"]
-        obj._cache_ref = c                     # packed_children() stores the traversal image back into the shared cache entry
         emb = map_states["voxel_vertex_emb"]
-        obj.emb = emb.detach() if (emb.is_cuda and emb.dtype == torch.bfloat16 and emb.is_contiguous()) else \
+        emb = emb.detach() if (emb.is_cuda and emb.dtype == torch.bfloat16 and emb.is_contiguous()) else \
             emb.detach().to(device=device, dtype=torch.bfloat16).contiguous()
-        obj.n_nodes = obj.centres.shape[0]
-        return obj
+        return cls.view(c["centres"], c["structure"], c["vox2row"], emb, packed=c["packed"], cache_ref=c)
 
 
 class DecoderBuffers:

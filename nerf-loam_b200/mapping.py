@@ -19,7 +19,7 @@ import torch
 
 from . import _capi
 from .engine import MapState
-from .svo import DeviceOctree, Octree, malformed_tree, validate_nodes
+from .svo import DeviceOctree, Octree, grown, malformed_tree, validate_nodes
 
 
 class _LazyMapStates(dict):
@@ -106,8 +106,6 @@ class MapUpdater:
             raise ValueError("octree='device' needs a CUDA device and the incremental update")
         self.svo = DeviceOctree(self.device) if self.on_device else Octree()
         self.svo.init(grid_dim, embed_dim, voxel_size)     # mapping.py:81-82
-        self._vertex = self._v2r = None    # device tree only: vertex ids and the vertex -> row table, both indexed by node id
-        self.vertex2row = np.full(0, -1, np.int32)
         self.n_rows = 0
         self.n_nodes = 0
         self._emb_buf = torch.zeros((1024, embed_dim), dtype=torch.bfloat16, device=self.device)
@@ -115,9 +113,18 @@ class MapUpdater:
         self._gen = torch.Generator(device="cpu").manual_seed(seed)
         self.map_states = None
         self.incremental = bool(incremental) and self.device.type == "cuda"
-        self._cap = 0
-        self._centres = self._structure = self._vox2row = self._packed = None
-        self._host = None            # host mirrors (centres, structure, vertex) for the reference-format dict
+        # capacity-doubling buffers indexed by node id (_grow_nodes): the hot-path arrays on the device; the vertex ids and the
+        # vertex -> row table where the tree numbers the rows (host tree: numpy, device tree: device); the host tree also keeps
+        # host mirrors of centres and structure for the reference-format dict
+        d, i32 = self.device, torch.int32
+        self._centres, self._packed = torch.zeros((0, 3), dtype=torch.float32, device=d), torch.zeros(0, dtype=torch.uint8, device=d)
+        self._structure, self._vox2row = torch.zeros((0, 9), dtype=i32, device=d), torch.zeros((0, 8), dtype=i32, device=d)
+        if self.on_device:
+            self._vertex, self._v2r = torch.zeros((0, 8), dtype=i32, device=d), torch.zeros(0, dtype=i32, device=d)
+            self._host = ()
+        else:
+            self._vertex, self._v2r = np.zeros((0, 8), np.int32), np.zeros(0, np.int32)
+            self._host = (np.zeros((0, 3), np.float32), np.zeros((0, 9), np.int32))
         self.generation = 0
         self.last_update = {}
         self.readers = None          # optional share.SharedMap: in-place updates wait (on the stream) for its readers
@@ -135,13 +142,7 @@ class MapUpdater:
     @property
     def vertex2row(self):
         """i32 vertex (node id) -> embedding row, -1 = none (numpy; copied from the device with octree="device")."""
-        if self._v2r is not None:
-            return self._v2r[:self.n_nodes].cpu().numpy()
-        return self._vertex2row
-
-    @vertex2row.setter
-    def vertex2row(self, v):
-        self._vertex2row = v
+        return torch.as_tensor(self._v2r[:self.n_nodes]).cpu().numpy()
 
     # -- checkpoints ------------------------------------------------------------------------------------------------------------
     FORMAT = 1
@@ -214,27 +215,22 @@ class MapUpdater:
         mu._gen.set_state(sd["generator"])
         mu._emb_buf[:n_rows].copy_(sd["embeddings"])
         mu.n_rows = n_rows
+        mu._v2r = grown(mu._v2r, n, 0, -1)
+        torch.as_tensor(mu._v2r)[:n].copy_(v2r)             # numpy (host tree) or device (device tree): one copy either way
         if mu.on_device:
-            mu._v2r[:n].copy_(v2r)
             mu.svo.load_nodes(*nodes, vertex2row=mu._v2r, n_rows=n_rows)
-            mu.svo.rebuild_map(mu._centres, mu._structure, mu._vertex, mu._v2r, mu._vox2row, n_rows)
-            _capi.check(_capi.lib().nl_octree_pack_children(n, _capi.ptr(mu._centres), _capi.ptr(mu._structure), _capi.ptr(mu._packed),
-                                                            _capi.stream_ptr()), "nl_octree_pack_children")
-            _capi.LAUNCHES += 1
-            mu.n_nodes = n
-            mu._publish_device()
         else:
             bits = validate_nodes(sd["grid_dim"], *nodes, v2r, n_rows)
             if bits:
                 raise malformed_tree("MapUpdater.from_state_dict", bits)
             mu.svo.load_nodes(*nodes)
-            mu.vertex2row = v2r.numpy().copy()
-            if mu.incremental:
-                c, s, v = (t.numpy() for t in mu.svo.export_map())
-                mu._apply_rows(np.arange(n, dtype=np.int32), c, s, v)
-                mu._publish_host()
-            else:
-                mu._update_full()
+        if mu.incremental:
+            ids, m, _ = mu._patch_rows(n, every_row=True)
+            mu.n_nodes = n
+            mu._pack_rows(ids, m)
+            mu._publish()
+        else:
+            mu._update_full()
         mu.generation = sd["generation"]
         return mu
 
@@ -244,7 +240,7 @@ class MapUpdater:
         T = torch.as_tensor(pose, dtype=torch.float32, device=self.device)
         world = pts @ T[:3, :3].transpose(-1, -2) + T[:3, 3]
         voxels = torch.div(world, self.voxel_size, rounding_mode="floor")
-        self.svo.insert(voxels.int() if self.on_device else voxels.cpu().int())
+        self.svo.insert(voxels.int())
         return self.update_grid_features()
 
     def insert_voxels(self, voxels_i32):
@@ -253,97 +249,57 @@ class MapUpdater:
 
     # ---------------------------------------------------------------------------------------------------------------
     def _grow_rows(self, new_rows):
-        if new_rows > self._emb_buf.shape[0]:                                  # grow in place (mapping.py:309-314 re-uploads everything)
-            cap = max(new_rows, 2 * self._emb_buf.shape[0])
-            buf = torch.zeros((cap, 16), dtype=torch.bfloat16, device=self.device)
-            buf[:self.n_rows] = self._emb_buf[:self.n_rows]
-            self._emb_buf = buf
+        self._emb_buf = grown(self._emb_buf, new_rows, self.n_rows, 0)          # grow in place (mapping.py:309-314 re-uploads everything)
         if self.init_std > 0 and new_rows > self.n_rows:                       # reference: zeros (mapping.py:305-307)
             add = torch.randn((new_rows - self.n_rows, 16), generator=self._gen) * self.init_std
             self._emb_buf[self.n_rows:new_rows] = add.to(torch.bfloat16).to(self.device)
         self.n_rows = new_rows
 
     def _grow_nodes(self, n):
-        if n <= self._cap:
-            return
-        cap = max(n, 2 * self._cap, 4096)
-        d = self.device
-        new = (torch.zeros((cap, 3), dtype=torch.float32, device=d), torch.full((cap, 9), -1, dtype=torch.int32, device=d),
-               torch.full((cap, 8), -1, dtype=torch.int32, device=d), torch.zeros(cap * 128, dtype=torch.uint8, device=d))
-        if self._cap:
-            k = self.n_nodes
-            new[0][:k] = self._centres[:k]; new[1][:k] = self._structure[:k]; new[2][:k] = self._vox2row[:k]
-            new[3][:k * 128] = self._packed[:k * 128]
-        self._centres, self._structure, self._vox2row, self._packed = new
-        if self.on_device:
-            vx, v2r = torch.full((cap, 8), -1, dtype=torch.int32, device=d), torch.full((cap,), -1, dtype=torch.int32, device=d)
-            if self._cap:
-                vx[:self.n_nodes] = self._vertex[:self.n_nodes]; v2r[:self.n_nodes] = self._v2r[:self.n_nodes]
-            self._vertex, self._v2r = vx, v2r
-        self._cap = cap
+        k = self.n_nodes
+        self._centres, self._structure, self._vox2row, self._vertex, self._v2r = (
+            grown(b, n, k, fill, 4096) for b, fill in ((self._centres, 0), (self._structure, -1), (self._vox2row, -1), (self._vertex, -1),
+                                                       (self._v2r, -1)))
+        self._packed = grown(self._packed, 128 * n, 128 * k, 0, 128 * 4096)
+        self._host = tuple(grown(b, n, k, None, 4096) for b in self._host)
 
     def update_grid_features(self):
         """mapping.py:320-339.  Returns the engine.MapState (also stored, with the reference's dict keys, in self.map_states)."""
-        if self.on_device:
-            return self._update_device()
-        return self._update_incremental() if self.incremental else self._update_full()
-
-    def _update_device(self):
+        if not self.incremental:
+            return self._update_full()
         n = self.svo.count_export_nodes()
         self._grow_nodes(n)
         if self.readers is not None:      # a tracker on another stream may still traverse the arrays that are patched below
             for ev in self.readers.reader_events():
                 torch.cuda.current_stream(self.device).wait_event(ev)
-        ids, m, new_rows = self.svo.update_map(self._centres, self._structure, self._vertex, self._v2r, self._vox2row, self.n_rows)
+        ids, m, new_rows = self._patch_rows(n)
         self._grow_rows(new_rows)
-        if m:
-            _capi.check(_capi.lib().nl_octree_pack_children_rows(m, _capi.ptr(ids), _capi.ptr(self._centres), _capi.ptr(self._structure),
-                                                                 _capi.ptr(self._packed), _capi.stream_ptr()), "nl_octree_pack_children_rows")
-            _capi.LAUNCHES += 1
+        self._pack_rows(ids, m)
         self.n_nodes = n
         self.generation += 1
         self.last_update = {"dirty_rows": int(m), "nodes": int(n), "embedding_rows": int(new_rows)}
-        return self._publish_device()
+        return self._publish()
 
-    def _publish_device(self):
-        n = self.n_nodes
-        ms = MapState.__new__(MapState)
-        ms.centres, ms.structure, ms.vox2row = self._centres[:n], self._structure[:n], self._vox2row[:n]
-        ms.emb = self.embeddings
-        ms.emb_full = self._emb_buf
-        ms.n_nodes = n
-        ms._packed = self._packed[:n * 128]
-        ms.stable = True
-        c, s, v, r = self._centres[:n], self._structure[:n], self._vertex[:n], self._v2r[:n]
-        build = lambda: {"voxel_vertex_idx": v.cpu(), "voxel_center_xyz": c.cpu(), "voxel_structure": s.cpu(),
-                         "voxel_id2embedding_id": r.cpu().view(-1, 1)}
-        self.map_states = _LazyMapStates({"voxel_vertex_emb": self.embeddings, "_mapstate": ms}, build)
-        return ms
-
-    def _update_incremental(self):
-        ids, c, s, v = self.svo.export_dirty()
-        new_rows = self._apply_rows(ids, c, s, v)
-        self.generation += 1
-        self.last_update = {"dirty_rows": int(ids.shape[0]), "nodes": int(self.n_nodes), "embedding_rows": int(new_rows)}
-        return self._publish_host()
-
-    def _apply_rows(self, ids, c, s, v):
-        """Patches the exported rows ids (ascending) into the device buffers and host mirrors, numbering their new vertices;
-        returns the new number of embedding rows."""
-        n = self.svo.count_export_nodes()
+    def _patch_rows(self, n, every_row=False):
+        """Writes the rows that changed since the last update (every_row: all n rows of a restored tree) into the node buffers, at
+        row = node id, and numbers their new vertices.  Returns (ids, m, rows): ids[:m] are the patched node ids (device), rows
+        the new number of embedding rows."""
+        if self.on_device:
+            if not every_row:
+                return self.svo.update_map(self._centres, self._structure, self._vertex, self._v2r, self._vox2row, self.n_rows)
+            self.svo.rebuild_map(self._centres, self._structure, self._vertex, self._v2r, self._vox2row, self.n_rows)
+            return torch.arange(n, dtype=torch.int32, device=self.device), n, self.n_rows
+        if every_row:
+            ids, (c, s, v) = np.arange(n, dtype=np.int32), (t.numpy() for t in self.svo.export_map())
+        else:
+            ids, c, s, v = self.svo.export_dirty()
         m = ids.shape[0]
-        if self.vertex2row.shape[0] < n:
-            self.vertex2row = np.concatenate([self.vertex2row, np.full(n - self.vertex2row.shape[0], -1, np.int32)])
         rows = np.empty((m, 8), np.int32)
-        new_rows = int(_capi.lib().nl_assign_embedding_rows_subset(v.ctypes.data_as(C.c_void_p), m, n, self.vertex2row.ctypes.data_as(C.c_void_p),
+        new_rows = int(_capi.lib().nl_assign_embedding_rows_subset(v.ctypes.data_as(C.c_void_p), m, n, self._v2r.ctypes.data_as(C.c_void_p),
                                                                    self.n_rows, rows.ctypes.data_as(C.c_void_p)))
         if new_rows < 0:
             raise _capi.NerfLoamError(_capi.lib().nl_last_error().decode())
-        self._grow_rows(new_rows)
-        self._grow_nodes(n)
-        if self.readers is not None:      # a tracker on another stream may still traverse the arrays that are patched below
-            for ev in self.readers.reader_events():
-                torch.cuda.current_stream(self.device).wait_event(ev)
+        idx = None
         if m:
             d = self.device
             idx = torch.from_numpy(ids).to(d, non_blocking=True)
@@ -351,53 +307,51 @@ class MapUpdater:
             self._centres.index_copy_(0, idl, torch.from_numpy(c).to(d, non_blocking=True))
             self._structure.index_copy_(0, idl, torch.from_numpy(s).to(d, non_blocking=True))
             self._vox2row.index_copy_(0, idl, torch.from_numpy(rows).to(d, non_blocking=True))
-            _capi.check(_capi.lib().nl_octree_pack_children_rows(m, _capi.ptr(idx), _capi.ptr(self._centres), _capi.ptr(self._structure),
+        self._host[0][ids], self._host[1][ids], self._vertex[ids] = c, s, v
+        return idx, m, new_rows
+
+    def _pack_rows(self, ids, m):
+        """Re-packs the traversal image of the nodes ids[:m]."""
+        if m:
+            _capi.check(_capi.lib().nl_octree_pack_children_rows(m, _capi.ptr(ids), _capi.ptr(self._centres), _capi.ptr(self._structure),
                                                                  _capi.ptr(self._packed), _capi.stream_ptr()), "nl_octree_pack_children_rows")
             _capi.LAUNCHES += 1
-        # host mirrors for the reference-format dict (CPU tensors like mapping.py:321-337), patched in place as well
-        if self._host is None or self._host[0].shape[0] < n:
-            cap = max(n, 2 * (self._host[0].shape[0] if self._host is not None else 0))
-            hc, hs, hv = np.zeros((cap, 3), np.float32), np.full((cap, 9), -1, np.int32), np.full((cap, 8), -1, np.int32)
-            if self._host is not None:
-                k = self.n_nodes
-                hc[:k], hs[:k], hv[:k] = self._host[0][:k], self._host[1][:k], self._host[2][:k]
-            self._host = (hc, hs, hv)
-        self._host[0][ids], self._host[1][ids], self._host[2][ids] = c, s, v
-        self.n_nodes = n
-        return new_rows
 
-    def _publish_host(self):
+    def _publish(self):
+        """The MapState of the current map version over the buffers, and self.map_states."""
         n = self.n_nodes
-        ms = MapState.__new__(MapState)
-        ms.centres, ms.structure, ms.vox2row = self._centres[:n], self._structure[:n], self._vox2row[:n]
-        ms.emb = self.embeddings
-        ms.emb_full = self._emb_buf              # capacity-sized table at a stable address (rows >= n_rows: zero, never referenced)
-        ms.n_nodes = n
-        ms._packed = self._packed[:n * 128]
-        ms.stable = True                          # base addresses survive map updates until a capacity doubling
-        centres_h, structure_h, vertex_h = (torch.from_numpy(a[:n]) for a in self._host)
-        id2 = torch.from_numpy(self.vertex2row[:n]).view(-1, 1)
-        self.map_states = {"voxel_vertex_idx": vertex_h, "voxel_center_xyz": centres_h, "voxel_structure": structure_h,
-                           "voxel_vertex_emb": self.embeddings, "voxel_id2embedding_id": id2, "_mapstate": ms}
+        # emb_full: the capacity-sized table at a stable address (rows >= n_rows: zero, never referenced); stable: the base addresses
+        # survive map updates until a capacity doubling
+        ms = MapState.view(self._centres[:n], self._structure[:n], self._vox2row[:n], self.embeddings, emb_full=self._emb_buf,
+                           stable=True, packed=self._packed[:n * 128])
+        if self.on_device:
+            c, s, v, r = self._centres[:n], self._structure[:n], self._vertex[:n], self._v2r[:n]
+            build = lambda: {"voxel_vertex_idx": v.cpu(), "voxel_center_xyz": c.cpu(), "voxel_structure": s.cpu(),
+                             "voxel_id2embedding_id": r.cpu().view(-1, 1)}
+            self.map_states = _LazyMapStates({"voxel_vertex_emb": self.embeddings, "_mapstate": ms}, build)
+        else:          # CPU tensors like mapping.py:321-337, over the host mirrors
+            c, s = (torch.from_numpy(a[:n]) for a in self._host)
+            self.map_states = {"voxel_vertex_idx": torch.from_numpy(self._vertex[:n]), "voxel_center_xyz": c, "voxel_structure": s,
+                               "voxel_vertex_emb": self.embeddings, "voxel_id2embedding_id": torch.from_numpy(self._v2r[:n]).view(-1, 1),
+                               "_mapstate": ms}
         return ms
 
     def _update_full(self):
         self.svo.export_dirty()                                                # keep the dirty list from growing without bound
         centres, structure, vertex = self.svo.export_map()                     # mapping.py:321-326
         n = centres.shape[0]
-        if self.vertex2row.shape[0] < n:
-            self.vertex2row = np.concatenate([self.vertex2row, np.full(n - self.vertex2row.shape[0], -1, np.int32)])
+        self._v2r = grown(self._v2r, n, self.n_nodes, -1)
         v = vertex.numpy()
-        new_rows = int(_capi.lib().nl_assign_embedding_rows(v.ctypes.data_as(C.c_void_p), n,
-                                                            self.vertex2row.ctypes.data_as(C.c_void_p), self.n_rows))
+        new_rows = int(_capi.lib().nl_assign_embedding_rows(v.ctypes.data_as(C.c_void_p), n, self._v2r.ctypes.data_as(C.c_void_p), self.n_rows))
         if new_rows < 0:
             raise _capi.NerfLoamError(_capi.lib().nl_last_error().decode())
         self._grow_rows(new_rows)
         self.n_nodes = n
         self.generation += 1
-        vox2row = np.where(v >= 0, self.vertex2row[np.clip(v, 0, None)], -1).astype(np.int32)
-        ms = MapState(centres, structure, torch.from_numpy(vox2row), self.embeddings, self.device)
-        id2 = torch.from_numpy(self.vertex2row[:n].copy()).view(-1, 1)
+        vox2row = np.where(v >= 0, self._v2r[np.clip(v, 0, None)], -1).astype(np.int32)
+        d = self.device
+        ms = MapState.view(centres.to(d), structure.to(d), torch.from_numpy(vox2row).to(d), self.embeddings)
+        id2 = torch.from_numpy(self._v2r[:n].copy()).view(-1, 1)
         self.map_states = {"voxel_vertex_idx": vertex, "voxel_center_xyz": centres, "voxel_structure": structure,
                            "voxel_vertex_emb": self.embeddings, "voxel_id2embedding_id": id2, "_mapstate": ms}
         return ms

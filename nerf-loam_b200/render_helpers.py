@@ -372,10 +372,7 @@ class _MapGraph:
         R = F * N_rays
         eng = SDFEngine(R, R * spr, dev)            # private: captured pointers must stay valid
         bufs = DecoderBuffers(sdf_network, dev)
-        mg = MapState.__new__(MapState)              # the map as the graph sees it: same arrays, the table at the size that is optimised
-        mg.__dict__.update(m.__dict__)
-        mg.emb = emb
-        m = mg
+        m = m.replace(emb=emb)                       # the map as the graph sees it: same arrays, the table at the size that is optimised
         self.key, self.eng, self.bufs, self.m, self.emb, self.F, self.N, self.cap = key, eng, bufs, m, emb, F, N_rays, cap
         self.packed = m.packed_children()
         self.dirs = torch.tensor([0.0, 0.0, -1.0], device=dev).repeat(F, cap, 1).contiguous()
@@ -436,8 +433,8 @@ class _MapGraph:
     @classmethod
     def get(cls, m, emb, sdf_network, cfg, F, N_rays, lrs, update_decoder, pose_rows, deterministic, n_points, spr):
         cap = max(1 << 17, 1 << (int(n_points) - 1).bit_length())
-        stable = getattr(m, "stable", False)
-        if stable and getattr(m, "emb_full", None) is not None and emb.data_ptr() == m.emb_full.data_ptr():
+        stable = m.stable
+        if stable and m.emb_full is not None and emb.data_ptr() == m.emb_full.data_ptr():
             # a mapping.MapUpdater map: every array sits in a capacity-sized buffer at a fixed address, so the captured graph stays
             # valid across map updates; the table is optimised at its full capacity (rows not yet handed out are zero, receive zero
             # gradients and therefore do not move under Adam)
@@ -550,7 +547,7 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
     if cuda_graph is None:
         # automatic only for maps whose arrays keep their addresses across map updates (mapping.MapUpdater): a capture costs about
         # as much as 1.5 eager calls, so re-capturing for every new map (the reference's per-frame dicts) would be a net loss
-        cuda_graph = graph_ok and getattr(m, "stable", False)
+        cuda_graph = graph_ok and m.stable
     elif cuda_graph and not graph_ok:
         raise ValueError("cuda_graph=True needs ray_selection='device', no per-iteration host inputs/outputs and >= N_rays points per scan")
     cap = R * SAMPLES_PER_RAY_MAP
@@ -644,7 +641,7 @@ class _TrackGraph:
     @classmethod
     def get(cls, m, sdf_network, cfg, N_rays, lr, deterministic, n_points, samples_per_ray=64):
         cap = max(1 << 17, 1 << (int(n_points) - 1).bit_length())
-        stable = getattr(m, "stable", False)      # mapping.MapUpdater map: fixed base addresses, the graph survives map updates
+        stable = m.stable                         # mapping.MapUpdater map: fixed base addresses, the graph survives map updates
         key = (N_rays, float(lr), bool(deterministic), cap, int(samples_per_ray), m.centres.data_ptr(), m.structure.data_ptr(), m.vox2row.data_ptr(),
                m.packed_children().data_ptr(), m.emb.data_ptr(), -1 if stable else m.n_nodes, -1 if stable else int(m.emb.shape[0]),
                tuple(p.data_ptr() for p in _decoder_params(sdf_network)), tuple(sorted(cfg.items())))
@@ -727,7 +724,8 @@ def track_frame(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, 
         raise ValueError("ray_selection must be 'host' or 'device'")
     graph_ok = ray_selection == "device" and noise_per_iter is None and loss_log is None and curr_frame.points.shape[0] >= N_rays
     if cuda_graph is None:          # default: the captured path for maps with stable addresses (mapping.MapUpdater), see bundle_adjust_frames
-        stable = getattr(map_states, "stable", False) or getattr(map_states.get("_mapstate") if isinstance(map_states, dict) else None, "stable", False)
+        ms = map_states if isinstance(map_states, MapState) else map_states.get("_mapstate")
+        stable = ms is not None and ms.stable
         cuda_graph = graph_ok and stable and os.environ.get("NL_TRACK_GRAPH", "1") != "0"
     if cuda_graph:
         if not graph_ok:

@@ -78,19 +78,14 @@ class SharedMap:
             cur.wait_event(s.read_done)                      # the previous reader of this slot is done with it
         n_rows = map_state.emb.shape[0]
         if s.emb is None or s.emb.shape[0] < n_rows:
-            full = getattr(map_state, "emb_full", None)       # a MapUpdater map: mirror its capacity, so the slot's address is as stable as the map's
+            full = map_state.emb_full                        # a MapUpdater map: mirror its capacity, so the slot's address is as stable as the map's
             want = max(n_rows, 2 * (s.emb.shape[0] if s.emb is not None else 0), full.shape[0] if full is not None else 0)
             s.emb = torch.empty((want, 16), dtype=torch.bfloat16, device=map_state.emb.device)
         s.emb[:n_rows].copy_(map_state.emb, non_blocking=True)
         s.dec_flat = _flat_decoder_state(decoder, s.dec_flat)
-        m = MapState.__new__(MapState)
-        m.__dict__.update(map_state.__dict__)
-        m.emb = s.emb[:n_rows]
-        m.emb_full = None
         # A MapUpdater map keeps its structural arrays at fixed addresses and each slot's table is a capacity buffer, so a slot is as
         # stable as the map it mirrors: the tracker's captured graph is reused per slot (render_helpers._TrackGraph keeps a few live)
-        m.stable = bool(getattr(map_state, "stable", False))
-        s.map = m
+        s.map = map_state.replace(emb=s.emb[:n_rows], emb_full=None)
         s.published = torch.cuda.Event()
         s.published.record(cur)
         self.version += 1

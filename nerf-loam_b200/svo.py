@@ -43,7 +43,73 @@ def encode(x, y, z):
     return int(_capi.lib().nl_morton_encode(int(x), int(y), int(z)))
 
 
-class Octree:
+def grown(buf, n, keep, fill=None, floor=0):
+    """`buf` (a torch tensor or a numpy array) if it has room for n rows, else a new buffer like it of max(n, 2 * its rows, floor)
+    rows that holds its first `keep` rows, the others set to `fill` (None: uninitialised).  Capacity doubling, so that the
+    addresses of a growing buffer change at most log2(size) times."""
+    cap = buf.shape[0]
+    if n <= cap:
+        return buf
+    shape = (max(n, 2 * cap, floor), *buf.shape[1:])
+    if isinstance(buf, np.ndarray):
+        new = np.empty(shape, buf.dtype) if fill is None else np.full(shape, fill, buf.dtype)
+    else:
+        new = buf.new_empty(shape) if fill is None else buf.new_full(shape, fill)
+    new[:keep] = buf[:keep]
+    return new
+
+
+def _int32(vox):
+    """Voxel coordinates as the reference's accessor<int,2> takes them: a tensor must be int32, anything else is converted."""
+    if not isinstance(vox, torch.Tensor):
+        return torch.from_numpy(np.ascontiguousarray(vox, dtype=np.int32))
+    if vox.dtype != torch.int32:
+        raise RuntimeError("expected an int32 tensor (the reference accessor<int,2> throws here)")
+    return vox.detach()
+
+
+class _ReferenceMethods:
+    """The input rules of the reference's methods (octree.cpp, bindings.cpp:11-31), shared by both trees: each method checks its
+    input here and hands a well-formed int32 [N,3] batch (a CPU numpy [3] for has_voxel) to the tree's _insert / _try_insert /
+    _has_voxel."""
+
+    def _check(self):
+        if self._init_args is None:
+            raise RuntimeError("Octree not initialized!")  # octree.cpp:56-59 prints this and carries on
+
+    def _check_query(self):
+        self._check()
+
+    # -- bindings.cpp:15 insert(Tensor int32[N,3])
+    def insert(self, vox):
+        self._check()
+        v = _int32(vox)
+        if v.dim() != 2 or v.shape[1] != 3:
+            print(f"Point dimensions mismatch: inputs are {v.shape[-1]} expect 3")  # octree.cpp:62-66
+            return
+        self._insert(v)
+
+    def try_insert(self, vox):
+        """The share of the batch's distinct corner keys that are already in the tree (-1.0 for an empty or malformed batch)."""
+        self._check_query()
+        v = _int32(vox)
+        if v.dim() != 2 or v.shape[1] != 3 or v.shape[0] == 0:
+            return -1.0
+        return self._try_insert(v)
+
+    def has_voxel(self, xyz):
+        self._check()
+        v = _int32(xyz).cpu().contiguous().numpy().reshape(-1)
+        if v.shape[0] != 3:
+            return False
+        return self._has_voxel(v)
+
+    def get_features(self, pts):
+        """Empty body in the reference (octree.cpp:208-210)."""
+        return None
+
+
+class Octree(_ReferenceMethods):
     def __init__(self):
         self._h = None
         self._all_pts = []              # None: restored from node arrays, no point history
@@ -53,42 +119,25 @@ class Octree:
     def init(self, grid_dim, feat_dim, voxel_size):
         if self._h is not None:
             _capi.lib().nl_octree_destroy(self._h)
+        self._init_args = None
         self._h = _capi.lib().nl_octree_create(int(grid_dim), int(feat_dim), float(voxel_size))
         if not self._h:
             raise _capi.NerfLoamError(_capi.lib().nl_last_error().decode())
         self._init_args = (int(grid_dim), int(feat_dim), float(voxel_size))
         self._all_pts = []
 
-    def _check(self):
-        if self._h is None:
-            raise RuntimeError("Octree not initialized!")  # octree.cpp:56-59 prints this and carries on
-
-    @staticmethod
-    def _as_i32(vox):
-        if isinstance(vox, torch.Tensor):
-            if vox.dtype != torch.int32:
-                raise RuntimeError("expected an int32 tensor (the reference accessor<int,2> throws here)")
-            vox = vox.detach().cpu().contiguous().numpy()
-        vox = np.ascontiguousarray(vox, dtype=np.int32)
-        return vox
-
-    # -- bindings.cpp:15 insert(Tensor int32[N,3])
-    def insert(self, vox):
-        self._check()
-        v = self._as_i32(vox)
-        if v.ndim != 2 or v.shape[1] != 3:
-            print(f"Point dimensions mismatch: inputs are {v.shape[-1]} expect 3")  # octree.cpp:62-66
-            return
-        _capi.check(_capi.lib().nl_octree_insert(self._h, v.ctypes.data_as(C.c_void_p), v.shape[0]), "nl_octree_insert")
+    def _insert(self, v):
+        v = v.cpu().contiguous().numpy()
+        _capi.check(_capi.lib().nl_octree_insert(self._h, _np_ptr(v), v.shape[0]), "nl_octree_insert")
         if self._all_pts is not None:
             self._all_pts.append(torch.from_numpy(v.copy()))
 
-    def try_insert(self, vox):
-        self._check()
-        v = self._as_i32(vox)
-        if v.ndim != 2 or v.shape[1] != 3:
-            return -1.0
-        return float(_capi.lib().nl_octree_try_insert(self._h, v.ctypes.data_as(C.c_void_p), v.shape[0]))
+    def _try_insert(self, v):
+        v = v.cpu().contiguous().numpy()
+        return float(_capi.lib().nl_octree_try_insert(self._h, _np_ptr(v), v.shape[0]))
+
+    def _has_voxel(self, v):
+        return bool(_capi.lib().nl_octree_has_voxel(self._h, _np_ptr(v)))
 
     def count_nodes(self):
         self._check()
@@ -97,17 +146,6 @@ class Octree:
     def count_leaf_nodes(self):
         self._check()
         return int(_capi.lib().nl_octree_count_leaf_nodes(self._h))
-
-    def has_voxel(self, xyz):
-        self._check()
-        v = self._as_i32(xyz).reshape(-1)
-        if v.shape[0] != 3:
-            return False
-        return bool(_capi.lib().nl_octree_has_voxel(self._h, v.ctypes.data_as(C.c_void_p)))
-
-    def get_features(self, pts):
-        """Empty body in the reference (octree.cpp:208-210)."""
-        return None
 
     def get_voxels(self):
         self._check()
@@ -233,7 +271,7 @@ def _at(t, byte_offset):
     return C.c_void_p(t.data_ptr() + byte_offset)
 
 
-class DeviceOctree:
+class DeviceOctree(_ReferenceMethods):
     """`Octree` with the tree in device memory (csrc/octree_dev.cu, include/nerfloam_b200.h section 1b): the same node ids,
     exports and counts as the host tree bit for bit, without copying the batch or the tree to the host.
 
@@ -262,39 +300,35 @@ class DeviceOctree:
             raise _capi.NerfLoamError("DeviceOctree.init: grid_dim must be a power of two in [2, 2^20]")
         self._init_args = (gd, int(feat_dim), float(voxel_size))
         self._restored = False
-        self._cap = 0
-        self._n = 1                     # the root, id 0 (octree.cpp:41-43)
+        d = self.device
+        self._child = torch.empty((0, 8), dtype=torch.int32, device=d)
+        self._code, self._type, self._level, self._scratch = (torch.empty(0, dtype=t, device=d)
+                                                              for t in (torch.int64, torch.int8, torch.uint8, torch.int32))
+        self._n = 0
         self._grow(4096)
+        self._n = 1                     # the root, id 0 (octree.cpp:41-43): its row is the fill values of _grow
         self._base = 0                  # node count at the last dirty export: ids >= base are dirty
         self._pending_points = 0        # points inserted since the last dirty export
-        self._list = torch.full((1024,), _NONE_U32, dtype=torch.int32, device=self.device)
+        self._list = torch.full((1024,), _NONE_U32, dtype=torch.int32, device=d)
         self._list_used = 0
-        self._counts = torch.zeros(8, dtype=torch.int64, device=self.device)
-        self._qcounts = torch.zeros(2, dtype=torch.int64, device=self.device)   # the queries' read-back block
-        self._ws = torch.empty(0, dtype=torch.uint8, device=self.device)
-        self._ids = torch.empty(1024, dtype=torch.int32, device=self.device)
-
-    def _check(self):
-        if self._init_args is None:
-            raise RuntimeError("Octree not initialized!")
+        self._counts = torch.zeros(8, dtype=torch.int64, device=d)
+        self._qcounts = torch.zeros(2, dtype=torch.int64, device=d)   # the queries' read-back block
+        self._ws = torch.empty(0, dtype=torch.uint8, device=d)
+        self._ids = torch.empty(1024, dtype=torch.int32, device=d)
 
     @property
     def grid_dim(self):
         return self._init_args[0]
 
+    def _ptrs(self, *names):
+        """C pointers of the node arrays `names` ("child", "code", "type", "level", "scratch"); by default the tree's four, in the
+        order every entry point takes them."""
+        return [_capi.ptr(getattr(self, "_" + k)) for k in names or self._STATE]
+
     def _grow(self, n):
-        if n <= self._cap:
-            return
-        cap = max(n, 2 * self._cap, 4096)
-        d = self.device
-        new = (torch.full((cap, 8), -1, dtype=torch.int32, device=d), torch.zeros(cap, dtype=torch.int64, device=d),
-               torch.full((cap,), -1, dtype=torch.int8, device=d), torch.zeros(cap, dtype=torch.uint8, device=d),
-               torch.full((cap,), _REST, dtype=torch.int32, device=d))
-        if self._cap:
-            for a, b in zip(new, (self._child, self._code, self._type, self._level, self._scratch)):
-                a[:self._n] = b[:self._n]
-        self._child, self._code, self._type, self._level, self._scratch = new
-        self._cap = cap
+        k = self._n
+        self._child, self._code, self._type, self._level, self._scratch = (
+            grown(a, n, k, fill, 4096) for a, fill in zip((self._child, self._code, self._type, self._level, self._scratch), (-1, 0, -1, 0, _REST)))
 
     def _workspace(self, n_points, query_nodes=None):
         """The workspace of an insert / export of n_points, or with query_nodes given, of a query over that many nodes."""
@@ -314,22 +348,14 @@ class DeviceOctree:
             raise NotImplementedError("DeviceOctree's queries run on a CUDA device; use svo.Octree on the CPU")
         self._check()
 
-    def insert(self, vox):
-        self._check()
-        if not isinstance(vox, torch.Tensor):
-            vox = torch.from_numpy(np.ascontiguousarray(vox, dtype=np.int32))
-        if vox.dtype != torch.int32:
-            raise RuntimeError("expected an int32 tensor (the reference accessor<int,2> throws here)")
-        if vox.dim() != 2 or vox.shape[1] != 3:
-            print(f"Point dimensions mismatch: inputs are {vox.shape[-1]} expect 3")  # octree.cpp:62-66
-            return
-        v = vox.detach().to(self.device).contiguous()
+    def _insert(self, v):
+        v = v.to(self.device).contiguous()
         n = v.shape[0]
         if n == 0:
             return
         L = _capi.lib()
         ws = self._workspace(n)
-        _capi.check(L.nl_devoctree_insert_count(self.grid_dim, _capi.ptr(self._child), _capi.ptr(v), n, _capi.ptr(ws), ws.numel(),
+        _capi.check(L.nl_devoctree_insert_count(self.grid_dim, *self._ptrs("child"), _capi.ptr(v), n, _capi.ptr(ws), ws.numel(),
                                                 _capi.ptr(self._counts), _capi.stream_ptr()), "nl_devoctree_insert_count")
         bad, n_new = self._counts[:2].tolist()                       # read-back 1: rejection flag, new nodes
         if bad:
@@ -338,12 +364,8 @@ class DeviceOctree:
         n0 = self._n
         self._grow(n0 + n_new)
         need = self._list_used + min(self._base, 10 * n)            # pending-list entries this batch may append
-        if need > self._list.numel():
-            lst = torch.full((max(need, 2 * self._list.numel()),), _NONE_U32, dtype=torch.int32, device=self.device)
-            lst[:self._list_used] = self._list[:self._list_used]
-            self._list = lst
-        _capi.check(L.nl_devoctree_insert_commit(self.grid_dim, n0, n_new, self._base, _capi.ptr(self._child), _capi.ptr(self._code),
-                                                 _capi.ptr(self._type), _capi.ptr(self._level), _capi.ptr(self._scratch),
+        self._list = grown(self._list, need, self._list_used, _NONE_U32)
+        _capi.check(L.nl_devoctree_insert_commit(self.grid_dim, n0, n_new, self._base, *self._ptrs(), *self._ptrs("scratch"),
                                                  _capi.ptr(self._list), n, _capi.ptr(ws), ws.numel(), _capi.ptr(self._counts),
                                                  _capi.stream_ptr()), "nl_devoctree_insert_commit")
         _capi.LAUNCHES += 2
@@ -368,20 +390,15 @@ class DeviceOctree:
         self._check()
         return self._base != self._n or self._list_used > 0 or self._pending_points > 0
 
-    def has_voxel(self, xyz):
-        self._check()
-        v = Octree._as_i32(xyz).reshape(-1)
-        if v.shape[0] != 3:
-            return False
+    def _has_voxel(self, v):
         out = torch.empty(1, dtype=torch.int32, device=self.device)
-        _capi.check(_capi.lib().nl_devoctree_find(self.grid_dim, _capi.ptr(self._child), _capi.ptr(torch.from_numpy(v).to(self.device)), 1,
+        _capi.check(_capi.lib().nl_devoctree_find(self.grid_dim, *self._ptrs("child"), _capi.ptr(torch.from_numpy(v).to(self.device)), 1,
                                                   _capi.ptr(out), _capi.stream_ptr()), "nl_devoctree_find")
         return bool(int(out[0]) >= 0)
 
     def _export(self, rows, ids, count_ptr, compact, centres, structure, vertex):
         _capi.check(_capi.lib().nl_devoctree_export(self.grid_dim, self._init_args[2], rows, _capi.ptr(ids), count_ptr, int(compact),
-                                                    _capi.ptr(self._child), _capi.ptr(self._code), _capi.ptr(self._type),
-                                                    _capi.ptr(self._level), _capi.ptr(centres), _capi.ptr(structure), _capi.ptr(vertex),
+                                                    *self._ptrs(), _capi.ptr(centres), _capi.ptr(structure), _capi.ptr(vertex),
                                                     _capi.stream_ptr()), "nl_devoctree_export")
         _capi.LAUNCHES += 1
 
@@ -398,12 +415,11 @@ class DeviceOctree:
     def _dirty_ids(self):
         """Sorted dirty ids into self._ids (device count in counts[2]); returns (their bound, points since the last export)."""
         rows = self._list_used + self._n - self._base
-        if rows > self._ids.numel():
-            self._ids = torch.empty(max(rows, 2 * self._ids.numel()), dtype=torch.int32, device=self.device)
+        self._ids = grown(self._ids, rows, 0)
         pts = self._pending_points
         ws = self._workspace(pts)
         _capi.check(_capi.lib().nl_devoctree_dirty_ids(self.grid_dim, self._n, self._base, self._list_used, _capi.ptr(self._list),
-                                                       _capi.ptr(self._scratch), _capi.ptr(self._ids), pts, _capi.ptr(ws), ws.numel(),
+                                                       *self._ptrs("scratch"), _capi.ptr(self._ids), pts, _capi.ptr(ws), ws.numel(),
                                                        _capi.ptr(self._counts), _capi.stream_ptr()), "nl_devoctree_dirty_ids")
         _capi.LAUNCHES += 1
         self._base, self._list_used, self._pending_points = self._n, 0, 0
@@ -435,8 +451,8 @@ class DeviceOctree:
         rows, pts = self._dirty_ids()
         self._export(rows, self._ids, _at(self._counts, 16), False, centres, structure, vertex)
         ws = self._workspace(pts)
-        _capi.check(_capi.lib().nl_devoctree_assign_rows(self.grid_dim, rows, _capi.ptr(self._ids), self._n, _capi.ptr(self._type),
-                                                         _capi.ptr(vertex), _capi.ptr(vertex2row), _capi.ptr(self._scratch), int(n_emb_rows),
+        _capi.check(_capi.lib().nl_devoctree_assign_rows(self.grid_dim, rows, _capi.ptr(self._ids), self._n, *self._ptrs("type"),
+                                                         _capi.ptr(vertex), _capi.ptr(vertex2row), *self._ptrs("scratch"), int(n_emb_rows),
                                                          _capi.ptr(vox2row), pts, _capi.ptr(ws), ws.numel(), _capi.ptr(self._counts),
                                                          _capi.stream_ptr()), "nl_devoctree_assign_rows")
         _capi.LAUNCHES += 1
@@ -453,26 +469,17 @@ class DeviceOctree:
         ids = torch.arange(n, dtype=torch.int32, device=self.device)
         self._counts[2].fill_(n)                                        # the id list's device-side length
         ws = self._workspace(0, query_nodes=n)
-        _capi.check(_capi.lib().nl_devoctree_assign_rows(self.grid_dim, n, _capi.ptr(ids), n, _capi.ptr(self._type), _capi.ptr(vertex),
-                                                         _capi.ptr(vertex2row), _capi.ptr(self._scratch), int(n_emb_rows), _capi.ptr(vox2row),
+        _capi.check(_capi.lib().nl_devoctree_assign_rows(self.grid_dim, n, _capi.ptr(ids), n, *self._ptrs("type"), _capi.ptr(vertex),
+                                                         _capi.ptr(vertex2row), *self._ptrs("scratch"), int(n_emb_rows), _capi.ptr(vox2row),
                                                          0, _capi.ptr(ws), ws.numel(), _capi.ptr(self._counts), _capi.stream_ptr()),
                     "nl_devoctree_assign_rows")
         _capi.LAUNCHES += 1
 
-    def try_insert(self, vox):
-        """Octree.try_insert: the share of the batch's distinct corner keys that are already in the tree (-1.0 for an empty or
-        malformed batch)."""
-        self._check_query()
-        if not isinstance(vox, torch.Tensor):
-            vox = torch.from_numpy(np.ascontiguousarray(vox, dtype=np.int32))
-        if vox.dtype != torch.int32:
-            raise RuntimeError("expected an int32 tensor (the reference accessor<int,2> throws here)")
-        if vox.dim() != 2 or vox.shape[1] != 3 or vox.shape[0] == 0:
-            return -1.0
-        v = vox.detach().to(self.device).contiguous()
+    def _try_insert(self, v):
+        v = v.to(self.device).contiguous()
         n = v.shape[0]
         ws = self._workspace(n, query_nodes=0)
-        _capi.check(_capi.lib().nl_devoctree_try_insert(self.grid_dim, _capi.ptr(self._child), _capi.ptr(v), n, _capi.ptr(ws), ws.numel(),
+        _capi.check(_capi.lib().nl_devoctree_try_insert(self.grid_dim, *self._ptrs("child"), _capi.ptr(v), n, _capi.ptr(ws), ws.numel(),
                                                         _capi.ptr(self._qcounts), _capi.stream_ptr()), "nl_devoctree_try_insert")
         _capi.LAUNCHES += 1
         hits, keys = self._qcounts.tolist()
@@ -480,8 +487,8 @@ class DeviceOctree:
 
     def _preorder(self, out, leaves_only):
         ws = self._workspace(0, query_nodes=self._n)
-        _capi.check(_capi.lib().nl_devoctree_preorder(self.grid_dim, self._n, _capi.ptr(self._code), _capi.ptr(self._type),
-                                                      _capi.ptr(self._level), int(leaves_only), _capi.ptr(out), _capi.ptr(self._qcounts),
+        _capi.check(_capi.lib().nl_devoctree_preorder(self.grid_dim, self._n, *self._ptrs("code", "type", "level"),
+                                                      int(leaves_only), _capi.ptr(out), _capi.ptr(self._qcounts),
                                                       _capi.ptr(ws), ws.numel(), _capi.stream_ptr()), "nl_devoctree_preorder")
         _capi.LAUNCHES += 1
 
@@ -506,15 +513,11 @@ class DeviceOctree:
         voxels = torch.empty((n, 4), dtype=torch.float32, device=d)
         children = torch.empty((n, 8), dtype=torch.float32, device=d)
         features = torch.empty((n, 8), dtype=torch.int32, device=d)
-        _capi.check(_capi.lib().nl_devoctree_export_nodes(self.grid_dim, self._init_args[2], n, None, None, 0, _capi.ptr(self._child),
-                                                          _capi.ptr(self._code), _capi.ptr(self._type), _capi.ptr(self._level),
+        _capi.check(_capi.lib().nl_devoctree_export_nodes(self.grid_dim, self._init_args[2], n, None, None, 0, *self._ptrs(),
                                                           _capi.ptr(voxels), _capi.ptr(children), None, None, _capi.ptr(features),
                                                           _capi.stream_ptr()), "nl_devoctree_export_nodes")
         _capi.LAUNCHES += 1
         return voxels.cpu(), children.cpu(), features.cpu()
-
-    def get_features(self, pts):
-        return None
 
     def export_nodes(self):
         """Octree.export_nodes: child i32[n,8], code i64[n], type i8[n], level u8[n] as CPU tensors."""
@@ -527,8 +530,7 @@ class DeviceOctree:
         the OR of the failed NL_TREE_* checks' bits, 0 for a well-formed tree.  Reads back 16 bytes."""
         self._check()
         ws = self._workspace(0, query_nodes=self._n)
-        _capi.check(_capi.lib().nl_devoctree_validate(self.grid_dim, self._n, _capi.ptr(self._child), _capi.ptr(self._code), _capi.ptr(self._type),
-                                                      _capi.ptr(self._level), _capi.ptr(vertex2row), int(n_rows), _capi.ptr(ws), ws.numel(),
+        _capi.check(_capi.lib().nl_devoctree_validate(self.grid_dim, self._n, *self._ptrs(), _capi.ptr(vertex2row), int(n_rows), _capi.ptr(ws), ws.numel(),
                                                       _capi.ptr(self._qcounts), _capi.stream_ptr()), "nl_devoctree_validate")
         _capi.LAUNCHES += 1
         structural, rows = self._qcounts.tolist()

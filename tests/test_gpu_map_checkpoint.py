@@ -50,7 +50,7 @@ def _assert_same_map(a, b, updated=True):
     if b.on_device:
         assert torch.equal(a._vertex[:n], b._vertex[:n])
     else:
-        for x, y in zip(a._host, b._host):
+        for x, y in zip((*a._host, a._vertex), (*b._host, b._vertex)):
             assert np.array_equal(x[:n], y[:n])
     assert set(a.map_states) == set(b.map_states)
     for k in a.map_states:
