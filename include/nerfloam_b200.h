@@ -299,6 +299,30 @@ NL_API int nl_octree_pack_children_rows(int32_t n_ids, const int32_t *d_ids, con
                                  void *stream);
 NL_API int nl_render_samples(const nl_render_args *args, void *stream);
 
+/* --------------------------------------------------------------------------------------------
+ * 3b. Batched front end: K independent problems in one ray batch (render_helpers.track_frames).  Rays [k N, (k+1) N) belong to
+ *     problem k, N = n_rays / K.  Every problem is sampled exactly as nl_render_samples over only its N rays would sample it:
+ *     its hit ranks, R_hit, P, S_max, max_steps_ceil, error bit 0, the loss-mask counters and the loss constants land in
+ *     d_problem_stats[k], and both reference_compat quirks and the 800-ray chunking are keyed by the problem's own (rank, R_hit, P).
+ *     args->d_stats receives the call-wide totals that size the rest of the chain: n_hit_rays, n_samples (bit1 of error: the
+ *     sample capacity, which all problems share) and bit2 of error.  d_hit_rank holds the rank within the problem, d_s_ray the
+ *     global ray index (problem = s_ray / N); the sample list is problem 0's samples in their solo order, then problem 1's, ...
+ *     Noise: args->d_noise (if given) is f32[K][noise_rows][noise_stride], rows by hit rank within the problem; otherwise problem
+ *     k draws hash noise from d_problem_seeds[k] (0 is mapped to 1, as for args->d_rng_seed) with the ray index WITHIN the problem
+ *     as counter, so under one seed it draws what a solo call draws; without d_problem_seeds every problem uses args' seed.
+ * -------------------------------------------------------------------------------------------- */
+#define NL_BATCH_MAX_PROBLEMS 31     /* the per-problem pose step runs one warp per problem in one block (as nl_pose_step) */
+typedef struct {
+    int32_t n_problems;                 /* K, 1 <= K <= NL_BATCH_MAX_PROBLEMS; args->n_rays must be a multiple of K */
+    int32_t noise_rows;                 /* rows per problem of args->d_noise */
+    nl_render_stats *d_problem_stats;   /* [K] */
+    const uint32_t *d_problem_seeds;    /* [K] or NULL */
+    int32_t *d_problem_base;            /* i32[K] written: global hit rank of problem k's first hit ray */
+} nl_batch_args;
+/* sizeof(nl_batch_args), NL_BATCH_MAX_PROBLEMS: checked by the bindings at load time like nl_abi_sizes */
+NL_API void nl_abi_sizes_batch(int32_t out[2]);
+NL_API int nl_render_samples_batch(const nl_render_args *args, const nl_batch_args *batch, void *stream);
+
 /* ============================================================================================
  * 4. Embedding gather + trilinear interpolation (render_helpers.py:40-93) and its backward
  * ============================================================================================ */
@@ -362,6 +386,17 @@ NL_API int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *d_fea
                     const int32_t *d_s_ray, const float *d_cos, const float *d_gt_depth, nl_render_stats *d_stats, float truncation,
                     float *d_sdf, float *d_dfeats, const nl_mlp_grads *grads, float *d_act, const float *d_dsdf_ext, void *wgrad_stream,
                     void *stream);
+/* Batched loss for a frozen decoder (no weight gradients; the samples of nl_render_samples_batch): sample m belongs to problem
+ * d_s_ray[m] / rays_per_problem, reads that problem's loss constants in d_problem_stats and adds its squared errors into that
+ * problem's fs_sum / sdf_sum.  sdf and dfeats are per sample the single-problem kernels' values bit for bit. */
+NL_API int nl_mlp_train_batch(int64_t M, const int32_t *d_M_dev, const float *d_feats, const nl_mlp_weights *w, const uint8_t *d_s_flag,
+                              const float *d_s_depth, const int32_t *d_s_ray, const float *d_cos, const float *d_gt_depth,
+                              nl_render_stats *d_problem_stats, int32_t rays_per_problem, float truncation, float *d_sdf, float *d_dfeats,
+                              void *stream);
+NL_API int nl_mlp_tc_train_batch(int64_t M, const int32_t *d_M_dev, const float *d_feats, const void *d_panels, const float *d_b0,
+                                 const float *d_b1, const float *d_w2, const float *d_b2, const uint8_t *d_s_flag, const float *d_s_depth,
+                                 const int32_t *d_s_ray, const float *d_cos, const float *d_gt_depth, nl_render_stats *d_problem_stats,
+                                 int32_t rays_per_problem, float truncation, float *d_sdf, float *d_dfeats, void *stream);
 /* loss constants from the sample statistics (criterion.py:84-88, 97-100); call after nl_render_samples */
 NL_API int nl_loss_prepare(nl_render_stats *d_stats, float fs_weight, float sdf_weight, void *stream);
 NL_API int nl_loss_finalize(nl_render_stats *d_stats, float fs_weight, float sdf_weight, void *stream);
@@ -396,6 +431,11 @@ NL_API int nl_pose_step(int n_frames, float *d_pose6, const float *d_pose_acc, f
 NL_API int nl_select_rays(int n_frames, int cap, int n_select, const int64_t *d_n_points, const uint32_t *d_seed, uint32_t seed,
                    const float *d_dirs_all, const float *d_gt_all, const float *d_cos_all, float *d_dirs, float *d_gt, float *d_cos,
                    int32_t *d_idx, void *stream);
+/* The same for n_problems independent problems: scan k (row k of the arrays) is selected with its own seed d_seeds[k], exactly as
+ * nl_select_rays(1, ...) with that seed selects it, so a batched problem draws the rays of a solo call under the same seed. */
+NL_API int nl_select_rays_batch(int n_problems, int cap, int n_select, const int64_t *d_n_points, const uint32_t *d_seeds,
+                                const float *d_dirs_all, const float *d_gt_all, const float *d_cos_all, float *d_dirs, float *d_gt,
+                                float *d_cos, int32_t *d_idx, void *stream);
 
 /* ============================================================================================
  * 7. Optimiser (torch.optim.Adam semantics, render_helpers.py:353/448): fp32 tensors and the bf16
@@ -433,6 +473,22 @@ NL_API int nl_adam_f32_ctl(int64_t n, float *d_param, const float *d_grad, float
                     double eps, const int32_t *d_ctl, void *stream);
 NL_API int nl_adam_bf16_ctl(int64_t n, uint16_t *d_param, const float *d_grad_f32, uint16_t *d_m, uint16_t *d_v, double lr, double beta1,
                      double beta2, double eps, const int32_t *d_ctl, void *stream);
+/* Batched tracking (section 3b): one control block per problem, d_ctl int32[K][NL_CTL_WORDS], initialised like a single block.
+ * An iteration in which problem k hits nothing (R_hit = 0, error bit 0 or no sample) stops problem k for the rest of the call, like
+ * the reference's `break` (render_helpers.py:488-491): NL_CTL_STOPPED is set, and from then on every iteration is a skipped one
+ * for it (SKIP_NOW = 1, Adam's step count frozen).  ERROR also receives the call-wide bits 1 and 2 of d_totals, MAX_SAMPLES the
+ * call-wide sample count (the capacity all problems share). */
+#define NL_CTL_STOPPED 7
+NL_API int nl_iter_status_batch(int n_problems, const nl_render_stats *d_totals, const nl_render_stats *d_problem_stats, int32_t *d_ctl,
+                                void *stream);
+/* nl_pose_step for K independent problems (K <= NL_BATCH_MAX_PROBLEMS), one pose each: warp k forms problem k's pose gradient from
+ * its accumulator row, applies Adam with its own rate d_lr[k] (f64), step count and skip flag (d_ctl[k]), finalises its loss
+ * (nl_loss_finalize on d_problem_stats[k]; d_last_loss[k] = that loss if the iteration was not skipped) and advances its seeds
+ * d_seeds_a[k] += inc_a, d_seeds_b[k] += inc_b (either array may be NULL). */
+NL_API int nl_pose_step_batch(int n_problems, float *d_pose6, const float *d_pose_acc, float *d_grad6, float *d_m, float *d_v, const double *d_lr,
+                              double beta1, double beta2, double eps, const int32_t *d_ctl, nl_render_stats *d_problem_stats, float fs_weight,
+                              float sdf_weight, float *d_last_loss, int32_t *d_seeds_a, int32_t inc_a, int32_t *d_seeds_b, int32_t inc_b,
+                              void *stream);
 
 /* ============================================================================================
  * 9. Multi-GPU exchange helpers (SURVEY.md 8 e): the per-iteration statistics that make the loss global are packed into ONE

@@ -11,6 +11,7 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     se3pose.OptimizablePose         <- src/se3pose.py
     frame.LidarFrame                <- src/lidarFrame.py
     render_helpers.render_rays / bundle_adjust_frames / track_frame / get_scores  <- src/variations/render_helpers.py
+    track_frames (= render_helpers.track_frames, track_batch)  K independent track_frame problems in one launch chain
     mapping.MapUpdater              <- Mapping.create_voxels / update_grid_features / get_embeddings (src/mapping.py)
     mesh.extract_mesh / marching_cubes  <- MeshExtractor.create_mesh / marching_cubes (src/utils/mesh_util.py)
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
@@ -18,11 +19,14 @@ no CPU or eager-PyTorch fallback for the kernels.
 """
 from . import _capi  # noqa: F401
 
-__all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share"]
+__all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
+           "track_batch", "track_frames"]
 
 
 def __getattr__(name):
+    import importlib
+    if name == "track_frames":
+        return importlib.import_module(".track_batch", __name__).track_frames
     if name in __all__:
-        import importlib
         return importlib.import_module("." + name, __name__)
     raise AttributeError(name)

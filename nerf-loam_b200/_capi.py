@@ -41,6 +41,12 @@ class RenderArgs(C.Structure):
     ]
 
 
+class BatchArgs(C.Structure):
+    """nl_batch_args (K independent problems in one ray batch, nl_render_samples_batch)."""
+    _fields_ = [("n_problems", C.c_int32), ("noise_rows", C.c_int32), ("d_problem_stats", vp), ("d_problem_seeds", vp),
+                ("d_problem_base", vp)]
+
+
 class MlpWeights(C.Structure):
     _fields_ = [("width", C.c_int32), ("W0", vp), ("b0", vp), ("W1", vp), ("b1", vp), ("W2", vp), ("b2", vp),
                 ("W0t", vp), ("W1t", vp)]
@@ -129,10 +135,21 @@ _SIGNATURES = {
     "nl_mc_count": (C.c_int, [C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, vp]),
     "nl_mc_emit": (C.c_int, [C.c_int32, C.c_int32, C.c_float, vp, vp, vp, vp, vp, C.c_int64, C.c_int64, vp, vp, vp]),
     "nl_mc_case_table": (C.c_int, [vp, vp, vp]),
+    # batched tracking (include/nerfloam_b200.h section 3b)
+    "nl_abi_sizes_batch": (None, [C.POINTER(C.c_int32 * 2)]),
+    "nl_render_samples_batch": (C.c_int, [C.POINTER(RenderArgs), C.POINTER(BatchArgs), vp]),
+    "nl_mlp_train_batch": (C.c_int, [C.c_int64, vp, vp, C.POINTER(MlpWeights), vp, vp, vp, vp, vp, vp, C.c_int32, C.c_float, vp, vp, vp]),
+    "nl_mlp_tc_train_batch": (C.c_int, [C.c_int64] + [vp] * 13 + [C.c_int32, C.c_float, vp, vp, vp]),
+    "nl_iter_status_batch": (C.c_int, [C.c_int, vp, vp, vp, vp]),
+    "nl_pose_step_batch": (C.c_int, [C.c_int, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, vp, vp, C.c_float, C.c_float, vp,
+                                     vp, C.c_int32, vp, C.c_int32, vp]),
+    "nl_select_rays_batch": (C.c_int, [C.c_int, C.c_int, C.c_int] + [vp] * 10),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)
 CTL_ERROR, CTL_SKIPPED, CTL_SKIP_NOW, CTL_ADAM_STEP, CTL_MIN_HIT, CTL_ITERS, CTL_MAX_SAMPLES, CTL_WORDS = 0, 1, 2, 3, 4, 5, 6, 8
+CTL_STOPPED = 7              # batched control blocks only (nl_iter_status_batch)
+BATCH_MAX_PROBLEMS = 31      # NL_BATCH_MAX_PROBLEMS
 STATS_PACK_FIXED = 10
 # node-array checks, bit i = 1 << i (NL_TREE_* in include/nerfloam_b200.h section 1)
 TREE_CHECKS = ("ROOT", "RANGE", "LINK", "PARENTS", "SHAPE", "ROWS", "VERTICES")
@@ -169,6 +186,11 @@ def lib():
         mine = [C.sizeof(RenderStats), RenderStats.n_samples.offset, C.sizeof(RenderArgs), C.sizeof(MlpWeights)]
         if list(sizes) != mine:
             raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so: {list(sizes)} vs {mine}")
+        bsizes = (C.c_int32 * 2)()
+        L.nl_abi_sizes_batch(C.byref(bsizes))
+        bmine = [C.sizeof(BatchArgs), BATCH_MAX_PROBLEMS]
+        if list(bsizes) != bmine:
+            raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (batch): {list(bsizes)} vs {bmine}")
         _lib = L
     return _lib
 

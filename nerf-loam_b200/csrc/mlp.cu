@@ -17,6 +17,7 @@
 //     h1 -> dh2 -> dh1.  ReLU masks are 128 bits per thread in registers.
 // Nothing but the input features [M,16], sdf [M], d features [M,16] and -- only when the decoder is being
 // trained -- h1 / dh2 [M,W] (for the split-K dW1 GEMM) touches HBM.
+#include "loss.cuh"
 #include "nl_cuda.cuh"
 
 namespace {
@@ -135,10 +136,13 @@ struct MlpParams {
     nl_mlp_grads g;
     float *act_h1, *act_dh2;
     const float *dsdf_ext;
+    int seg_rays;         // SEG: rays per problem; stats = the problems' statistics, problem = s_ray / seg_rays
 };
 
-template <int W, bool TRAIN, bool WGRAD>
+// SEG (training without weight gradients only): nl_mlp_train_batch's loss, per problem (see k_mlp_wg in mlp_tc.cu)
+template <int W, bool TRAIN, bool WGRAD, bool SEG = false>
 __global__ void __launch_bounds__(NTHREADS, 1) k_mlp(MlpParams p) {
+    static_assert(!SEG || (TRAIN && !WGRAD), "the batched loss is for frozen-decoder training only");
     using C = Cfg<W>;
     constexpr int J = C::J;
     constexpr int NMASK = (16 * J + 31) / 32;
@@ -274,25 +278,36 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp(MlpParams p) {
 #pragma unroll
             for (int i = 0; i < 16; ++i) mine = (lane == i) ? ps[i] : mine;
             const long long m = m0 + t0 + lane;
-            if (lane < 16 && m < M && p.dsdf_ext) {
+            int seg_k = -1;                          // SEG: this lane's problem
+            double seg_fs = 0.0, seg_sdf = 0.0;
+            if (!SEG && lane < 16 && m < M && p.dsdf_ext) {
                 my_dsdf = p.dsdf_ext[m];
             } else if (lane < 16 && m < M) {
                 const uint32_t fl = p.s_flag[m];
                 const int r = p.s_ray[m];
+                float gf = g_fs, gs = g_sdf;
+                if constexpr (SEG) {
+                    seg_k = r / p.seg_rays;
+                    gf = p.stats[seg_k].g_fs;
+                    gs = p.stats[seg_k].g_sdf;
+                }
                 const float cosr = p.cosv ? p.cosv[r] : 1.0f;
                 const float z = __fmul_rn(p.s_depth[m], cosr);
                 const float d = p.gt_depth[r];
                 if (fl & 1u) {  // front: (sdf*1*1 - 1)^2
                     const float e = mine - 1.0f;
-                    loss_fs += (double)e * (double)e;
-                    my_dsdf += 2.0f * g_fs * e;
+                    if constexpr (SEG) seg_fs = (double)e * (double)e;
+                    else loss_fs += (double)e * (double)e;
+                    my_dsdf += 2.0f * gf * e;
                 }
                 if (fl & 2u) {  // sdf band: ((z + sdf*trunc) - depth)^2
                     const float e = __fsub_rn(__fadd_rn(z, __fmul_rn(mine, p.truncation)), d);
-                    loss_sdf += (double)e * (double)e;
-                    my_dsdf += 2.0f * g_sdf * p.truncation * e;
+                    if constexpr (SEG) seg_sdf = (double)e * (double)e;
+                    else loss_sdf += (double)e * (double)e;
+                    my_dsdf += 2.0f * gs * p.truncation * e;
                 }
             }
+            if constexpr (SEG) nl_seg_loss_add(p.stats, seg_k, seg_fs, seg_sdf);
         }
         float dsdf[16];
 #pragma unroll
@@ -406,7 +421,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp(MlpParams p) {
         __syncwarp();
     }
 
-    if (TRAIN && !p.dsdf_ext) {
+    if (TRAIN && !SEG && !p.dsdf_ext) {
         for (int off = 16; off > 0; off >>= 1) {
             loss_fs += __shfl_down_sync(0xffffffffu, loss_fs, off);
             loss_sdf += __shfl_down_sync(0xffffffffu, loss_sdf, off);
@@ -488,25 +503,25 @@ __global__ void k_transpose(int rows, int cols, const float *__restrict__ in, fl
     }
 }
 
-template <int W, bool TRAIN, bool WGRAD>
+template <int W, bool TRAIN, bool WGRAD, bool SEG = false>
 int launch_mlp(const MlpParams &p, cudaStream_t stream) {
     const size_t smem = Cfg<W>::smem_floats(WGRAD) * sizeof(float);
     static NlPerDevice configured;
-    const cudaError_t e = configured.once([&] { return cudaFuncSetAttribute(k_mlp<W, TRAIN, WGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); });
+    const cudaError_t e = configured.once([&] { return cudaFuncSetAttribute(k_mlp<W, TRAIN, WGRAD, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); });
     if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
     const long long ntiles = (p.M_host + T_TILE - 1) / T_TILE;
     const int grid = (int)(ntiles < (long long)nl_num_sms() ? ntiles : (long long)nl_num_sms());
-    k_mlp<W, TRAIN, WGRAD><<<grid, NTHREADS, smem, stream>>>(p);
+    k_mlp<W, TRAIN, WGRAD, SEG><<<grid, NTHREADS, smem, stream>>>(p);
     return NL_OK;
 }
 
-template <bool TRAIN, bool WGRAD>
+template <bool TRAIN, bool WGRAD, bool SEG = false>
 int dispatch_width(const MlpParams &p, cudaStream_t stream) {
     switch (p.w.width) {
-        case 256: return launch_mlp<256, TRAIN, WGRAD>(p, stream);
-        case 128: return launch_mlp<128, TRAIN, WGRAD>(p, stream);
-        case 64: return launch_mlp<64, TRAIN, WGRAD>(p, stream);
-        case 32: return launch_mlp<32, TRAIN, WGRAD>(p, stream);
+        case 256: return launch_mlp<256, TRAIN, WGRAD, SEG>(p, stream);
+        case 128: return launch_mlp<128, TRAIN, WGRAD, SEG>(p, stream);
+        case 64: return launch_mlp<64, TRAIN, WGRAD, SEG>(p, stream);
+        case 32: return launch_mlp<32, TRAIN, WGRAD, SEG>(p, stream);
         default: return nl_set_error_code(NL_ERR_UNSUPPORTED, "decoder width must be 32, 64, 128 or 256");
     }
 }
@@ -574,5 +589,23 @@ extern "C" int nl_mlp_train(int64_t M, const int32_t *d_M_dev, const float *feat
         if (rc != NL_OK) return rc;
     }
     NL_CHECK_LAUNCH("nl_mlp_train");
+    return NL_OK;
+}
+
+extern "C" int nl_mlp_train_batch(int64_t M, const int32_t *d_M_dev, const float *feats, const nl_mlp_weights *w, const uint8_t *s_flag,
+                                  const float *s_depth, const int32_t *s_ray, const float *cosv, const float *gt_depth,
+                                  nl_render_stats *problem_stats, int32_t rays_per_problem, float truncation, float *sdf, float *dfeats,
+                                  void *stream) {
+    if (M < 0) return nl_set_error("nl_mlp_train_batch: negative M");
+    if (rays_per_problem <= 0) return nl_set_error("nl_mlp_train_batch: rays_per_problem must be positive");
+    if (M == 0) return NL_OK;
+    if (!feats || !sdf || !dfeats || !weights_ok(w) || !s_flag || !s_depth || !s_ray || !gt_depth || !problem_stats)
+        return nl_set_error("nl_mlp_train_batch: null pointer");
+    MlpParams p = {};
+    p.M_host = M; p.M_dev = d_M_dev; p.feats = feats; p.w = *w; p.sdf = sdf;
+    p.s_flag = s_flag; p.s_depth = s_depth; p.s_ray = s_ray; p.cosv = cosv; p.gt_depth = gt_depth; p.stats = problem_stats;
+    p.truncation = truncation; p.dfeats = dfeats; p.seg_rays = rays_per_problem;
+    if (int rc = dispatch_width<true, false, true>(p, (cudaStream_t)stream)) return rc;
+    NL_CHECK_LAUNCH("nl_mlp_train_batch");
     return NL_OK;
 }

@@ -24,6 +24,7 @@
 // registers and B = the exact 0/1 mask expanded into a K-major tile.  gW0 = dh1^T x (mma.sync) and the column sums run beside it.
 #include <mutex>
 
+#include "loss.cuh"
 #include "nl_cuda.cuh"
 
 namespace tc {
@@ -213,6 +214,7 @@ struct Params {
     const float *dsdf_ext;
     float *act_dh1, *act_d;            // WGRAD: [cap][256], [cap]
     uint32_t *act_m2;                  // WGRAD: relu'(h2) rows, [cap][8] (see m2_word)
+    int seg_rays;                      // SEG: rays per problem; stats = the problems' statistics, problem = s_ray / seg_rays
 };
 
 // relu'(h2) of one sample as 8 words (32 B): quad thread t of the training kernel holds columns 8j + 2t + e (j = 0..31,
@@ -235,8 +237,11 @@ __device__ __forceinline__ void item_of(int i, int &stage, int &half) {
     else { half = 0; stage = 17 + (i - 34); }
 }
 
-template <bool TRAIN, bool WGRAD>
+// SEG (training without weight gradients only): the loss of nl_mlp_tc_train_batch -- every sample reads the loss constants of its
+// problem and adds its squared errors into that problem's sums; the per-sample arithmetic is the single-problem kernel's.
+template <bool TRAIN, bool WGRAD, bool SEG = false>
 __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
+    static_assert(!SEG || (TRAIN && !WGRAD), "the batched loss is for frozen-decoder training only");
     constexpr int IPT = TRAIN ? ITEMS_TRAIN : ITEMS_FWD;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -393,26 +398,44 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
         if constexpr (TRAIN) {
             // ---- loss (criterion.py:92-103) and d loss / d sdf for both rows ----
             float dsdf[2] = {0.f, 0.f};
+            int seg_k[2] = {-1, -1};                 // SEG: problem of each row (-1: no row)
+            double seg_fs[2] = {0.0, 0.0}, seg_sdf[2] = {0.0, 0.0};
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
                 const long long m = r ? m1 : m0;
                 const float s = r ? sdf1 : sdf0;
                 if (!(r ? live1 : live0)) continue;
-                if (p.dsdf_ext) { dsdf[r] = p.dsdf_ext[m]; continue; }
+                if (!SEG && p.dsdf_ext) { dsdf[r] = p.dsdf_ext[m]; continue; }
                 const uint32_t fl = p.s_flag[m];
                 const int ray = p.s_ray[m];
+                float gf = g_fs, gs = g_sdf;
+                if constexpr (SEG) {
+                    seg_k[r] = ray / p.seg_rays;
+                    gf = p.stats[seg_k[r]].g_fs;
+                    gs = p.stats[seg_k[r]].g_sdf;
+                }
                 const float z = __fmul_rn(p.s_depth[m], p.cosv ? p.cosv[ray] : 1.0f);
                 const float dgt = p.gt_depth[ray];
                 if (fl & 1u) {
                     const float e = s - 1.0f;
-                    if (t == 0) loss_fs += (double)e * (double)e;
-                    dsdf[r] += 2.0f * g_fs * e;
+                    if (t == 0) {
+                        if constexpr (SEG) seg_fs[r] = (double)e * (double)e;
+                        else loss_fs += (double)e * (double)e;
+                    }
+                    dsdf[r] += 2.0f * gf * e;
                 }
                 if (fl & 2u) {
                     const float e = __fsub_rn(__fadd_rn(z, __fmul_rn(s, p.truncation)), dgt);
-                    if (t == 0) loss_sdf += (double)e * (double)e;
-                    dsdf[r] += 2.0f * g_sdf * p.truncation * e;
+                    if (t == 0) {
+                        if constexpr (SEG) seg_sdf[r] = (double)e * (double)e;
+                        else loss_sdf += (double)e * (double)e;
+                    }
+                    dsdf[r] += 2.0f * gs * p.truncation * e;
                 }
+            }
+            if constexpr (SEG) {                     // one quad thread per row carries its squared errors
+#pragma unroll
+                for (int r = 0; r < 2; ++r) nl_seg_loss_add(p.stats, t == 0 ? seg_k[r] : -1, seg_fs[r], seg_sdf[r]);
             }
             if (WGRAD) {
                 if (t == 0) {
@@ -487,7 +510,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
             }
         }
     }
-    if (TRAIN && !p.dsdf_ext) {
+    if (TRAIN && !SEG && !p.dsdf_ext) {
         for (int off = 16; off > 0; off >>= 1) {
             loss_fs += __shfl_down_sync(0xffffffffu, loss_fs, off);
             loss_sdf += __shfl_down_sync(0xffffffffu, loss_sdf, off);
@@ -801,14 +824,14 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
     }
 }
 
-template <bool TRAIN, bool WGRAD>
+template <bool TRAIN, bool WGRAD, bool SEG = false>
 int launch(const Params &p, cudaStream_t stream) {
     static NlPerDevice configured;
-    const cudaError_t e = configured.once([] { return cudaFuncSetAttribute(k_mlp_wg<TRAIN, WGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL); });
+    const cudaError_t e = configured.once([] { return cudaFuncSetAttribute(k_mlp_wg<TRAIN, WGRAD, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL); });
     if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
     const long long ntiles = (p.M_host + TM - 1) / TM;
     const int grid = (int)(ntiles < (long long)nl_num_sms() ? ntiles : (long long)nl_num_sms());
-    k_mlp_wg<TRAIN, WGRAD><<<grid, NTHREADS, SMEM_TOTAL, stream>>>(p);
+    k_mlp_wg<TRAIN, WGRAD, SEG><<<grid, NTHREADS, SMEM_TOTAL, stream>>>(p);
     return NL_OK;
 }
 
@@ -888,5 +911,24 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
     tc::k_wgrad_tc<<<4 * nsplit, 256, tc::WG_SMEM, ws>>>(M, d_M_dev, feats, p.act_dh1, p.act_m2, p.act_d, p.panels, b0, W1, b1, w2, *grads,
                                                           nsplit);
     NL_CHECK_LAUNCH("nl_mlp_tc_train");
+    return NL_OK;
+}
+
+extern "C" int nl_mlp_tc_train_batch(int64_t M, const int32_t *d_M_dev, const float *feats, const void *panels, const float *b0, const float *b1,
+                                     const float *w2, const float *b2, const uint8_t *s_flag, const float *s_depth, const int32_t *s_ray,
+                                     const float *cosv, const float *gt_depth, nl_render_stats *problem_stats, int32_t rays_per_problem,
+                                     float truncation, float *sdf, float *dfeats, void *stream) {
+    if (M < 0) return nl_set_error("nl_mlp_tc_train_batch: negative M");
+    if (rays_per_problem <= 0) return nl_set_error("nl_mlp_tc_train_batch: rays_per_problem must be positive");
+    if (M == 0) return NL_OK;
+    if (!feats || !panels || !b0 || !b1 || !w2 || !b2 || !sdf || !dfeats || !s_flag || !s_depth || !s_ray || !gt_depth || !problem_stats)
+        return nl_set_error("nl_mlp_tc_train_batch: null pointer");
+    tc::Params p = {};
+    p.M_host = M; p.M_dev = d_M_dev; p.feats = feats; p.panels = (const uint8_t *)panels;
+    p.b0 = b0; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.sdf = sdf; p.dfeats = dfeats;
+    p.s_flag = s_flag; p.s_depth = s_depth; p.s_ray = s_ray; p.cosv = cosv; p.gt_depth = gt_depth; p.stats = problem_stats;
+    p.truncation = truncation; p.seg_rays = rays_per_problem;
+    if (int rc = tc::launch<true, false, true>(p, (cudaStream_t)stream)) return rc;
+    NL_CHECK_LAUNCH("nl_mlp_tc_train_batch");
     return NL_OK;
 }

@@ -24,3 +24,8 @@ extern "C" void nl_abi_sizes(int32_t out[4]) {
     out[2] = (int32_t)sizeof(nl_render_args);
     out[3] = (int32_t)sizeof(nl_mlp_weights);
 }
+
+extern "C" void nl_abi_sizes_batch(int32_t out[2]) {
+    out[0] = (int32_t)sizeof(nl_batch_args);
+    out[1] = NL_BATCH_MAX_PROBLEMS;
+}

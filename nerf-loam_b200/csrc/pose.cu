@@ -185,7 +185,44 @@ __global__ void __launch_bounds__(1024) k_pose_step(int F, float *__restrict__ p
     }
 }
 
+// k_pose_step for K independent problems: warp k = problem k's pose gradient, its Adam step under its own rate, step count and skip
+// flag (control block k), its loss read-out and the advance of its two seeds.
+__global__ void __launch_bounds__(1024) k_pose_step_batch(int K, float *__restrict__ pose6, const float *__restrict__ acc, float *__restrict__ grad6,
+                                                           float *__restrict__ m, float *__restrict__ v, const double *__restrict__ lr, double beta1,
+                                                           double beta2, float eps, const int32_t *__restrict__ ctl, nl_render_stats *stats,
+                                                           float fs_weight, float sdf_weight, float *__restrict__ last_loss, int32_t *seeds_a,
+                                                           int32_t inc_a, int32_t *seeds_b, int32_t inc_b) {
+    const int k = threadIdx.x >> 5, i = threadIdx.x & 31;
+    if (k >= K) return;                                  // warp-uniform
+    const int32_t *c = ctl + k * NL_CTL_WORDS;
+    const bool skip = c[NL_CTL_SKIP_NOW] != 0;
+    pose_grad_warp(k, pose6, acc, grad6);
+    __syncwarp();                                        // lanes 0..2 wrote grad6[k][0..5]; every lane has read pose6[k]
+    if (!skip && i < 6) {
+        const NlAdamConst a = nl_adam_const(lr[k], beta1, beta2, eps, c[NL_CTL_ADAM_STEP]);
+        nl_adam_f32_elem(a, grad6[k * 6 + i], pose6[k * 6 + i], m[k * 6 + i], v[k * 6 + i]);
+    }
+    if (i == 6 && stats) {
+        nl_loss_finalize_dev(stats + k, fs_weight, sdf_weight);
+        if (last_loss && !skip) last_loss[k] = stats[k].loss;
+    }
+    if (i == 7 && seeds_a) seeds_a[k] = (int32_t)((uint32_t)seeds_a[k] + (uint32_t)inc_a);
+    if (i == 8 && seeds_b) seeds_b[k] = (int32_t)((uint32_t)seeds_b[k] + (uint32_t)inc_b);
+}
+
 }  // namespace
+
+extern "C" int nl_pose_step_batch(int K, float *pose6, const float *acc, float *grad6, float *m, float *v, const double *d_lr, double beta1,
+                                  double beta2, double eps, const int32_t *d_ctl, nl_render_stats *d_problem_stats, float fs_weight,
+                                  float sdf_weight, float *d_last_loss, int32_t *d_seeds_a, int32_t inc_a, int32_t *d_seeds_b, int32_t inc_b,
+                                  void *stream) {
+    if (K < 1 || K > NL_BATCH_MAX_PROBLEMS) return nl_set_error("nl_pose_step_batch: need 1 <= n_problems <= 31");
+    if (!pose6 || !acc || !grad6 || !m || !v || !d_lr || !d_ctl) return nl_set_error("nl_pose_step_batch: null pointer");
+    k_pose_step_batch<<<1, K * 32, 0, (cudaStream_t)stream>>>(K, pose6, acc, grad6, m, v, d_lr, beta1, beta2, (float)eps, d_ctl, d_problem_stats,
+                                                              fs_weight, sdf_weight, d_last_loss, d_seeds_a, inc_a, d_seeds_b, inc_b);
+    NL_CHECK_LAUNCH("nl_pose_step_batch");
+    return NL_OK;
+}
 
 extern "C" int nl_pose_matrices(int F, const float *pose6, float *Rt12, void *stream) {
     if (F <= 0 || !pose6 || !Rt12) return nl_set_error("nl_pose_matrices: bad arguments");

@@ -527,6 +527,12 @@ struct SampleParams {
     uint8_t *s_flag;
     int32_t *ray_nsamp;
     const int32_t *ray_offset;
+    // batched problems (k_sample<., true>): N rays per problem, their statistics, first global hit rank, seeds, noise rows
+    int seg_n;
+    nl_render_stats *seg_stats;
+    const int32_t *seg_base;
+    const uint32_t *seg_seeds;
+    int noise_rows;
 };
 
 // criterion.py:67-82 for one cell: bit0 front_mask, bit1 sdf_mask
@@ -542,16 +548,30 @@ __device__ __forceinline__ uint32_t loss_flags(float z, float d, float trunc, fl
 // The [200, K', P] padding / 800-ray chunking of the reference wrapper only matters through the two
 // index quirks of the kernel tail (SURVEY A.3); they are reproduced from (q, R_hit, P) directly.
 // ------------------------------------------------------------------------------------------------
-template <bool FILL>
+// SEG: the q-th hit ray of the whole batch is hit ray q - base of its problem k = r / seg_n, and everything a solo call keys by
+// (rank, R_hit, P), the noise counter and the statistics are the problem's (nl_render_samples_batch); `stats` holds the totals.
+template <bool FILL, bool SEG = false>
 __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl_render_stats *stats) {
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    const int R_hit = stats->n_hit_rays;
+    const int q_all = blockIdx.x * blockDim.x + threadIdx.x;
+    const int R_all = stats->n_hit_rays;
     const int R = p.R;
     long long c_fs = 0, c_sdf = 0;
     int nsamp = 0, steps_ceil = 0;
-    if (q < R_hit) {
-        const int r = ws.hitray[q];
-        const int P = stats->max_hits;
+    int seg_k = -1;                                       // SEG: this thread's problem
+    nl_render_stats *ps = stats;                          // statistics this ray is counted in
+    if (q_all < R_all) {
+        const int r = ws.hitray[q_all];
+        int q = q_all, q_base = 0, R_hit = R_all;
+        uint32_t r_ctr = (uint32_t)r;                     // noise counter: the ray index within its problem
+        if constexpr (SEG) {
+            seg_k = r / p.seg_n;
+            ps = p.seg_stats + seg_k;
+            q_base = p.seg_base[seg_k];
+            q = q_all - q_base;
+            R_hit = ps->n_hit_rays;
+            r_ctr = (uint32_t)(r - seg_k * p.seg_n);
+        }
+        const int P = ps->max_hits;
         int32_t bidx[NL_MAX_HITS];
         float bmin[NL_MAX_HITS], bmax[NL_MAX_HITS], prob[NL_MAX_HITS];
         float tot = 0.f;
@@ -570,7 +590,7 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
             if (c < P) prob[c] = __fdiv_rn(prob[c], tot);                        // :576
         const float steps = __fdiv_rn(tot, p.step_size);                         // :577
         if (!FILL) {
-            if (tot > 10.0f * NL_MAX_DEPTH_FILL) atomicOr(&stats->error, 1);      // :579
+            if (tot > 10.0f * NL_MAX_DEPTH_FILL) atomicOr(&ps->error, 1);         // :579
             steps_ceil = nl_strata_count(steps);
         }
         // position of this ray in the reference's [200, K', P] layout and 800-wide launches (voxel_helpers.py:274-316)
@@ -578,7 +598,7 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
         const int b = q / Kp, j0 = q - b * Kp;
         const int ch = j0 / NL_SAMPLE_CHUNK, j = j0 - ch * NL_SAMPLE_CHUNK;
         const int num_rays = min(NL_SAMPLE_CHUNK, Kp - ch * NL_SAMPLE_CHUNK);
-        const int r_lead = ws.hitray[b * Kp + ch * NL_SAMPLE_CHUNK];            // ray 0 of this (batch, chunk)
+        const int r_lead = ws.hitray[q_base + b * Kp + ch * NL_SAMPLE_CHUNK];   // ray 0 of this (batch, chunk)
         const int H = j * P;
 
         const float cosr = p.cosv ? p.cosv[r] : 1.0f;
@@ -613,6 +633,8 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
         //      (batch, chunk) of num_rays rays: flush only while num_rays > j*P + bin; continuation test on the chunk's leader ray ----
         uint32_t seed = p.rng_seed;
         if (p.rng_seed_dev) { seed = *p.rng_seed_dev; seed = seed ? seed : 1u; }
+        if (SEG && p.seg_seeds) { seed = p.seg_seeds[seg_k]; seed = seed ? seed : 1u; }
+        const size_t noise_row0 = SEG ? (size_t)seg_k * p.noise_rows : 0;
         struct {
             const int32_t *i; const float *a, *b, *pr;
             __device__ __forceinline__ int idx(int c) const { return i[c]; }
@@ -623,8 +645,8 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
         nl_inverse_cdf_walk(
             P, bins, steps, -1.0f,
             [&](int i) {
-                if (p.noise) return p.noise[(size_t)q * p.noise_stride + i];
-                return seed ? hash_uniform(seed, (uint32_t)r, (uint32_t)i) : 0.5f;
+                if (p.noise) return p.noise[(noise_row0 + (size_t)q) * p.noise_stride + i];
+                return seed ? hash_uniform(seed, r_ctr, (uint32_t)i) : 0.5f;
             },
             [&](int vox, float z0, float z1) { emit(vox, __fmul_rn(__fadd_rn(z1, z0), 0.5f)); },
             [&](int bin) { return !p.compat || num_rays > (H + bin); },
@@ -635,17 +657,32 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
             if (with_loss) {  // padded cells of this row: z_vals = MAX_DEPTH (voxel_helpers.py:590), sdf = 1, valid = 0
                 const uint32_t fl = loss_flags(__fmul_rn(NL_MAX_DEPTH_FILL, cosr), gd, p.truncation, p.max_depth);
                 if (fl & 1u) {
-                    atomicAdd((unsigned long long *)&stats->pad_fs_rays, 1ULL);
-                    atomicAdd((unsigned long long *)&stats->pad_fs_nsamp, (unsigned long long)nsamp);
+                    atomicAdd((unsigned long long *)&ps->pad_fs_rays, 1ULL);
+                    atomicAdd((unsigned long long *)&ps->pad_fs_nsamp, (unsigned long long)nsamp);
                 }
                 if (fl & 2u) {
-                    atomicAdd((unsigned long long *)&stats->pad_sdf_rays, 1ULL);
-                    atomicAdd((unsigned long long *)&stats->pad_sdf_nsamp, (unsigned long long)nsamp);
-                    atomicAdd(&stats->pad_sdf_d2, (double)gd * (double)gd);
-                    atomicAdd(&stats->pad_sdf_d2_nsamp, (double)gd * (double)gd * (double)nsamp);
+                    atomicAdd((unsigned long long *)&ps->pad_sdf_rays, 1ULL);
+                    atomicAdd((unsigned long long *)&ps->pad_sdf_nsamp, (unsigned long long)nsamp);
+                    atomicAdd(&ps->pad_sdf_d2, (double)gd * (double)gd);
+                    atomicAdd(&ps->pad_sdf_d2_nsamp, (double)gd * (double)gd * (double)nsamp);
                 }
             }
         }
+    }
+    if (SEG && !FILL) {
+        // hit rays are in problem order, so a warp almost always holds one problem: warp-wide reductions then, else lane by lane
+        const int kmax = __reduce_max_sync(0xffffffffu, seg_k);
+        if (!__all_sync(0xffffffffu, seg_k < 0 || seg_k == kmax)) {
+            if (seg_k >= 0) {
+                if (nsamp > 0) atomicMax(&ps->max_samples, nsamp);
+                if (steps_ceil > 0) atomicMax(&ps->max_steps_ceil, steps_ceil);
+                if (c_fs) atomicAdd((unsigned long long *)&ps->cnt_fs_valid, (unsigned long long)c_fs);
+                if (c_sdf) atomicAdd((unsigned long long *)&ps->cnt_sdf_valid, (unsigned long long)c_sdf);
+            }
+            return;
+        }
+        if (kmax < 0) return;
+        stats = p.seg_stats + kmax;
     }
     if (!FILL) {
         const int wm = warp_max(nsamp);
@@ -664,7 +701,7 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p, Workspace ws, nl
 }
 
 // criterion.py:84-88 and the mean() denominators of :97-100
-__global__ void k_loss_prepare(nl_render_stats *s, float fs_weight, float sdf_weight) {
+__device__ __forceinline__ void loss_prepare_dev(nl_render_stats *s, float fs_weight, float sdf_weight) {
     const long long S = s->max_samples;
     const long long n_fs = s->cnt_fs_valid + s->pad_fs_rays * S - s->pad_fs_nsamp;
     const long long n_sdf = s->cnt_sdf_valid + s->pad_sdf_rays * S - s->pad_sdf_nsamp;
@@ -685,6 +722,53 @@ __global__ void k_loss_prepare(nl_render_stats *s, float fs_weight, float sdf_we
     s->loss = s->fs_loss = s->sdf_loss = 0.f;
 }
 
+__global__ void k_loss_prepare(nl_render_stats *s, float fs_weight, float sdf_weight) { loss_prepare_dev(s, fs_weight, sdf_weight); }
+
+// ---- batched problems (nl_render_samples_batch) ----
+// After the hit scan over the whole batch: block k finds problem k's first global hit rank (its hit rays are the contiguous run of
+// the compacted list that starts at the first ray >= k N), its R_hit and P, and turns its rays' global ranks into ranks within it.
+__global__ void __launch_bounds__(256) k_batch_hits(int N, const int32_t *__restrict__ nvalid, int32_t *__restrict__ hit_rank,
+                                                     const int32_t *__restrict__ hitray, const nl_render_stats *tot, nl_render_stats *ps,
+                                                     int32_t *__restrict__ base_out) {
+    __shared__ int s_base, s_max, s_cnt;
+    const int k = blockIdx.x, r0 = k * N;
+    if (threadIdx.x == 0) {
+        int lo = 0, hi = tot->n_hit_rays;                // lower bound of r0 in the ascending hitray[0, R_hit)
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (hitray[mid] < r0) lo = mid + 1; else hi = mid;
+        }
+        s_base = lo; s_max = 0; s_cnt = 0;
+    }
+    __syncthreads();
+    const int base = s_base;
+    int mx = 0, cnt = 0;
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+        const int nv = nvalid[r0 + i];
+        mx = max(mx, nv);
+        if (nv > 0) { ++cnt; hit_rank[r0 + i] -= base; }
+    }
+    mx = __reduce_max_sync(0xffffffffu, mx);
+    cnt = (int)__reduce_add_sync(0xffffffffu, (unsigned)cnt);
+    if ((threadIdx.x & 31) == 0) { atomicMax(&s_max, mx); atomicAdd(&s_cnt, cnt); }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        ps[k].max_hits = s_max;
+        ps[k].n_hit_rays = s_cnt;
+        base_out[k] = base;
+    }
+}
+
+// After the sample scan: problem k's samples are the run [ray_offset[k N], ray_offset[(k+1) N]) of the list; then its loss constants.
+__global__ void k_batch_finish(int K, int N, const int32_t *__restrict__ ray_offset, const nl_render_stats *tot, nl_render_stats *ps,
+                               int with_loss, float fs_weight, float sdf_weight) {
+    const int k = threadIdx.x;
+    if (k >= K) return;
+    const int end = k + 1 < K ? ray_offset[(k + 1) * N] : tot->n_samples;
+    ps[k].n_samples = end - ray_offset[k * N];
+    if (with_loss) loss_prepare_dev(ps + k, fs_weight, sdf_weight);
+}
+
 __global__ void k_loss_finalize(nl_render_stats *s, float fs_weight, float sdf_weight) { nl_loss_finalize_dev(s, fs_weight, sdf_weight); }
 
 // Fold one iteration's statistics into the call-wide control block (include/nerfloam_b200.h section 8).
@@ -700,6 +784,24 @@ __global__ void k_iter_status(const nl_render_stats *s, const int32_t *prev, int
     ctl[NL_CTL_MIN_HIT] = min(ctl[NL_CTL_MIN_HIT], s->n_hit_rays);
     ctl[NL_CTL_ITERS] += 1;
     ctl[NL_CTL_MAX_SAMPLES] = max(ctl[NL_CTL_MAX_SAMPLES], s->n_samples);
+}
+
+// The same per problem of a batch (include/nerfloam_b200.h section 8): a problem that hits nothing stops for the rest of the call.
+__global__ void k_iter_status_batch(int K, const nl_render_stats *tot, const nl_render_stats *ps, int32_t *ctl_all) {
+    const int k = threadIdx.x;
+    if (k >= K) return;
+    int32_t *ctl = ctl_all + k * NL_CTL_WORDS;
+    const nl_render_stats *s = ps + k;
+    const int err = (s->error & 1) | (tot->error & 6);
+    const int skip = ctl[NL_CTL_STOPPED] || (s->n_hit_rays <= 0) || (err & 1) || (s->n_samples <= 0);
+    ctl[NL_CTL_ERROR] |= err;
+    ctl[NL_CTL_SKIPPED] += skip;
+    ctl[NL_CTL_SKIP_NOW] = skip;
+    ctl[NL_CTL_STOPPED] = skip;
+    ctl[NL_CTL_ADAM_STEP] += skip ? 0 : 1;
+    ctl[NL_CTL_MIN_HIT] = min(ctl[NL_CTL_MIN_HIT], s->n_hit_rays);
+    ctl[NL_CTL_ITERS] += 1;
+    ctl[NL_CTL_MAX_SAMPLES] = max(ctl[NL_CTL_MAX_SAMPLES], tot->n_samples);
 }
 
 // Statistics exchange, packed (section 9): every value that must become global travels in one f64 vector reduced with SUM.
@@ -779,6 +881,15 @@ extern "C" int nl_stats_unpack_peers(nl_render_stats *d_stats, const double *con
     return NL_OK;
 }
 
+extern "C" int nl_iter_status_batch(int n_problems, const nl_render_stats *d_totals, const nl_render_stats *d_problem_stats, int32_t *d_ctl,
+                                    void *stream) {
+    if (n_problems < 1 || n_problems > NL_BATCH_MAX_PROBLEMS) return nl_set_error("nl_iter_status_batch: need 1 <= n_problems <= 31");
+    if (!d_totals || !d_problem_stats || !d_ctl) return nl_set_error("nl_iter_status_batch: null pointer");
+    k_iter_status_batch<<<1, 32, 0, (cudaStream_t)stream>>>(n_problems, d_totals, d_problem_stats, d_ctl);
+    NL_CHECK_LAUNCH("nl_iter_status_batch");
+    return NL_OK;
+}
+
 extern "C" int nl_iter_status(const nl_render_stats *d_stats, const int32_t *d_ctl_prev, int32_t *d_ctl, void *stream) {
     if (!d_stats || !d_ctl || !d_ctl_prev) return nl_set_error("nl_iter_status: null pointer");
     k_iter_status<<<1, 1, 0, (cudaStream_t)stream>>>(d_stats, d_ctl_prev, d_ctl);
@@ -832,8 +943,9 @@ extern "C" int64_t nl_render_workspace_bytes(int32_t n_rays) {
     return (int64_t)(3 * align256(4 * NL_MAX_HITS * R) + 2 * align256(4 * R) + align256(8 * 2 * SCAN_SCRATCH) + 256);
 }
 
-extern "C" int nl_render_samples(const nl_render_args *a, void *stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
+// nl_render_samples (b == NULL) and nl_render_samples_batch: one chain, the batch adds k_batch_hits after the hit scan, the problem
+// variant of the sampler and k_batch_finish in place of the loss preparation
+static int render_samples(const nl_render_args *a, const nl_batch_args *b, cudaStream_t stream) {
     if (!a) return nl_set_error("nl_render_samples: null args");
     if (a->n_rays <= 0 || a->n_nodes <= 0) return nl_set_error("nl_render_samples: n_rays and n_nodes must be positive");
     if (!a->d_centres || !a->d_structure || !a->d_ray_o || !a->d_ray_d || !a->d_stats || !a->d_hit_rank || !a->d_s_ray ||
@@ -845,6 +957,14 @@ extern "C" int nl_render_samples(const nl_render_args *a, void *stream_) {
     if ((((uintptr_t)a->d_ray_nsamp | (uintptr_t)a->d_ray_offset | (uintptr_t)a->d_hit_rank | (uintptr_t)a->d_workspace) & 15u) != 0)
         return nl_set_error("nl_render_samples: d_ray_nsamp, d_ray_offset, d_hit_rank and d_workspace must be 16-byte aligned");
     const int R = a->n_rays;
+    const int K = b ? b->n_problems : 1, N = R / K;
+    if (b) {
+        if (K < 1 || K > NL_BATCH_MAX_PROBLEMS || R % K != 0)
+            return nl_set_error("nl_render_samples_batch: need 1 <= n_problems <= 31 dividing n_rays");
+        if (!b->d_problem_stats || !b->d_problem_base) return nl_set_error("nl_render_samples_batch: null pointer");
+        if (a->d_noise && b->noise_rows <= 0) return nl_set_error("nl_render_samples_batch: noise_rows must be > 0 with d_noise");
+        cudaMemsetAsync(b->d_problem_stats, 0, sizeof(nl_render_stats) * K, stream);
+    }
     Workspace ws = carve(a->d_workspace, R);
     cudaMemsetAsync(a->d_stats, 0, sizeof(nl_render_stats), stream);
     const int blocks = nl_div_up(R, 128);
@@ -875,20 +995,40 @@ extern "C" int nl_render_samples(const nl_render_args *a, void *stream_) {
         k_scan_chained<SCAN_HITS><<<scan_tiles, 1024, 0, stream>>>(R, ws.nvalid, a->d_hit_rank, ws.hitray, a->d_stats, 0, ws.scan);
     } else if (scan_stage) k_scan<SCAN_HITS, true><<<1, 1024, 0, stream>>>(R, ws.nvalid, a->d_hit_rank, ws.hitray, a->d_stats, 0);
     else k_scan<SCAN_HITS, false><<<1, 1024, 0, stream>>>(R, ws.nvalid, a->d_hit_rank, ws.hitray, a->d_stats, 0);
-    SampleParams p;
+    if (b) k_batch_hits<<<K, 256, 0, stream>>>(N, ws.nvalid, a->d_hit_rank, ws.hitray, a->d_stats, b->d_problem_stats, b->d_problem_base);
+    SampleParams p = {};
     p.R = R; p.sample_capacity = a->sample_capacity; p.compat = a->reference_compat;
     p.step_size = a->step_size; p.truncation = a->truncation; p.max_depth = a->max_depth;
     p.ray_o = a->d_ray_o; p.ray_d = a->d_ray_d; p.gt_depth = a->d_gt_depth; p.cosv = a->d_cos; p.noise = a->d_noise;
     p.noise_stride = a->noise_stride; p.rng_seed = a->rng_seed; p.rng_seed_dev = a->d_noise ? nullptr : a->d_rng_seed;
     p.s_ray = a->d_s_ray; p.s_vox = a->d_s_vox; p.s_depth = a->d_s_depth; p.s_xyz = a->d_s_xyz; p.s_flag = a->d_s_flag;
     p.ray_nsamp = a->d_ray_nsamp; p.ray_offset = a->d_ray_offset;
-    k_sample<false><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
+    if (b) {
+        p.seg_n = N; p.seg_stats = b->d_problem_stats; p.seg_base = b->d_problem_base; p.seg_seeds = b->d_problem_seeds;
+        p.noise_rows = b->noise_rows;
+        k_sample<false, true><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
+    } else {
+        k_sample<false><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
+    }
     if (chained) k_scan_chained<SCAN_SAMPLES><<<scan_tiles, 1024, 0, stream>>>(R, a->d_ray_nsamp, a->d_ray_offset, nullptr, a->d_stats, a->sample_capacity, ws.scan + SCAN_SCRATCH);
     else k_scan<SCAN_SAMPLES><<<1, 1024, 0, stream>>>(R, a->d_ray_nsamp, a->d_ray_offset, nullptr, a->d_stats, a->sample_capacity);
-    k_sample<true><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
-    if (a->d_gt_depth) k_loss_prepare<<<1, 1, 0, stream>>>(a->d_stats, a->fs_weight, a->sdf_weight);
+    if (b) {
+        k_sample<true, true><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
+        k_batch_finish<<<1, 32, 0, stream>>>(K, N, a->d_ray_offset, a->d_stats, b->d_problem_stats, a->d_gt_depth != nullptr, a->fs_weight,
+                                             a->sdf_weight);
+    } else {
+        k_sample<true><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
+        if (a->d_gt_depth) k_loss_prepare<<<1, 1, 0, stream>>>(a->d_stats, a->fs_weight, a->sdf_weight);
+    }
     NL_CHECK_LAUNCH("nl_render_samples");
     return NL_OK;
+}
+
+extern "C" int nl_render_samples(const nl_render_args *a, void *stream) { return render_samples(a, nullptr, (cudaStream_t)stream); }
+
+extern "C" int nl_render_samples_batch(const nl_render_args *a, const nl_batch_args *b, void *stream) {
+    if (!b) return nl_set_error("nl_render_samples_batch: null batch args");
+    return render_samples(a, b, (cudaStream_t)stream);
 }
 
 extern "C" int nl_loss_prepare(nl_render_stats *d_stats, float fs_weight, float sdf_weight, void *stream) {

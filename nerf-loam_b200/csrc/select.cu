@@ -80,7 +80,7 @@ template <int CL>
 __global__ void __launch_bounds__(SEL_THREADS)
     k_select_rays(int cap, int n_select, const int64_t *__restrict__ n_points, const uint32_t *__restrict__ seed_dev, uint32_t seed_host,
                   const float *__restrict__ dirs_all, const float *__restrict__ gt_all, const float *__restrict__ cos_all, float *__restrict__ dirs,
-                  float *__restrict__ gt, float *__restrict__ cosv, int32_t *__restrict__ idx_out) {
+                  float *__restrict__ gt, float *__restrict__ cosv, int32_t *__restrict__ idx_out, const uint32_t *__restrict__ seeds) {
     __shared__ __align__(8) int hist[3][SEL_BINS];          // one histogram per pass: no barrier needed before re-use
     __shared__ int s_scan[36];
     __shared__ unsigned long long s_w[SEL_THREADS / 32];
@@ -90,7 +90,9 @@ __global__ void __launch_bounds__(SEL_THREADS)
     const int n = (int)min((long long)n_points[f], (long long)cap);
     const int N = min(n_select, n);
     uint32_t seed = seed_dev ? *seed_dev : seed_host;
-    seed = mix32(seed ^ 0x9E3779B9u * (uint32_t)(f + 1));
+    // seeds (nl_select_rays_batch): scan f is an independent problem with its own seed, drawn as frame 0 of a one-scan call
+    if (seeds) seed = seeds[f];
+    seed = mix32(seed ^ 0x9E3779B9u * (uint32_t)((seeds ? 0 : f) + 1));
     // this CTA's contiguous share of the scan, and inside it every thread's contiguous run (for the ordered emission)
     const int share = (n + CL - 1) / CL;
     const int c0 = min(c * share, n), c1 = min(c0 + share, n);
@@ -164,15 +166,15 @@ __global__ void __launch_bounds__(SEL_THREADS)
 
 }  // namespace
 
-extern "C" int nl_select_rays(int n_frames, int cap, int n_select, const int64_t *d_n_points, const uint32_t *d_seed, uint32_t seed,
-                              const float *d_dirs_all, const float *d_gt_all, const float *d_cos_all, float *d_dirs, float *d_gt, float *d_cos,
-                              int32_t *d_idx, void *stream) {
+static int select_rays(int n_frames, int cap, int n_select, const int64_t *d_n_points, const uint32_t *d_seed, uint32_t seed,
+                       const float *d_dirs_all, const float *d_gt_all, const float *d_cos_all, float *d_dirs, float *d_gt, float *d_cos,
+                       int32_t *d_idx, const uint32_t *d_seeds, void *stream) {
     if (n_frames <= 0 || cap <= 0 || n_select <= 0) return nl_set_error("nl_select_rays: sizes must be positive");
     if (!d_n_points || !d_dirs_all || !d_gt_all || !d_cos_all || !d_dirs || !d_gt || !d_cos) return nl_set_error("nl_select_rays: null pointer");
     static const bool single = [] { const char *e = getenv("NL_SEL_CLUSTER"); return e && e[0] == '0'; }();
     if (single) {
         k_select_rays<1><<<n_frames, SEL_THREADS, 0, (cudaStream_t)stream>>>(cap, n_select, d_n_points, d_seed, seed, d_dirs_all, d_gt_all, d_cos_all,
-                                                                                d_dirs, d_gt, d_cos, d_idx);
+                                                                                d_dirs, d_gt, d_cos, d_idx, d_seeds);
     } else {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(n_frames * SEL_CLUSTER);
@@ -183,9 +185,24 @@ extern "C" int nl_select_rays(int n_frames, int cap, int n_select, const int64_t
         at[0].val.clusterDim.x = SEL_CLUSTER; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
         const cudaError_t e = cudaLaunchKernelEx(&cfg, k_select_rays<SEL_CLUSTER>, cap, n_select, d_n_points, d_seed, seed, d_dirs_all, d_gt_all, d_cos_all,
-                                                 d_dirs, d_gt, d_cos, d_idx);
+                                                 d_dirs, d_gt, d_cos, d_idx, d_seeds);
         if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
     }
     NL_CHECK_LAUNCH("nl_select_rays");
     return NL_OK;
+}
+
+extern "C" int nl_select_rays(int n_frames, int cap, int n_select, const int64_t *d_n_points, const uint32_t *d_seed, uint32_t seed,
+                              const float *d_dirs_all, const float *d_gt_all, const float *d_cos_all, float *d_dirs, float *d_gt, float *d_cos,
+                              int32_t *d_idx, void *stream) {
+    return select_rays(n_frames, cap, n_select, d_n_points, d_seed, seed, d_dirs_all, d_gt_all, d_cos_all, d_dirs, d_gt, d_cos, d_idx, nullptr,
+                       stream);
+}
+
+extern "C" int nl_select_rays_batch(int n_problems, int cap, int n_select, const int64_t *d_n_points, const uint32_t *d_seeds,
+                                    const float *d_dirs_all, const float *d_gt_all, const float *d_cos_all, float *d_dirs, float *d_gt,
+                                    float *d_cos, int32_t *d_idx, void *stream) {
+    if (!d_seeds) return nl_set_error("nl_select_rays_batch: null seeds");
+    return select_rays(n_problems, cap, n_select, d_n_points, nullptr, 0u, d_dirs_all, d_gt_all, d_cos_all, d_dirs, d_gt, d_cos, d_idx, d_seeds,
+                       stream);
 }

@@ -395,9 +395,10 @@ class SDFEngine:
         _capi.LAUNCHES += 2
 
     def render_samples(self, m, R, cfg, ray_o=None, ray_d=None, gt_depth=None, cos=None, noise=None, rng_seed=0,
-                       reference_compat=True, rng_seed_dev=None):
+                       reference_compat=True, rng_seed_dev=None, batch=None):
         """rays -> compact sample list (nl_render_samples).  cfg: dict(voxel_size, step_size, max_distance,
-        truncation, max_depth, fs_weight, sdf_weight)."""
+        truncation, max_depth, fs_weight, sdf_weight).  batch: a _capi.BatchArgs -- R rays as K independent problems
+        (nl_render_samples_batch; `noise` is then f32[K * noise_rows, stride])."""
         assert R <= self.max_rays
         a = RenderArgs()
         a.n_rays, a.n_nodes, a.sample_capacity, a.reference_compat = R, m.n_nodes, self.max_samples, int(bool(reference_compat))
@@ -420,6 +421,10 @@ class SDFEngine:
         a.d_s_ray, a.d_s_vox, a.d_s_depth = self.s_ray.data_ptr(), self.s_vox.data_ptr(), self.s_depth.data_ptr()
         a.d_s_xyz, a.d_s_flag = self.s_xyz.data_ptr(), self.s_flag.data_ptr()
         a.d_ray_nsamp, a.d_ray_offset = self.ray_nsamp.data_ptr(), self.ray_offset.data_ptr()
+        if batch is not None:
+            _capi.check(_capi.lib().nl_render_samples_batch(C.byref(a), C.byref(batch), _capi.stream_ptr()), "nl_render_samples_batch")
+            _capi.LAUNCHES += 7
+            return
         _capi.check(_capi.lib().nl_render_samples(C.byref(a), _capi.stream_ptr()), "nl_render_samples")
         _capi.LAUNCHES += 6 if gt_depth is not None else 5
 

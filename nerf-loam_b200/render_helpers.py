@@ -782,3 +782,11 @@ def track_frame(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, 
     if n_last:
         hit_mask = (eng.hit_rank[:n_last] >= 0).clone()   # of the last iteration, like the reference's return value
     return init_pose, hit_mask
+
+
+def track_frames(frame_poses, frames, map_states, sdf_network, loss_criteria, voxel_size, N_rays=512, step_size=0.05, num_iterations=10,
+                 truncation=0.1, learning_rate=1e-3, max_voxel_hit=10, max_distance=10, **kw):
+    """K independent track_frame problems in one launch chain: track_batch.track_frames."""
+    from .track_batch import track_frames as _track_frames
+    return _track_frames(frame_poses, frames, map_states, sdf_network, loss_criteria, voxel_size, N_rays, step_size, num_iterations,
+                         truncation, learning_rate, max_voxel_hit, max_distance, **kw)
