@@ -310,10 +310,15 @@ NL_API int nl_render_samples(const nl_render_args *args, void *stream);
  *     Noise: args->d_noise (if given) is f32[K][noise_rows][noise_stride], rows by hit rank within the problem; otherwise problem
  *     k draws hash noise from d_problem_seeds[k] (0 is mapped to 1, as for args->d_rng_seed) with the ray index WITHIN the problem
  *     as counter, so under one seed it draws what a solo call draws; without d_problem_seeds every problem uses args' seed.
+ *     Scoring (render_helpers.score_poses): the front end and the loss alone take up to NL_SCORE_MAX_PROBLEMS problems -- K pose
+ *     hypotheses of one scan, which share rays and seed.  Tracking keeps at most NL_BATCH_MAX_PROBLEMS (its pose step and control
+ *     blocks).  The gap this fills: a lost scan is never re-localised; the reference falls back to the constant-velocity guess
+ *     (src/tracking.py:136-137).
  * -------------------------------------------------------------------------------------------- */
 #define NL_BATCH_MAX_PROBLEMS 31     /* the per-problem pose step runs one warp per problem in one block (as nl_pose_step) */
+#define NL_SCORE_MAX_PROBLEMS 65535  /* per-problem statistics stay at 160 B x K (about 10 MB) */
 typedef struct {
-    int32_t n_problems;                 /* K, 1 <= K <= NL_BATCH_MAX_PROBLEMS; args->n_rays must be a multiple of K */
+    int32_t n_problems;                 /* K, 1 <= K <= NL_SCORE_MAX_PROBLEMS; args->n_rays must be a multiple of K */
     int32_t noise_rows;                 /* rows per problem of args->d_noise */
     nl_render_stats *d_problem_stats;   /* [K] */
     const uint32_t *d_problem_seeds;    /* [K] or NULL */
@@ -321,6 +326,8 @@ typedef struct {
 } nl_batch_args;
 /* sizeof(nl_batch_args), NL_BATCH_MAX_PROBLEMS: checked by the bindings at load time like nl_abi_sizes */
 NL_API void nl_abi_sizes_batch(int32_t out[2]);
+/* NL_SCORE_MAX_PROBLEMS: checked by the bindings at load time */
+NL_API void nl_abi_sizes_score(int32_t out[1]);
 NL_API int nl_render_samples_batch(const nl_render_args *args, const nl_batch_args *batch, void *stream);
 
 /* ============================================================================================
@@ -397,9 +404,19 @@ NL_API int nl_mlp_tc_train_batch(int64_t M, const int32_t *d_M_dev, const float 
                                  const float *d_b1, const float *d_w2, const float *d_b2, const uint8_t *d_s_flag, const float *d_s_depth,
                                  const int32_t *d_s_ray, const float *d_cos, const float *d_gt_depth, nl_render_stats *d_problem_stats,
                                  int32_t rays_per_problem, float truncation, float *d_sdf, float *d_dfeats, void *stream);
+/* Scoring (section 3b, width 256): nl_mlp_tc_train_batch without the backward -- the forward layers, each problem's squared-error
+ * sums, and no d feats.  sdf is nl_mlp_tc_forward's bit for bit; each sample adds what nl_mlp_tc_train_batch adds. */
+NL_API int nl_mlp_tc_score_batch(int64_t M, const int32_t *d_M_dev, const float *d_feats, const void *d_panels, const float *d_b0,
+                                 const float *d_b1, const float *d_w2, const float *d_b2, const uint8_t *d_s_flag, const float *d_s_depth,
+                                 const int32_t *d_s_ray, const float *d_cos, const float *d_gt_depth, nl_render_stats *d_problem_stats,
+                                 int32_t rays_per_problem, float truncation, float *d_sdf, void *stream);
 /* loss constants from the sample statistics (criterion.py:84-88, 97-100); call after nl_render_samples */
 NL_API int nl_loss_prepare(nl_render_stats *d_stats, float fs_weight, float sdf_weight, void *stream);
 NL_API int nl_loss_finalize(nl_render_stats *d_stats, float fs_weight, float sdf_weight, void *stream);
+/* nl_loss_finalize on each of K <= NL_SCORE_MAX_PROBLEMS problem blocks; d_loss_out f32[K] = its loss, or NaN where render_rays
+ * returns None: no hit ray, error bit 0, or no sample */
+NL_API int nl_loss_finalize_batch(int n_problems, nl_render_stats *d_problem_stats, float fs_weight, float sdf_weight, float *d_loss_out,
+                                  void *stream);
 
 /* ============================================================================================
  * 6. SE(3) pose (src/se3pose.py): 6-vector [t, w] -> R(w) (11-term Taylor A,B), ray generation and

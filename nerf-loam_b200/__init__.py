@@ -12,6 +12,7 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     frame.LidarFrame                <- src/lidarFrame.py
     render_helpers.render_rays / bundle_adjust_frames / track_frame / get_scores  <- src/variations/render_helpers.py
     track_frames (= render_helpers.track_frames, track_batch)  K independent track_frame problems in one launch chain
+    score_poses / relocalise (= render_helpers.*, score)  the loss of up to 65 535 pose hypotheses of one scan; recovering a lost scan
     mapping.MapUpdater              <- Mapping.create_voxels / update_grid_features / get_embeddings (src/mapping.py)
     mesh.extract_mesh / marching_cubes  <- MeshExtractor.create_mesh / marching_cubes (src/utils/mesh_util.py)
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
@@ -20,13 +21,15 @@ no CPU or eager-PyTorch fallback for the kernels.
 from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
-           "track_batch", "track_frames"]
+           "track_batch", "track_frames", "score", "score_poses", "relocalise"]
 
 
 def __getattr__(name):
     import importlib
     if name == "track_frames":
         return importlib.import_module(".track_batch", __name__).track_frames
+    if name in ("score_poses", "relocalise"):
+        return getattr(importlib.import_module(".score", __name__), name)
     if name in __all__:
         return importlib.import_module("." + name, __name__)
     raise AttributeError(name)

@@ -144,12 +144,17 @@ _SIGNATURES = {
     "nl_pose_step_batch": (C.c_int, [C.c_int, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, vp, vp, C.c_float, C.c_float, vp,
                                      vp, C.c_int32, vp, C.c_int32, vp]),
     "nl_select_rays_batch": (C.c_int, [C.c_int, C.c_int, C.c_int] + [vp] * 10),
+    # scoring pose hypotheses (include/nerfloam_b200.h section 3b)
+    "nl_abi_sizes_score": (None, [C.POINTER(C.c_int32 * 1)]),
+    "nl_mlp_tc_score_batch": (C.c_int, [C.c_int64] + [vp] * 13 + [C.c_int32, C.c_float, vp, vp]),
+    "nl_loss_finalize_batch": (C.c_int, [C.c_int, vp, C.c_float, C.c_float, vp, vp]),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)
 CTL_ERROR, CTL_SKIPPED, CTL_SKIP_NOW, CTL_ADAM_STEP, CTL_MIN_HIT, CTL_ITERS, CTL_MAX_SAMPLES, CTL_WORDS = 0, 1, 2, 3, 4, 5, 6, 8
 CTL_STOPPED = 7              # batched control blocks only (nl_iter_status_batch)
 BATCH_MAX_PROBLEMS = 31      # NL_BATCH_MAX_PROBLEMS
+SCORE_MAX_PROBLEMS = 65535   # NL_SCORE_MAX_PROBLEMS
 STATS_PACK_FIXED = 10
 # node-array checks, bit i = 1 << i (NL_TREE_* in include/nerfloam_b200.h section 1)
 TREE_CHECKS = ("ROOT", "RANGE", "LINK", "PARENTS", "SHAPE", "ROWS", "VERTICES")
@@ -191,6 +196,10 @@ def lib():
         bmine = [C.sizeof(BatchArgs), BATCH_MAX_PROBLEMS]
         if list(bsizes) != bmine:
             raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (batch): {list(bsizes)} vs {bmine}")
+        ssizes = (C.c_int32 * 1)()
+        L.nl_abi_sizes_score(C.byref(ssizes))
+        if list(ssizes) != [SCORE_MAX_PROBLEMS]:
+            raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (score): {list(ssizes)} vs {[SCORE_MAX_PROBLEMS]}")
         _lib = L
     return _lib
 

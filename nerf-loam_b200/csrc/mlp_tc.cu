@@ -237,11 +237,12 @@ __device__ __forceinline__ void item_of(int i, int &stage, int &half) {
     else { half = 0; stage = 17 + (i - 34); }
 }
 
-// SEG (training without weight gradients only): the loss of nl_mlp_tc_train_batch -- every sample reads the loss constants of its
-// problem and adds its squared errors into that problem's sums; the per-sample arithmetic is the single-problem kernel's.
+// SEG (without weight gradients only): the loss of nl_mlp_tc_train_batch -- every sample reads the loss constants of its problem and
+// adds its squared errors into that problem's sums; the per-sample arithmetic is the single-problem kernel's.  SEG without TRAIN is
+// nl_mlp_tc_score_batch: the forward ring items, the same sums, no backward layers and no d feats.
 template <bool TRAIN, bool WGRAD, bool SEG = false>
 __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
-    static_assert(!SEG || (TRAIN && !WGRAD), "the batched loss is for frozen-decoder training only");
+    static_assert(!SEG || !WGRAD, "the batched loss is for a frozen decoder only");
     constexpr int IPT = TRAIN ? ITEMS_TRAIN : ITEMS_FWD;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -395,7 +396,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
             if (live0) p.sdf[m0] = sdf0;
             if (live1) p.sdf[m1] = sdf1;
         }
-        if constexpr (TRAIN) {
+        if constexpr (TRAIN || SEG) {
             // ---- loss (criterion.py:92-103) and d loss / d sdf for both rows ----
             float dsdf[2] = {0.f, 0.f};
             int seg_k[2] = {-1, -1};                 // SEG: problem of each row (-1: no row)
@@ -437,6 +438,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
 #pragma unroll
                 for (int r = 0; r < 2; ++r) nl_seg_loss_add(p.stats, t == 0 ? seg_k[r] : -1, seg_fs[r], seg_sdf[r]);
             }
+            if constexpr (!TRAIN) continue;          // scoring: the tile ends with its loss
             if (WGRAD) {
                 if (t == 0) {
                     if (live0) p.act_d[m0] = dsdf[0];
@@ -930,5 +932,24 @@ extern "C" int nl_mlp_tc_train_batch(int64_t M, const int32_t *d_M_dev, const fl
     p.truncation = truncation; p.seg_rays = rays_per_problem;
     if (int rc = tc::launch<true, false, true>(p, (cudaStream_t)stream)) return rc;
     NL_CHECK_LAUNCH("nl_mlp_tc_train_batch");
+    return NL_OK;
+}
+
+extern "C" int nl_mlp_tc_score_batch(int64_t M, const int32_t *d_M_dev, const float *feats, const void *panels, const float *b0, const float *b1,
+                                     const float *w2, const float *b2, const uint8_t *s_flag, const float *s_depth, const int32_t *s_ray,
+                                     const float *cosv, const float *gt_depth, nl_render_stats *problem_stats, int32_t rays_per_problem,
+                                     float truncation, float *sdf, void *stream) {
+    if (M < 0) return nl_set_error("nl_mlp_tc_score_batch: negative M");
+    if (rays_per_problem <= 0) return nl_set_error("nl_mlp_tc_score_batch: rays_per_problem must be positive");
+    if (M == 0) return NL_OK;
+    if (!feats || !panels || !b0 || !b1 || !w2 || !b2 || !sdf || !s_flag || !s_depth || !s_ray || !gt_depth || !problem_stats)
+        return nl_set_error("nl_mlp_tc_score_batch: null pointer");
+    tc::Params p = {};
+    p.M_host = M; p.M_dev = d_M_dev; p.feats = feats; p.panels = (const uint8_t *)panels;
+    p.b0 = b0; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.sdf = sdf;
+    p.s_flag = s_flag; p.s_depth = s_depth; p.s_ray = s_ray; p.cosv = cosv; p.gt_depth = gt_depth; p.stats = problem_stats;
+    p.truncation = truncation; p.seg_rays = rays_per_problem;
+    if (int rc = tc::launch<false, false, true>(p, (cudaStream_t)stream)) return rc;
+    NL_CHECK_LAUNCH("nl_mlp_tc_score_batch");
     return NL_OK;
 }

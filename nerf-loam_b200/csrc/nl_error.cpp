@@ -29,3 +29,5 @@ extern "C" void nl_abi_sizes_batch(int32_t out[2]) {
     out[0] = (int32_t)sizeof(nl_batch_args);
     out[1] = NL_BATCH_MAX_PROBLEMS;
 }
+
+extern "C" void nl_abi_sizes_score(int32_t out[1]) { out[0] = NL_SCORE_MAX_PROBLEMS; }

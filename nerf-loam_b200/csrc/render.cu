@@ -762,14 +762,24 @@ __global__ void __launch_bounds__(256) k_batch_hits(int N, const int32_t *__rest
 // After the sample scan: problem k's samples are the run [ray_offset[k N], ray_offset[(k+1) N]) of the list; then its loss constants.
 __global__ void k_batch_finish(int K, int N, const int32_t *__restrict__ ray_offset, const nl_render_stats *tot, nl_render_stats *ps,
                                int with_loss, float fs_weight, float sdf_weight) {
-    const int k = threadIdx.x;
-    if (k >= K) return;
-    const int end = k + 1 < K ? ray_offset[(k + 1) * N] : tot->n_samples;
-    ps[k].n_samples = end - ray_offset[k * N];
-    if (with_loss) loss_prepare_dev(ps + k, fs_weight, sdf_weight);
+    for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < K; k += gridDim.x * blockDim.x) {
+        const int end = k + 1 < K ? ray_offset[(k + 1) * N] : tot->n_samples;
+        ps[k].n_samples = end - ray_offset[k * N];
+        if (with_loss) loss_prepare_dev(ps + k, fs_weight, sdf_weight);
+    }
 }
 
 __global__ void k_loss_finalize(nl_render_stats *s, float fs_weight, float sdf_weight) { nl_loss_finalize_dev(s, fs_weight, sdf_weight); }
+
+// Each problem's loss, NaN where render_rays returns None (render_helpers.render_rays: no hit ray, error bit 0, no sample)
+__global__ void k_loss_finalize_batch(int K, nl_render_stats *ps, float fs_weight, float sdf_weight, float *loss) {
+    for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < K; k += gridDim.x * blockDim.x) {
+        nl_render_stats *s = ps + k;
+        nl_loss_finalize_dev(s, fs_weight, sdf_weight);
+        const bool none = s->n_hit_rays <= 0 || (s->error & 1) || s->n_samples <= 0;
+        loss[k] = none ? __int_as_float(0x7fffffff) : s->loss;
+    }
+}
 
 // Fold one iteration's statistics into the call-wide control block (include/nerfloam_b200.h section 8).
 __global__ void k_iter_status(const nl_render_stats *s, const int32_t *prev, int32_t *ctl) {
@@ -959,8 +969,8 @@ static int render_samples(const nl_render_args *a, const nl_batch_args *b, cudaS
     const int R = a->n_rays;
     const int K = b ? b->n_problems : 1, N = R / K;
     if (b) {
-        if (K < 1 || K > NL_BATCH_MAX_PROBLEMS || R % K != 0)
-            return nl_set_error("nl_render_samples_batch: need 1 <= n_problems <= 31 dividing n_rays");
+        if (K < 1 || K > NL_SCORE_MAX_PROBLEMS || R % K != 0)
+            return nl_set_error("nl_render_samples_batch: need 1 <= n_problems <= 65535 dividing n_rays");
         if (!b->d_problem_stats || !b->d_problem_base) return nl_set_error("nl_render_samples_batch: null pointer");
         if (a->d_noise && b->noise_rows <= 0) return nl_set_error("nl_render_samples_batch: noise_rows must be > 0 with d_noise");
         cudaMemsetAsync(b->d_problem_stats, 0, sizeof(nl_render_stats) * K, stream);
@@ -1014,8 +1024,8 @@ static int render_samples(const nl_render_args *a, const nl_batch_args *b, cudaS
     else k_scan<SCAN_SAMPLES><<<1, 1024, 0, stream>>>(R, a->d_ray_nsamp, a->d_ray_offset, nullptr, a->d_stats, a->sample_capacity);
     if (b) {
         k_sample<true, true><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
-        k_batch_finish<<<1, 32, 0, stream>>>(K, N, a->d_ray_offset, a->d_stats, b->d_problem_stats, a->d_gt_depth != nullptr, a->fs_weight,
-                                             a->sdf_weight);
+        k_batch_finish<<<nl_div_up(K, 256), 256, 0, stream>>>(K, N, a->d_ray_offset, a->d_stats, b->d_problem_stats, a->d_gt_depth != nullptr, a->fs_weight,
+                                                              a->sdf_weight);
     } else {
         k_sample<true><<<blocks, 128, 0, stream>>>(p, ws, a->d_stats);
         if (a->d_gt_depth) k_loss_prepare<<<1, 1, 0, stream>>>(a->d_stats, a->fs_weight, a->sdf_weight);
@@ -1042,5 +1052,15 @@ extern "C" int nl_loss_finalize(nl_render_stats *d_stats, float fs_weight, float
     if (!d_stats) return nl_set_error("nl_loss_finalize: null stats");
     k_loss_finalize<<<1, 1, 0, (cudaStream_t)stream>>>(d_stats, fs_weight, sdf_weight);
     NL_CHECK_LAUNCH("nl_loss_finalize");
+    return NL_OK;
+}
+
+extern "C" int nl_loss_finalize_batch(int n_problems, nl_render_stats *d_problem_stats, float fs_weight, float sdf_weight, float *d_loss_out,
+                                      void *stream) {
+    if (n_problems < 1 || n_problems > NL_SCORE_MAX_PROBLEMS) return nl_set_error("nl_loss_finalize_batch: need 1 <= n_problems <= 65535");
+    if (!d_problem_stats || !d_loss_out) return nl_set_error("nl_loss_finalize_batch: null pointer");
+    k_loss_finalize_batch<<<nl_div_up(n_problems, 256), 256, 0, (cudaStream_t)stream>>>(n_problems, d_problem_stats, fs_weight, sdf_weight,
+                                                                                          d_loss_out);
+    NL_CHECK_LAUNCH("nl_loss_finalize_batch");
     return NL_OK;
 }

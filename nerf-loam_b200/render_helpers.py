@@ -790,3 +790,15 @@ def track_frames(frame_poses, frames, map_states, sdf_network, loss_criteria, vo
     from .track_batch import track_frames as _track_frames
     return _track_frames(frame_poses, frames, map_states, sdf_network, loss_criteria, voxel_size, N_rays, step_size, num_iterations,
                          truncation, learning_rate, max_voxel_hit, max_distance, **kw)
+
+
+def score_poses(frame_poses, frame, map_states, sdf_network, loss_criteria, voxel_size, N_rays=512, step_size=0.05, max_distance=10, **kw):
+    """The loss of K pose hypotheses of one scan, forward only, in one launch chain per chunk: score.score_poses."""
+    from .score import score_poses as _score_poses
+    return _score_poses(frame_poses, frame, map_states, sdf_network, loss_criteria, voxel_size, N_rays, step_size, max_distance, **kw)
+
+
+def relocalise(frame, guess_pose, map_states, sdf_network, loss_criteria, voxel_size, **kw):
+    """Recover a lost scan's pose from a rough guess (yaw x translation search, then track_frames): score.relocalise."""
+    from .score import relocalise as _relocalise
+    return _relocalise(frame, guess_pose, map_states, sdf_network, loss_criteria, voxel_size, **kw)
