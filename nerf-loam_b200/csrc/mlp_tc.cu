@@ -40,7 +40,23 @@ constexpr int STEPS_TRAIN = 25;          // panel stages: layer 1, 8 x layer 2, 
 constexpr int ITEMS_FWD = 18;
 constexpr int ITEMS_TRAIN = 42;
 constexpr int NTHREADS = 256;
-constexpr int SMEM_TOTAL = NSLOT * SLOT + 3 * WN * 4 + 256 + 1024;   // ring + biases/w2 + barriers + alignment slack
+// k_mlp_wg's shared memory, from the 1024-aligned base: the ring, b0 / b1 / w2, the ring's mbarriers; training adds every thread's
+// relu'(h1) and relu'(h2) bits and loss sums (kept out of the register file so that ptxas need not serialise the wgmmas); weight
+// gradients add one staging area per warpgroup for the activations that leave through bulk copies.
+constexpr int SM_BIAS = NSLOT * SLOT;
+constexpr int SM_BAR = SM_BIAS + 3 * WN * 4;
+constexpr int SM_MASK = SM_BAR + 256;                     // mask1 [4][NTHREADS], mask2 [4][NTHREADS] words
+constexpr int SM_LOSS = SM_MASK + 2 * 4 * NTHREADS * 4;   // fs, sdf squared-error sums [2][NTHREADS] doubles
+constexpr int SM_STG = SM_LOSS + 2 * NTHREADS * 8;
+// Staging area of a warpgroup: one N = 128 half of dh1 for its 64 rows, pitch STG_LD floats (a half-warp's 8-byte stores of an
+// accumulator fragment hit 32 distinct banks; rows stay 16-byte aligned for the bulk copies), then its relu'(h2) words and dsdf.
+constexpr int STG_LD = 136;
+constexpr int STG_M2 = 64 * STG_LD * 4, STG_D = STG_M2 + 64 * 8 * 4, STG_WG = STG_D + 64 * 4;
+constexpr int SMEM_FWD = SM_MASK + 1024;                  // + alignment slack
+constexpr int SMEM_TRAIN = SM_STG + 1024;
+constexpr int SMEM_WGRAD = SM_STG + 2 * STG_WG + 1024;
+static_assert(SMEM_WGRAD <= 227 * 1024, "k_mlp_wg<train, wgrad> exceeds the 227 KB of shared memory a CTA may use");
+static_assert(SM_LOSS % 8 == 0 && SM_STG % 16 == 0 && STG_LD * 4 % 16 == 0 && STG_D % 16 == 0 && STG_WG % 16 == 0, "alignment");
 
 // byte offset of 16-byte chunk c (0..7) of row r inside a K-major SWIZZLE_128B panel
 __host__ __device__ __forceinline__ int panel_off(int r, int c) { return (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4); }
@@ -85,6 +101,22 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
                  "r"(bytes), "r"(bar) : "memory");
+}
+// shared -> global bulk copy, tracked in the issuing thread's bulk groups
+__device__ __forceinline__ void bulk_s2g(void *dst, uint32_t src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every bulk copy this thread committed has finished reading shared memory (the source may be overwritten)
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... and has completed its writes
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy shared-memory writes made visible to the async proxy (the bulk copies that read them)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier 1 + wg over the 128 threads of warpgroup wg (barrier 0 is __syncthreads')
+__device__ __forceinline__ void wg_bar_sync(int wg) {
+    if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+    else asm volatile("bar.sync 2, 128;" ::: "memory");
 }
 
 // ---- wgmma -------------------------------------------------------------------------------------------
@@ -249,15 +281,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
     const uint32_t base = (raw + 1023u) & ~1023u;    // SWIZZLE_128B panels need 1024-byte alignment
     uint8_t *sm = smem_raw + (base - raw);
     const uint32_t ring = base;
-    float *b0s = reinterpret_cast<float *>(sm + NSLOT * SLOT);
+    float *b0s = reinterpret_cast<float *>(sm + SM_BIAS);
     float *b1s = b0s + WN;
     float *w2s = b1s + WN;
-    const uint32_t bar0 = smem_u32(w2s + WN);       // FULL[s] at 8s, EMPTY[s] at 8 (NSLOT + s)
+    const uint32_t bar0 = base + SM_BAR;            // FULL[s] at 8s, EMPTY[s] at 8 (NSLOT + s)
     auto FULL = [&](uint32_t s) { return bar0 + 8u * s; };
     auto EMPTY = [&](uint32_t s) { return bar0 + 8u * (NSLOT + s); };
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
+    // TRAIN: relu'(h1) / relu'(h2) bit words i of this thread at [i * NTHREADS + tid]; squared-error sums at [tid], [NTHREADS + tid]
+    uint32_t *mask1s = reinterpret_cast<uint32_t *>(sm + SM_MASK), *mask2s = mask1s + 4 * NTHREADS;
+    double *lsum = reinterpret_cast<double *>(sm + SM_LOSS);
     const long long M = p.M_dev ? min((long long)*p.M_dev, p.M_host) : p.M_host;
     const long long ntiles = (M + TM - 1) / TM;
     const long long my_tiles = (long long)blockIdx.x < ntiles ? (ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
@@ -308,9 +343,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
     };
 
     const float b2 = p.b2[0];
-    float g_fs = 0.f, g_sdf = 0.f;
-    if (TRAIN && !p.dsdf_ext) { g_fs = p.stats->g_fs; g_sdf = p.stats->g_sdf; }
-    double loss_fs = 0.0, loss_sdf = 0.0;
+    if constexpr (TRAIN) { lsum[tid] = 0.0; lsum[NTHREADS + tid] = 0.0; }
 
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const long long m0 = tile * TM + warp * 16 + g, m1 = m0 + 8;   // this thread's two rows
@@ -344,17 +377,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 release();
             }
         }
-        // h1 = relu(D1 + b0), relu'(h1) bits: bit (4j + x) of the 128-bit mask
-        uint32_t mask1[4] = {0u, 0u, 0u, 0u}, mask2[4] = {0u, 0u, 0u, 0u};
+        // h1 = relu(D1 + b0), relu'(h1) bits: bit (4j + x) of the 128-bit mask, parked in shared memory until dh1
+        {
+            uint32_t mask1[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-        for (int j = 0; j < 32; ++j)
+            for (int j = 0; j < 32; ++j)
 #pragma unroll
-            for (int x = 0; x < 4; ++x) {
-                const float v = h[4 * j + x] + b0s[8 * j + 2 * t + (x & 1)];
-                const bool on = v > 0.f;
-                h[4 * j + x] = on ? v : 0.f;
-                if (on) mask1[j >> 3] |= 1u << ((j & 7) * 4 + x);
+                for (int x = 0; x < 4; ++x) {
+                    const float v = h[4 * j + x] + b0s[8 * j + 2 * t + (x & 1)];
+                    const bool on = v > 0.f;
+                    h[4 * j + x] = on ? v : 0.f;
+                    if (on) mask1[j >> 3] |= 1u << ((j & 7) * 4 + x);
+                }
+            if constexpr (TRAIN) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) mask1s[i * NTHREADS + tid] = mask1[i];
             }
+        }
 
         // ---- layer 2 (two N halves) + output layer partial sums ----
         float ps0 = 0.f, ps1 = 0.f;
@@ -375,18 +414,24 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 for (int ks = 0; ks < 4; ++ks) mma3<64>(d, ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
                 release();
             }
+            // relu'(h2) bits: bit (4j + x) of the 128-bit mask (j = 16 half + jj), words 2 half and 2 half + 1 of it
+            uint32_t mask2[2] = {0u, 0u};
 #pragma unroll
             for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
                 for (int x = 0; x < 4; ++x) {
-                    const int col = 128 * half + 8 * jj + 2 * t + (x & 1), j = 16 * half + jj;
+                    const int col = 128 * half + 8 * jj + 2 * t + (x & 1);
                     const float v = d[4 * jj + x] + b1s[col];
                     const bool on = v > 0.f;
                     const float hv = on ? v : 0.f;
                     d[4 * jj + x] = hv;
-                    if (on) mask2[j >> 3] |= 1u << ((j & 7) * 4 + x);
+                    if (on) mask2[jj >> 3] |= 1u << ((jj & 7) * 4 + x);
                     if (x < 2) ps0 = fmaf(hv, w2s[col], ps0); else ps1 = fmaf(hv, w2s[col], ps1);
                 }
+            if constexpr (TRAIN) {
+                mask2s[(2 * half) * NTHREADS + tid] = mask2[0];
+                mask2s[(2 * half + 1) * NTHREADS + tid] = mask2[1];
+            }
         }
         // the 4 threads of a quad hold the 4 column classes of the same two rows
         ps0 += __shfl_xor_sync(0xffffffffu, ps0, 1); ps0 += __shfl_xor_sync(0xffffffffu, ps0, 2);
@@ -409,19 +454,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 if (!SEG && p.dsdf_ext) { dsdf[r] = p.dsdf_ext[m]; continue; }
                 const uint32_t fl = p.s_flag[m];
                 const int ray = p.s_ray[m];
-                float gf = g_fs, gs = g_sdf;
-                if constexpr (SEG) {
-                    seg_k[r] = ray / p.seg_rays;
-                    gf = p.stats[seg_k[r]].g_fs;
-                    gs = p.stats[seg_k[r]].g_sdf;
-                }
+                int k = 0;
+                if constexpr (SEG) k = seg_k[r] = ray / p.seg_rays;
+                const float gf = p.stats[k].g_fs, gs = p.stats[k].g_sdf;
                 const float z = __fmul_rn(p.s_depth[m], p.cosv ? p.cosv[ray] : 1.0f);
                 const float dgt = p.gt_depth[ray];
                 if (fl & 1u) {
                     const float e = s - 1.0f;
                     if (t == 0) {
                         if constexpr (SEG) seg_fs[r] = (double)e * (double)e;
-                        else loss_fs += (double)e * (double)e;
+                        else lsum[tid] += (double)e * (double)e;
                     }
                     dsdf[r] += 2.0f * gf * e;
                 }
@@ -429,7 +471,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                     const float e = __fsub_rn(__fadd_rn(z, __fmul_rn(s, p.truncation)), dgt);
                     if (t == 0) {
                         if constexpr (SEG) seg_sdf[r] = (double)e * (double)e;
-                        else loss_sdf += (double)e * (double)e;
+                        else lsum[NTHREADS + tid] += (double)e * (double)e;
                     }
                     dsdf[r] += 2.0f * gs * p.truncation * e;
                 }
@@ -439,17 +481,57 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 for (int r = 0; r < 2; ++r) nl_seg_loss_add(p.stats, t == 0 ? seg_k[r] : -1, seg_fs[r], seg_sdf[r]);
             }
             if constexpr (!TRAIN) continue;          // scoring: the tile ends with its loss
+            // WGRAD: the activation buffer rows of this warpgroup leave through bulk copies from its staging area (dh1 half | relu'(h2)
+            // words | dsdf).  The first warp's lanes issue them (two dh1 rows each); a staged half is overwritten only after those lanes
+            // saw their copies finish reading it and the warpgroup passed a barrier behind them.  Everything here is derived from tid
+            // and tile where it is used.
+            auto staging = [&]() { return reinterpret_cast<float *>(sm + SM_STG + (warp >> 2) * STG_WG); };
             if (WGRAD) {
-                if (t == 0) {
-                    if (live0) p.act_d[m0] = dsdf[0];
-                    if (live1) p.act_d[m1] = dsdf[1];
+                const int lr = (warp & 3) * 16 + g;   // this thread's rows inside the warpgroup's 64: lr, lr + 8
+                // mask2 bit 4j + x: row x >> 1, column 8j + 2t + (x & 1).  The previous tile's copies of these words finished reading
+                // them before its second dh1 half was staged.
+                uint32_t w[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) w[i] = mask2s[i * NTHREADS + tid];
+                uint32_t *stg_m2 = reinterpret_cast<uint32_t *>(staging() + STG_M2 / 4);
+                *reinterpret_cast<uint2 *>(stg_m2 + lr * 8 + 2 * t) =
+                    make_uint2(m2_pack(w[0]) | m2_pack(w[1]) << 16, m2_pack(w[2]) | m2_pack(w[3]) << 16);
+                *reinterpret_cast<uint2 *>(stg_m2 + (lr + 8) * 8 + 2 * t) =
+                    make_uint2(m2_pack(w[0] >> 2) | m2_pack(w[1] >> 2) << 16, m2_pack(w[2] >> 2) | m2_pack(w[3] >> 2) << 16);
+                if (t == 0) {   // dsdf leaves in whole 16-byte pieces of 4 rows; the rows of a partly live piece are stored directly
+                    float *stg_d = staging() + STG_D / 4;
+                    stg_d[lr] = dsdf[0];
+                    stg_d[lr + 8] = dsdf[1];
+                    if (live0 && (m0 | 3) >= M) p.act_d[m0] = dsdf[0];
+                    if (live1 && (m1 | 3) >= M) p.act_d[m1] = dsdf[1];
                 }
-                // mask2 bit 4j + x: row x >> 1, column 8j + 2t + (x & 1)
-                if (live0) *reinterpret_cast<uint2 *>(p.act_m2 + (size_t)m0 * 8 + 2 * t) =
-                    make_uint2(m2_pack(mask2[0]) | m2_pack(mask2[1]) << 16, m2_pack(mask2[2]) | m2_pack(mask2[3]) << 16);
-                if (live1) *reinterpret_cast<uint2 *>(p.act_m2 + (size_t)m1 * 8 + 2 * t) =
-                    make_uint2(m2_pack(mask2[0] >> 2) | m2_pack(mask2[1] >> 2) << 16, m2_pack(mask2[2] >> 2) | m2_pack(mask2[3] >> 2) << 16);
             }
+            // stage dh1 columns 128 hh .. 128 hh + 127 (and with hh = 0 the relu'(h2) words and dsdf) and start their copies
+            auto stage_half = [&](int hh) {
+                const int wg = warp >> 2, lr = (warp & 3) * 16 + g;
+                float *stg = staging();
+                if ((warp & 3) == 0) bulk_wait_read();
+                wg_bar_sync(wg);
+#pragma unroll
+                for (int jj = 0; jj < 16; ++jj) {
+                    const int j = 16 * hh + jj;
+                    *reinterpret_cast<float2 *>(stg + lr * STG_LD + 8 * jj + 2 * t) = make_float2(h[4 * j], h[4 * j + 1]);
+                    *reinterpret_cast<float2 *>(stg + (lr + 8) * STG_LD + 8 * jj + 2 * t) = make_float2(h[4 * j + 2], h[4 * j + 3]);
+                }
+                fence_proxy_async();
+                wg_bar_sync(wg);
+                if ((warp & 3) == 0) {
+                    const long long r0 = tile * TM + 64 * wg;               // rows r0 .. r0 + nrows - 1
+                    const int nrows = (int)min(max(M - r0, 0LL), 64LL);
+                    for (int r = lane; r < nrows; r += 32)
+                        bulk_s2g(p.act_dh1 + (size_t)(r0 + r) * WN + 128 * hh, smem_u32(stg + r * STG_LD), 128 * 4);
+                    if (hh == 0 && lane == 0 && nrows > 0) {
+                        bulk_s2g(p.act_m2 + (size_t)r0 * 8, smem_u32(stg + STG_M2 / 4), nrows * 8 * 4);
+                        if (nrows >= 4) bulk_s2g(p.act_d + r0, smem_u32(stg + STG_D / 4), (nrows & ~3) * 4);
+                    }
+                    bulk_commit();
+                }
+            };
             // ---- backward layer 2: D3 = relu'(h2) . (diag(w2) W1).  The A operand is the 0/1 mask (exact in tf32: 2 terms) ----
 #pragma unroll
             for (int i = 0; i < 128; ++i) h[i] = 0.f;
@@ -458,10 +540,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
 #pragma unroll
                 for (int kb = 0; kb < 8; ++kb) {
                     uint32_t a[4][4];
+                    const uint32_t wk = mask2s[(kb >> 1) * NTHREADS + tid];
 #pragma unroll
                     for (int ks = 0; ks < 4; ++ks) {
                         const int j = 4 * kb + ks;
-                        const uint32_t w = mask2[j >> 3] >> ((j & 7) * 4);
+                        const uint32_t w = wk >> ((j & 7) * 4);
                         a[ks][0] = (w & 1u) ? 0x3f800000u : 0u; a[ks][1] = (w & 4u) ? 0x3f800000u : 0u;
                         a[ks][2] = (w & 2u) ? 0x3f800000u : 0u; a[ks][3] = (w & 8u) ? 0x3f800000u : 0u;
                     }
@@ -478,23 +561,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
             }
             // dh1 = dsdf * D3 * relu'(h1)
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
+            for (int i = 0; i < 4; ++i) {
+                const uint32_t m1w = mask1s[i * NTHREADS + tid];
 #pragma unroll
-                for (int x = 0; x < 4; ++x)
-                    h[4 * j + x] = ((mask1[j >> 3] >> ((j & 7) * 4 + x)) & 1u) ? dsdf[x >> 1] * h[4 * j + x] : 0.f;
-            if (WGRAD) {
+                for (int j = 8 * i; j < 8 * i + 8; ++j)
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    if (live0) *reinterpret_cast<float2 *>(p.act_dh1 + (size_t)m0 * WN + 8 * j + 2 * t) = make_float2(h[4 * j], h[4 * j + 1]);
-                    if (live1) *reinterpret_cast<float2 *>(p.act_dh1 + (size_t)m1 * WN + 8 * j + 2 * t) = make_float2(h[4 * j + 2], h[4 * j + 3]);
-                }
+                    for (int x = 0; x < 4; ++x)
+                        h[4 * j + x] = ((m1w >> ((j & 7) * 4 + x)) & 1u) ? dsdf[x >> 1] * h[4 * j + x] : 0.f;
             }
-            // ---- backward layer 1: d x = dh1 . W0 (N = 16) ----
+            // ---- backward layer 1: d x = dh1 . W0 (N = 16); each dh1 half is staged and copied out before its K-blocks ----
             float dx[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) dx[i] = 0.f;
 #pragma unroll
             for (int kb = 0; kb < 8; ++kb) {
+                if (WGRAD && kb % 4 == 0) stage_half(kb / 4);
                 uint32_t ah[4][4], al[4][4];
 #pragma unroll
                 for (int ks = 0; ks < 4; ++ks) frag3(h, 4 * kb + ks, ah[ks], al[ks]);
@@ -512,7 +593,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
             }
         }
     }
+    if (WGRAD && (warp & 3) == 0) bulk_wait();   // the staging areas stay valid until the copies out of them have completed
     if (TRAIN && !SEG && !p.dsdf_ext) {
+        // every thread's sums in the order it added them, then over the warp: the same fp64 partials as register accumulators
+        double loss_fs = lsum[tid], loss_sdf = lsum[NTHREADS + tid];
         for (int off = 16; off > 0; off >>= 1) {
             loss_fs += __shfl_down_sync(0xffffffffu, loss_fs, off);
             loss_sdf += __shfl_down_sync(0xffffffffu, loss_sdf, off);
@@ -828,12 +912,13 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
 
 template <bool TRAIN, bool WGRAD, bool SEG = false>
 int launch(const Params &p, cudaStream_t stream) {
+    constexpr int smem = WGRAD ? SMEM_WGRAD : TRAIN ? SMEM_TRAIN : SMEM_FWD;
     static NlPerDevice configured;
-    const cudaError_t e = configured.once([] { return cudaFuncSetAttribute(k_mlp_wg<TRAIN, WGRAD, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL); });
+    const cudaError_t e = configured.once([] { return cudaFuncSetAttribute(k_mlp_wg<TRAIN, WGRAD, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
     if (e != cudaSuccess) return nl_set_error_code(NL_ERR_CUDA, cudaGetErrorString(e));
     const long long ntiles = (p.M_host + TM - 1) / TM;
     const int grid = (int)(ntiles < (long long)nl_num_sms() ? ntiles : (long long)nl_num_sms());
-    k_mlp_wg<TRAIN, WGRAD, SEG><<<grid, NTHREADS, SMEM_TOTAL, stream>>>(p);
+    k_mlp_wg<TRAIN, WGRAD, SEG><<<grid, NTHREADS, smem, stream>>>(p);
     return NL_OK;
 }
 
