@@ -381,18 +381,20 @@ NL_API int nl_mlp_tc_prepare(const float *d_W0, const float *d_W1, const float *
 NL_API int nl_mlp_tc_forward(int64_t M, const int32_t *d_M_dev, const float *d_feats, const void *d_panels, const float *d_b0,
                       const float *d_b1, const float *d_w2, const float *d_b2, float *d_sdf, void *stream);
 /* Tensor-core forward + loss + backward (same contract as nl_mlp_train, width 256 only).  With grads != NULL d_act is a
- * scratch buffer of nl_mlp_tc_act_floats(M) floats: dh1, the relu'(h2) bits and d loss / d sdf per sample (h1 is recomputed
- * from d_feats by the weight-gradient kernel).
+ * scratch buffer of nl_mlp_tc_act_floats(M) floats: the relu'(h2) bits [cap][8 words] and d loss / d sdf [cap] per sample, which
+ * the weight-gradient kernel reads (h1 is recomputed from d_feats; gW0 and gb0 are formed by the forward/backward kernel).
+ * d_act_dh1 (may be NULL): if given, nl_mlp_tc_dh1_floats(M) floats that receive dh1 [cap][256] as well; no gradient needs it.
  * The panels must have been prepared from the same W0 / W1 / w2 (the backward panels hold diag(w2) W1).
  * wgrad_stream (may be NULL = stream): the weight-gradient kernel is enqueued there, ordered after the forward/backward
  * kernel by an event, so that it overlaps with later work on `stream`; the caller joins the two streams before it reads
  * `grads`, reuses d_act, changes d_feats or d_panels or changes d_b0 / d_W1 / d_b1 / d_w2 (the weight-gradient kernel reads them). */
 NL_API int64_t nl_mlp_tc_act_floats(int64_t M);
+NL_API int64_t nl_mlp_tc_dh1_floats(int64_t M);
 NL_API int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *d_feats, const void *d_panels, const float *d_W1,
                     const float *d_b0, const float *d_b1, const float *d_w2, const float *d_b2, const uint8_t *d_s_flag, const float *d_s_depth,
                     const int32_t *d_s_ray, const float *d_cos, const float *d_gt_depth, nl_render_stats *d_stats, float truncation,
-                    float *d_sdf, float *d_dfeats, const nl_mlp_grads *grads, float *d_act, const float *d_dsdf_ext, void *wgrad_stream,
-                    void *stream);
+                    float *d_sdf, float *d_dfeats, const nl_mlp_grads *grads, float *d_act, float *d_act_dh1, const float *d_dsdf_ext,
+                    void *wgrad_stream, void *stream);
 /* Batched loss for a frozen decoder (no weight gradients; the samples of nl_render_samples_batch): sample m belongs to problem
  * d_s_ray[m] / rays_per_problem, reads that problem's loss constants in d_problem_stats and adds its squared errors into that
  * problem's fs_sum / sdf_sum.  sdf and dfeats are per sample the single-problem kernels' values bit for bit. */

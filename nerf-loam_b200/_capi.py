@@ -108,8 +108,9 @@ _SIGNATURES = {
     "nl_mlp_tc_prepare": (C.c_int, [vp, vp, vp, vp, vp]),
     "nl_mlp_tc_forward": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "nl_mlp_tc_act_floats": (C.c_int64, [C.c_int64]),
+    "nl_mlp_tc_dh1_floats": (C.c_int64, [C.c_int64]),
     "nl_mlp_tc_train": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, C.POINTER(MlpGrads),
-                                  vp, vp, vp, vp]),
+                                  vp, vp, vp, vp, vp]),
     "nl_octree_packed_bytes": (C.c_int64, [C.c_int32]),
     "nl_octree_pack_children": (C.c_int, [C.c_int32, vp, vp, vp, vp]),
     "nl_loss_prepare": (C.c_int, [vp, C.c_float, C.c_float, vp]),

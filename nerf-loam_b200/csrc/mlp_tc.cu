@@ -14,14 +14,15 @@
 // Per 128-sample training tile the ring carries 42 items: layer 1 (2 halves), layer 2 (2 halves x 8 K-blocks of 32),
 // backward layer 2 (2 x 8) and backward layer 1 (8 K-blocks, N = 16).
 //
-// Decoder weight gradients (nl_mlp_tc_train with grads): the training kernel stores dh1 [cap][256], the relu'(h2) bits
-// (32 B per sample) and d loss / d sdf.  The output layer has one unit, so dh2 = dsdf * w2 * m2 (m2 = relu'(h2)) and everything
+// Decoder weight gradients (nl_mlp_tc_train with grads): the training kernel forms gW0 = dh1^T x and gb0 = sum dh1 itself, from
+// dh1 staged in shared memory during backward layer 1, and stores the relu'(h2) bits (32 B per sample) and d loss / d sdf (and,
+// only when asked to, dh1 [cap][256]).  The output layer has one unit, so dh2 = dsdf * w2 * m2 (m2 = relu'(h2)) and everything
 // that would read h2 or dh2 follows from G = m2^T (dsdf * h1) and c = m2^T dsdf:
 //   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c
 // h1 = relu(x W0^T + b0) is not stored: its input x (K = 16, 64 B per sample) is, and recomputing h1 costs a tenth of G.  One
 // split-K kernel (k_wgrad_tc) recomputes h1 and forms G on wgmma, both transposed so that the sample is wgmma's K: h1^T = W0 x^T
 // with A = W0 from registers and B = x (K-major as stored), then G^T = (dsdf h1)^T m2 with A = the h1^T accumulator from
-// registers and B = the exact 0/1 mask expanded into a K-major tile.  gW0 = dh1^T x (mma.sync) and the column sums run beside it.
+// registers and B = the exact 0/1 mask expanded into a K-major tile.  The column sums c and gb2 run beside it.
 #include <mutex>
 
 #include "loss.cuh"
@@ -42,21 +43,30 @@ constexpr int ITEMS_TRAIN = 42;
 constexpr int NTHREADS = 256;
 // k_mlp_wg's shared memory, from the 1024-aligned base: the ring, b0 / b1 / w2, the ring's mbarriers; training adds every thread's
 // relu'(h1) and relu'(h2) bits and loss sums (kept out of the register file so that ptxas need not serialise the wgmmas); weight
-// gradients add one staging area per warpgroup for the activations that leave through bulk copies.
+// gradients add one staging area per warpgroup for dh1 and the activations that leave through bulk copies, and the CTA's gW0 / gb0
+// sums.
 constexpr int SM_BIAS = NSLOT * SLOT;
 constexpr int SM_BAR = SM_BIAS + 3 * WN * 4;
 constexpr int SM_MASK = SM_BAR + 256;                     // mask1 [4][NTHREADS], mask2 [4][NTHREADS] words
 constexpr int SM_LOSS = SM_MASK + 2 * 4 * NTHREADS * 4;   // fs, sdf squared-error sums [2][NTHREADS] doubles
 constexpr int SM_STG = SM_LOSS + 2 * NTHREADS * 8;
-// Staging area of a warpgroup: one N = 128 half of dh1 for its 64 rows, pitch STG_LD floats (a half-warp's 8-byte stores of an
-// accumulator fragment hit 32 distinct banks; rows stay 16-byte aligned for the bulk copies), then its relu'(h2) words and dsdf.
-constexpr int STG_LD = 136;
+// Staging area of a warpgroup: one N = 64 quarter of dh1 for its 64 rows, pitch STG_LD floats (STG_LD = 8 mod 32: a half-warp's
+// 8-byte stores of an accumulator fragment and a warp's mma.sync B-fragment loads -- sample t / t + 4, column g -- hit 32 distinct
+// banks; rows stay 16-byte aligned for the bulk copies), then its relu'(h2) words and dsdf.
+constexpr int STG_LD = 72;
 constexpr int STG_M2 = 64 * STG_LD * 4, STG_D = STG_M2 + 64 * 8 * 4, STG_WG = STG_D + 64 * 4;
+// gW0 [2][256][16] then gb0 [2][256] floats, summed over the CTA's tiles: one copy per warpgroup, every entry of a copy owned by
+// one thread, so they need no atomics.  Then each warpgroup's x tile: its 64 rows' features, [64][16] floats, row s holding feature
+// e at column e ^ xt_swz(s), so that the gW0 A-fragment loads (sample t / t + 4, feature g / g + 8) hit 32 distinct banks.
+constexpr int SM_GW0 = SM_STG + 2 * STG_WG, SM_GB0 = SM_GW0 + 2 * WN * 16 * 4, SM_XT = SM_GB0 + 2 * WN * 4;
 constexpr int SMEM_FWD = SM_MASK + 1024;                  // + alignment slack
 constexpr int SMEM_TRAIN = SM_STG + 1024;
-constexpr int SMEM_WGRAD = SM_STG + 2 * STG_WG + 1024;
+constexpr int SMEM_WGRAD = SM_XT + 2 * 64 * 16 * 4 + 1024;
 static_assert(SMEM_WGRAD <= 227 * 1024, "k_mlp_wg<train, wgrad> exceeds the 227 KB of shared memory a CTA may use");
-static_assert(SM_LOSS % 8 == 0 && SM_STG % 16 == 0 && STG_LD * 4 % 16 == 0 && STG_D % 16 == 0 && STG_WG % 16 == 0, "alignment");
+static_assert(SM_LOSS % 8 == 0 && SM_STG % 16 == 0 && STG_LD * 4 % 16 == 0 && STG_D % 16 == 0 && STG_WG % 16 == 0 && SM_GW0 % 16 == 0 && SM_XT % 16 == 0,
+              "alignment");
+static_assert(STG_LD % 32 == 8, "bank-conflict-free staging stores and B-fragment loads");
+__host__ __device__ __forceinline__ int xt_swz(int s) { return (s & 2) << 2; }
 
 // byte offset of 16-byte chunk c (0..7) of row r inside a K-major SWIZZLE_128B panel
 __host__ __device__ __forceinline__ int panel_off(int r, int c) { return (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4); }
@@ -113,6 +123,17 @@ __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.w
 __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // generic-proxy shared-memory writes made visible to the async proxy (the bulk copies that read them)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// v += x for a float in shared memory owned by this thread
+__device__ __forceinline__ void add_shared(uint32_t addr, float x) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v + x) : "memory");
+}
+__device__ __forceinline__ float ld_shared(uint32_t addr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+    return v;
+}
 // named barrier 1 + wg over the 128 threads of warpgroup wg (barrier 0 is __syncthreads')
 __device__ __forceinline__ void wg_bar_sync(int wg) {
     if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -193,6 +214,21 @@ __device__ __forceinline__ void mma3(float (&d)[NACC], const uint32_t (&a)[4], c
 }
 template <int NACC>
 __device__ __forceinline__ float (&sub64(float (&a)[NACC], int off))[64] { return *reinterpret_cast<float(*)[64]>(a + off); }
+// gW0^T = x^T dh1 (both kernels' weight gradients): one m16n8k8 tf32 term, A[e][s] = x[s][e], B[s][n] = dh1[s][n]
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { hi[i] = tf32_rna(v[i]); lo[i] = tf32_rna(v[i] - __uint_as_float(hi[i])); }
+}
+// tf32_rna for finite x in two integer operations (cvt.rna.tf32.f32 adds an inf / NaN test to the same round-half-away-from-zero)
+__device__ __forceinline__ uint32_t tf32_rna_finite(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
+__device__ __forceinline__ void split_finite(float v, uint32_t &hi, uint32_t &lo) {
+    hi = tf32_rna_finite(v);
+    lo = tf32_rna_finite(v - __uint_as_float(hi));
+}
 
 // ------------------------------------------------------------------------------------------------
 // Weight panels: the exact shared-memory image (K-major, 128B swizzle, K permuted by kperm, tf32 hi then lo) of every
@@ -244,8 +280,9 @@ struct Params {
     nl_render_stats *stats;
     float truncation;
     const float *dsdf_ext;
-    float *act_dh1, *act_d;            // WGRAD: [cap][256], [cap]
+    float *act_dh1, *act_d;            // WGRAD: [cap][256] (may be null: dh1 is not copied out), [cap]
     uint32_t *act_m2;                  // WGRAD: relu'(h2) rows, [cap][8] (see m2_word)
+    float *gW0, *gb0;                  // WGRAD: [256][16], [256], accumulated
     int seg_rays;                      // SEG: rays per problem; stats = the problems' statistics, problem = s_ray / seg_rays
 };
 
@@ -299,6 +336,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
     const uint32_t total = (uint32_t)(my_tiles * IPT);
 
     for (int i = tid; i < WN; i += NTHREADS) { b0s[i] = p.b0[i]; b1s[i] = p.b1[i]; w2s[i] = p.w2[i]; }
+    if constexpr (WGRAD) {
+        float *acc = reinterpret_cast<float *>(sm + SM_GW0);   // WGRAD: gW0 copy w: [w][n][e]; gb0 copy c: [c][n]
+        for (int i = tid; i < 2 * WN * 16 + 2 * WN; i += NTHREADS) acc[i] = 0.f;
+    }
     if (tid == 0) {
         for (int s = 0; s < NSLOT; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -481,10 +522,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 for (int r = 0; r < 2; ++r) nl_seg_loss_add(p.stats, t == 0 ? seg_k[r] : -1, seg_fs[r], seg_sdf[r]);
             }
             if constexpr (!TRAIN) continue;          // scoring: the tile ends with its loss
-            // WGRAD: the activation buffer rows of this warpgroup leave through bulk copies from its staging area (dh1 half | relu'(h2)
-            // words | dsdf).  The first warp's lanes issue them (two dh1 rows each); a staged half is overwritten only after those lanes
-            // saw their copies finish reading it and the warpgroup passed a barrier behind them.  Everything here is derived from tid
-            // and tile where it is used.
+            // WGRAD: the activation buffer rows of this warpgroup leave through bulk copies from its staging area (dh1 quarter |
+            // relu'(h2) words | dsdf).  The first warp's lanes issue them (two dh1 rows each, when dh1 is copied out at all); a staged
+            // quarter is overwritten only after those lanes saw their copies finish reading it and the warpgroup passed a barrier
+            // behind them, which also orders it after the gW0 / gb0 reads of the previous quarter.  Everything here is derived from
+            // tid and tile where it is used.
             auto staging = [&]() { return reinterpret_cast<float *>(sm + SM_STG + (warp >> 2) * STG_WG); };
             if (WGRAD) {
                 const int lr = (warp & 3) * 16 + g;   // this thread's rows inside the warpgroup's 64: lr, lr + 8
@@ -506,15 +548,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                     if (live1 && (m1 | 3) >= M) p.act_d[m1] = dsdf[1];
                 }
             }
-            // stage dh1 columns 128 hh .. 128 hh + 127 (and with hh = 0 the relu'(h2) words and dsdf) and start their copies
-            auto stage_half = [&](int hh) {
+            // stage dh1 columns 64 qq .. 64 qq + 63 (and with qq = 0 the relu'(h2) words, dsdf and the x tile) and start their copies
+            auto stage_quarter = [&](int qq) {
                 const int wg = warp >> 2, lr = (warp & 3) * 16 + g;
                 float *stg = staging();
                 if ((warp & 3) == 0) bulk_wait_read();
                 wg_bar_sync(wg);
+                if (qq == 0) {   // thread (row r, quarter t): features 4t .. 4t + 3 of rows r and r + 8 of the warpgroup's 64, exactly 0
+                                 // past M, where the feature array may hold anything (indices read afresh, as in gw0_quarter)
+                    uint32_t th;
+                    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(th));
+                    const int r = ((th >> 5) & 3) * 16 + ((th >> 2) & 7), c = 4 * (th & 3);
+                    const long long s = tile * TM + 64 * (th >> 7) + r;
+                    float *xt = reinterpret_cast<float *>(sm + SM_XT) + (th >> 7) * 64 * 16;
+                    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+                    const float4 v0 = s < M ? __ldg(reinterpret_cast<const float4 *>(p.feats + (size_t)s * 16 + c)) : z;
+                    const float4 v1 = s + 8 < M ? __ldg(reinterpret_cast<const float4 *>(p.feats + (size_t)(s + 8) * 16 + c)) : z;
+                    *reinterpret_cast<float4 *>(xt + r * 16 + (c ^ xt_swz(r))) = v0;
+                    *reinterpret_cast<float4 *>(xt + (r + 8) * 16 + (c ^ xt_swz(r + 8))) = v1;
+                }
 #pragma unroll
-                for (int jj = 0; jj < 16; ++jj) {
-                    const int j = 16 * hh + jj;
+                for (int jj = 0; jj < 8; ++jj) {
+                    const int j = 8 * qq + jj;
                     *reinterpret_cast<float2 *>(stg + lr * STG_LD + 8 * jj + 2 * t) = make_float2(h[4 * j], h[4 * j + 1]);
                     *reinterpret_cast<float2 *>(stg + (lr + 8) * STG_LD + 8 * jj + 2 * t) = make_float2(h[4 * j + 2], h[4 * j + 3]);
                 }
@@ -523,13 +578,72 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 if ((warp & 3) == 0) {
                     const long long r0 = tile * TM + 64 * wg;               // rows r0 .. r0 + nrows - 1
                     const int nrows = (int)min(max(M - r0, 0LL), 64LL);
-                    for (int r = lane; r < nrows; r += 32)
-                        bulk_s2g(p.act_dh1 + (size_t)(r0 + r) * WN + 128 * hh, smem_u32(stg + r * STG_LD), 128 * 4);
-                    if (hh == 0 && lane == 0 && nrows > 0) {
+                    if (p.act_dh1)
+                        for (int r = lane; r < nrows; r += 32)
+                            bulk_s2g(p.act_dh1 + (size_t)(r0 + r) * WN + 64 * qq, smem_u32(stg + r * STG_LD), 64 * 4);
+                    if (qq == 0 && lane == 0 && nrows > 0) {
                         bulk_s2g(p.act_m2 + (size_t)r0 * 8, smem_u32(stg + STG_M2 / 4), nrows * 8 * 4);
                         if (nrows >= 4) bulk_s2g(p.act_d + r0, smem_u32(stg + STG_D / 4), (nrows & ~3) * 4);
                     }
                     bulk_commit();
+                }
+            };
+            // gW0^T += x^T dh1 and gb0 += sum dh1 over the warpgroup's 64 rows, for the staged quarter qq.  Warp w of the warpgroup owns
+            // columns 64 qq + 16 w .. + 15 (two n8 tiles) and uses k_wgrad_tc's former 3xTF32 terms, each accumulator restarted every 32
+            // samples (see the truncation note at k_wgrad_tc).  x comes from the warpgroup's x tile, exactly 0 on rows at or past M; dh1 is
+            // 0 there already.  Both are finite, so they are split with tf32_rna_finite.  The B fragments a warp loads cover all 64
+            // rows of its 16 columns (lanes t = 0..3 of a column together), so gb0 is their sum over the k-steps and the 4 lanes.
+            auto gw0_quarter = [&](int qq) {
+                uint32_t th;   // read afresh: nothing here is computed early and held through the forward layers
+                asm volatile("mov.u32 %0, %%tid.x;" : "=r"(th));
+                const int wg = th >> 7, wq = (th >> 5) & 3, g = (th >> 2) & 7, t = th & 3, sw = xt_swz(t);
+                const float *stg = reinterpret_cast<const float *>(sm + SM_STG + wg * STG_WG);
+                const float *xt = reinterpret_cast<const float *>(sm + SM_XT) + wg * 64 * 16;
+                float cs[2] = {0.f, 0.f};   // gb0 partial of column 16 wq + 8 nt + g
+#pragma unroll 1
+                for (int hk = 0; hk < 2; ++hk) {
+                    float pw[2][3][4];
+#pragma unroll
+                    for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+                        for (int m = 0; m < 3; ++m)
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) pw[nt][m][i] = 0.f;
+#pragma unroll
+                    for (int k4 = 0; k4 < 4; ++k4) {
+                        const int ks = 4 * hk + k4;
+                        const float *xa = xt + (8 * ks + t) * 16, *xb = xa + 4 * 16;   // rows 8 ks + t and + 4: same swizzle
+                        const float av[4] = {xa[g ^ sw], xa[(g + 8) ^ sw], xb[g ^ sw], xb[(g + 8) ^ sw]};
+                        uint32_t xh[4], xl[4];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) split_finite(av[i], xh[i], xl[i]);
+#pragma unroll
+                        for (int nt = 0; nt < 2; ++nt) {
+                            const float *qr = stg + (8 * ks + t) * STG_LD + 16 * wq + 8 * nt + g;
+                            const float bv[2] = {qr[0], qr[4 * STG_LD]};
+                            uint32_t bh[2], bl[2];
+#pragma unroll
+                            for (int i = 0; i < 2; ++i) split_finite(bv[i], bh[i], bl[i]);
+                            cs[nt] += bv[0] + bv[1];
+                            mma_tf32(pw[nt][0], xh, bh[0], bh[1]);
+                            mma_tf32(pw[nt][1], xh, bl[0], bl[1]);
+                            mma_tf32(pw[nt][2], xl, bh[0], bh[1]);
+                        }
+                    }
+                    // fragment entry i: row (e) g + 8 (i >> 1), column (n) 2t + (i & 1) of n8 tile nt
+#pragma unroll
+                    for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+                            add_shared(base + SM_GW0 + 4 * ((wg * WN + 64 * qq + 16 * wq + 8 * nt + 2 * t + (i & 1)) * 16 + g + 8 * (i >> 1)),
+                                       pw[nt][0][i] + pw[nt][1][i] + pw[nt][2][i]);
+                }
+#pragma unroll
+                for (int nt = 0; nt < 2; ++nt) {
+                    float c = cs[nt];
+                    c += __shfl_xor_sync(0xffffffffu, c, 1);
+                    c += __shfl_xor_sync(0xffffffffu, c, 2);
+                    if (t == 0) add_shared(base + SM_GB0 + 4 * (wg * WN + 64 * qq + 16 * wq + 8 * nt + g), c);
                 }
             };
             // ---- backward layer 2: D3 = relu'(h2) . (diag(w2) W1).  The A operand is the 0/1 mask (exact in tf32: 2 terms) ----
@@ -569,13 +683,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                     for (int x = 0; x < 4; ++x)
                         h[4 * j + x] = ((m1w >> ((j & 7) * 4 + x)) & 1u) ? dsdf[x >> 1] * h[4 * j + x] : 0.f;
             }
-            // ---- backward layer 1: d x = dh1 . W0 (N = 16); each dh1 half is staged and copied out before its K-blocks ----
+            // ---- backward layer 1: d x = dh1 . W0 (N = 16); each dh1 quarter is staged (and copied out) before its two K-blocks,
+            // and its gW0 / gb0 terms run while the wgmmas of the first of them are in flight ----
             float dx[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) dx[i] = 0.f;
 #pragma unroll
             for (int kb = 0; kb < 8; ++kb) {
-                if (WGRAD && kb % 4 == 0) stage_half(kb / 4);
+                if (WGRAD && kb % 2 == 0) stage_quarter(kb / 2);
                 uint32_t ah[4][4], al[4][4];
 #pragma unroll
                 for (int ks = 0; ks < 4; ++ks) frag3(h, 4 * kb + ks, ah[ks], al[ks]);
@@ -584,6 +699,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < 4; ++ks) mma3<8>(dx, ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
+                if (WGRAD && kb % 2 == 0) gw0_quarter(kb / 2);
                 release();
             }
 #pragma unroll
@@ -594,6 +710,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
         }
     }
     if (WGRAD && (warp & 3) == 0) bulk_wait();   // the staging areas stay valid until the copies out of them have completed
+    if constexpr (WGRAD) {                        // the CTA's gW0 / gb0 (if it had a tile): one fp32 atomic per entry
+        __syncthreads();
+        if (n > 0) {
+            uint32_t th;
+            asm volatile("mov.u32 %0, %%tid.x;" : "=r"(th));
+            const uint32_t acc = (smem_u32(smem_raw) + 1023u & ~1023u) + SM_GW0, acb = acc + (SM_GB0 - SM_GW0);
+            for (uint32_t i = th; i < WN * 16; i += NTHREADS) atomicAdd(p.gW0 + i, ld_shared(acc + 4 * i) + ld_shared(acc + 4 * (WN * 16 + i)));
+            atomicAdd(p.gb0 + th, ld_shared(acb + 4 * th) + ld_shared(acb + 4 * (WN + th)));
+        }
+    }
     if (TRAIN && !SEG && !p.dsdf_ext) {
         // every thread's sums in the order it added them, then over the warp: the same fp64 partials as register accumulators
         double loss_fs = lsum[tid], loss_sdf = lsum[NTHREADS + tid];
@@ -608,12 +734,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
     }
 }
 
-// Every decoder weight gradient from dh1, x = feats, the relu'(h2) bits and dsdf; h1 is recomputed from x instead of stored.
+// The decoder weight gradients past layer 1 from x = feats, the relu'(h2) bits and dsdf; h1 is recomputed from x instead of stored.
 // With G = m2^T (dsdf * h1) and c = m2^T dsdf (section at the top of the file):
 //   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c   gb2 = sum_s dsdf
-//   gW0 = dh1^T x      gb0 = sum_s dh1
-// Grid = 4 tiles x nsplit (one CTA per SM), split-K over samples.  CTA (tile, split) owns the 128 x 128 tile (k0, j0) of G^T and the
-// 64-column quarter 64 * tile of dh1, so dh1 is read exactly once.  The reduction index is the sample, and wgmma's tf32 forms take
+// (gW0 = dh1^T x and gb0 = sum_s dh1 are formed by the training kernel, where dh1 is.)
+// Grid = 4 tiles x nsplit (one CTA per SM), split-K over samples.  CTA (tile, split) owns the 128 x 128 tile (k0, j0) of G^T.
+// The reduction index is the sample, and wgmma's tf32 forms take
 // B only as K-major shared memory and A from registers or K-major shared memory, so G is formed transposed with K = samples,
 // G^T[k, j] = sum_s (dsdf * h1)^T[k, s] m2[s, j]: A comes from registers and B, the mask, is rebuilt per chunk as a K-major tile.
 // Warpgroup w owns rows k0 + 64 w .. +63 (wgmma M = 64) and all 128 columns j.  Per chunk of WG_KC = 64 samples it
@@ -625,41 +751,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
 //      tile stores its samples in kperm order;
 //   3. accumulates G^T with 2 terms (the mask is exact in tf32): A from the registers of step 2, B = the mask expanded from its bits
 //      into a [128 j][64 s] tile of 0 / 1.0f (K-major, 128-byte swizzle, two K-blocks of 32 samples), shared by both warpgroups.
-// While the G wgmmas run, every warp forms its part of gW0^T (16 x 64) = x^T dh1 with 3xTF32 mma.sync m16n8k8 (warp w owns dh1
-// columns 8w .. 8w + 7 of the quarter), the column sums gb0, c (the k0 = 0 tiles) and gb2 (tile 0), and builds the next chunk's x
-// and mask tiles into the other of two tile buffers.  x, the mask rows, dsdf and the dh1 quarter stream through a WG_NS-slot
-// shared-memory ring filled by cp.async WG_NS - 1 chunks ahead; one __syncthreads per chunk publishes the next chunk's data and
-// tiles.
+// While the G wgmmas run, the warps form the column sums c (the k0 = 0 tiles) and gb2 (tile 0), and build the next chunk's x and
+// mask tiles into the other of two tile buffers.  x, the mask rows and dsdf stream through a WG_NS-slot shared-memory ring filled
+// by cp.async WG_NS - 1 chunks ahead; one __syncthreads per chunk publishes the next chunk's data and tiles.
 // The tensor core truncates the sums it accumulates, a bias that grows with the number of MMAs into one accumulator; so every
 // chunk's first wgmma starts from zero (scale-d = 0) and the chunk sums are added up in fp32 (G) or fp64 (the rest) over the ~2e4
 // samples of a split.
 // Samples at or past the device-side count are zero-filled in every streamed array (the feature array behind them holds stale
-// values, possibly non-finite): x = dh1 = dsdf = 0 and an empty mask, so they add exact zeros everywhere.
+// values, possibly non-finite): x = dsdf = 0 and an empty mask, so they add exact zeros everywhere.
 // The partial G is folded into the gradients it determines before the atomics:
 //   gW1[j][k] += w2[j] G[j][k]      gW2[j] += sum_k W1[j][k] G[j][k] (+ b1[j] c[j] from the k0 = 0 tiles)
 constexpr int WG_KC = 64, WG_NS = 4;
 constexpr int WG_LDX = 20;     // x rows in the ring: fragment loads (row g, column t) hit 32 distinct banks
-constexpr int WG_LDQ = 72;     // dh1 quarter rows: fragment loads (sample t / t+4, column g) hit 32 distinct banks
-constexpr int WG_OM = WG_KC * WG_LDX, WG_OD = WG_OM + WG_KC * 8, WG_OQ = WG_OD + WG_KC;   // slot: x | mask rows | dsdf | dh1 quarter
-constexpr int WG_SLOT = WG_OQ + WG_KC * WG_LDQ;                                            // floats
+constexpr int WG_OM = WG_KC * WG_LDX, WG_OD = WG_OM + WG_KC * 8;   // slot: x | mask rows | dsdf
+constexpr int WG_SLOT = WG_OD + WG_KC;                             // floats
 constexpr int WG_MT = (WG_KC / 32) * HALF;   // mask tile: K-blocks of 32 samples, 128 rows (j) x 128 B each
 constexpr int WG_XT = WG_KC * 128;           // x tile (hi or lo): a 128-byte row per sample, the 16 features in its first 64 B
-constexpr int WG_SMEM = 2 * (WG_MT + 2 * WG_XT) + WG_NS * WG_SLOT * 4 + 1024;   // 198 KB: 2 tile buffers, ring, alignment slack
-static_assert(WG_OM % 4 == 0 && WG_OD % 4 == 0 && WG_OQ % 4 == 0 && WG_SLOT % 4 == 0, "cp.async 16-byte destinations");
+constexpr int WG_SMEM = 2 * (WG_MT + 2 * WG_XT) + WG_NS * WG_SLOT * 4 + 1024;   // 126 KB: 2 tile buffers, ring, alignment slack
+static_assert(WG_OM % 4 == 0 && WG_OD % 4 == 0 && WG_SLOT % 4 == 0, "cp.async 16-byte destinations");
 static_assert(WG_KC == 64, "the loaders and the x-tile build assign one 16-byte piece of x per thread");
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
 __device__ __forceinline__ void cp_async4(uint32_t dst, const void *src, bool valid) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(valid ? 4 : 0) : "memory");
-}
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { hi[i] = tf32_rna(v[i]); lo[i] = tf32_rna(v[i] - __uint_as_float(hi[i])); }
 }
 // keeps the compiler from moving reads of wgmma accumulators above the wgmma.wait_group that completes them
 template <int N>
@@ -668,7 +783,7 @@ __device__ __forceinline__ void wg_fence_acc(float (&d)[N]) {
     for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int32_t *__restrict__ M_dev, const float *__restrict__ x,
-                                                     const float *__restrict__ dh1, const uint32_t *__restrict__ m2, const float *__restrict__ dsdf,
+                                                     const uint32_t *__restrict__ m2, const float *__restrict__ dsdf,
                                                      const uint8_t *__restrict__ panels, const float *__restrict__ b0, const float *__restrict__ W1,
                                                      const float *__restrict__ b1, const float *__restrict__ w2, nl_mlp_grads grads, int nsplit) {
     extern __shared__ uint8_t wg_smem[];
@@ -681,7 +796,7 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
     __shared__ double cred[2][128];   // c partials of the two sample halves
     const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
     const int tile = blockIdx.x & 3, split = blockIdx.x >> 2;
-    const int j0 = (tile >> 1) * 128, k0 = (tile & 1) * 128, q0 = tile * 64;
+    const int j0 = (tile >> 1) * 128, k0 = (tile & 1) * 128;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int kr = k0 + 64 * (warp >> 2) + 16 * (warp & 3) + g;   // this thread's rows of h1^T and G^T: kr and kr + 8
 
@@ -702,7 +817,7 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
     float tot[64];   // G^T: tot[4 jn + x] is row kr + 8 (x >> 1), column j0 + 8 jn + 2t + (x & 1)
 #pragma unroll
     for (int i = 0; i < 64; ++i) tot[i] = 0.f;
-    double gw0[4] = {0.0, 0.0, 0.0, 0.0}, gb0 = 0.0, c_acc = 0.0, gb2 = 0.0;
+    double c_acc = 0.0, gb2 = 0.0;
     const long long nch = (M + WG_KC - 1) / WG_KC;
     // Every thread commits one cp.async group per chunk, empty past the last chunk, so that wait_group n always means "all but the
     // n chunks issued last have landed".
@@ -710,13 +825,7 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
         if (ch >= nch) { asm volatile("cp.async.commit_group;" ::: "memory"); return; }
         float *sl = ring + buf * WG_SLOT;
         const long long s0 = ch * WG_KC;
-#pragma unroll
-        for (int i = 0; i < WG_KC / 16; ++i) {                           // dh1 quarter: 64 rows x 16 float4
-            const int f = tid + i * 256, r = f >> 4, c4 = (f & 15) * 4;
-            const bool v = s0 + r < M;
-            cp_async16(smem_u32(sl + WG_OQ + r * WG_LDQ + c4), dh1 + (size_t)(v ? s0 + r : 0) * WN + q0 + c4, v);
-        }
-        {                                                                // x: 64 rows x 4 float4
+        {                                                              // x: 64 rows x 4 float4
             const int r = tid >> 2, c4 = (tid & 3) * 4;
             const bool v = s0 + r < M;
             cp_async16(smem_u32(sl + r * WG_LDX + c4), x + (size_t)(v ? s0 + r : 0) * 16 + c4, v);
@@ -782,36 +891,6 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
         const int b = (int)(it & 1);
         const uint64_t xd = make_desc(base + 2 * WG_MT + 2 * b * WG_XT), md = make_desc(base + b * WG_MT);
 
-        // ---- gW0^T = x^T dh1 with mma.sync: A[e][s] = x[s][e], B[s][n] = dh1[s][n].  It runs before the wgmmas, where few registers
-        // are live, with an accumulator per term and per 32 samples, so that the MMAs do not wait on each other ----
-        {
-            float pw[WG_KC / 32][3][4];
-#pragma unroll
-            for (int hk = 0; hk < WG_KC / 32; ++hk)
-#pragma unroll
-                for (int m = 0; m < 3; ++m)
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) pw[hk][m][i] = 0.f;
-#pragma unroll
-            for (int ks = 0; ks < WG_KC / 8; ++ks) {
-                const float *xr = sl + (8 * ks + t) * WG_LDX + g;
-                const float av[4] = {xr[0], xr[8], xr[4 * WG_LDX], xr[4 * WG_LDX + 8]};
-                const float *qr = sl + WG_OQ + (8 * ks + t) * WG_LDQ + 8 * warp + g;
-                uint32_t xh[4], xl[4], bh[2], bl[2];
-                split4(av, xh, xl);
-                const float bv[2] = {qr[0], qr[4 * WG_LDQ]};
-#pragma unroll
-                for (int i = 0; i < 2; ++i) { bh[i] = tf32_rna(bv[i]); bl[i] = tf32_rna(bv[i] - __uint_as_float(bh[i])); }
-                mma_tf32(pw[ks >> 2][0], xh, bh[0], bh[1]);
-                mma_tf32(pw[ks >> 2][1], xh, bl[0], bl[1]);
-                mma_tf32(pw[ks >> 2][2], xl, bh[0], bh[1]);
-            }
-#pragma unroll
-            for (int hk = 0; hk < WG_KC / 32; ++hk)
-#pragma unroll
-                for (int i = 0; i < 4; ++i) gw0[i] += pw[hk][0][i] + pw[hk][1][i] + pw[hk][2][i];
-        }
-
         // ---- 1. h1^T = W0 x^T ----
         float d1[32];
         wg_fence();
@@ -852,16 +931,8 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
         }
         asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 
-        // ---- column sums gb0 (4 threads per column, 16 samples each) and gb2 (tile 0); c is summed in build() ----
-        {
-            const float *Qs = sl + WG_OQ;
-            const int cc = tid & 63, sg = tid >> 6;
-            float sb[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int i = 0; i < WG_KC / 4; ++i) sb[i & 3] += Qs[(WG_KC / 4 * sg + i) * WG_LDQ + cc];
-            gb0 += (sb[0] + sb[1]) + (sb[2] + sb[3]);
-            if (tile == 0 && tid < WG_KC) gb2 += sl[WG_OD + tid];
-        }
+        // ---- column sum gb2 (tile 0); c is summed in build() ----
+        if (tile == 0 && tid < WG_KC) gb2 += sl[WG_OD + tid];
 
         // ---- the next chunk's tiles, into the buffer that the previous chunk's wgmmas read ----
         if (ch + nsplit < nch) build(ring + ((it + 1) % WG_NS) * WG_SLOT, b ^ 1);
@@ -887,10 +958,6 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
             if (g == 0) red[warp][8 * jn + 2 * t + e] = r;
         }
     if (k0 == 0) cred[tid >> 7][tid & 127] = c_acc;
-    // gW0^T fragment: rows (e) g and g + 8, columns (k) 2t and 2t + 1 of the warp's 8
-#pragma unroll
-    for (int i = 0; i < 4; ++i) atomicAdd(grads.gW0 + (size_t)(q0 + 8 * warp + 2 * t + (i & 1)) * 16 + g + 8 * (i >> 1), (float)gw0[i]);
-    atomicAdd(grads.gb0 + q0 + (tid & 63), (float)gb0);
     if (tile == 0 && warp < WG_KC / 32) {
         for (int off = 16; off > 0; off >>= 1) gb2 += __shfl_xor_sync(0xffffffffu, gb2, off);
         if (lane == 0) atomicAdd(grads.gb2, (float)gb2);
@@ -947,13 +1014,14 @@ extern "C" int nl_mlp_tc_forward(int64_t M, const int32_t *d_M_dev, const float 
     return NL_OK;
 }
 
-// dh1 [cap][256], relu'(h2) bits [cap][8 words] and d loss / d sdf [cap], cap = M rounded up to whole tiles
-extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * (tc::WN + 8 + 1); }
+// relu'(h2) bits [cap][8 words] and d loss / d sdf [cap]; the optional dh1 plane is [cap][256].  cap = M rounded up to whole tiles
+extern "C" int64_t nl_mlp_tc_act_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * (8 + 1); }
+extern "C" int64_t nl_mlp_tc_dh1_floats(int64_t M) { return ((M + tc::TM - 1) / tc::TM) * tc::TM * tc::WN; }
 
 extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *feats, const void *panels, const float *W1, const float *b0,
                                const float *b1, const float *w2, const float *b2, const uint8_t *s_flag, const float *s_depth,
                                const int32_t *s_ray, const float *cosv, const float *gt_depth, nl_render_stats *stats,
-                               float truncation, float *sdf, float *dfeats, const nl_mlp_grads *grads, float *act,
+                               float truncation, float *sdf, float *dfeats, const nl_mlp_grads *grads, float *act, float *act_dh1,
                                const float *dsdf_ext, void *wgrad_stream_, void *stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (M < 0) return nl_set_error("nl_mlp_tc_train: negative M");
@@ -973,8 +1041,9 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
         NL_CHECK_LAUNCH("nl_mlp_tc_train");
         return NL_OK;
     }
-    const size_t cap = (size_t)((M + tc::TM - 1) / tc::TM) * tc::TM, plane = cap * tc::WN;
-    p.act_dh1 = act; p.act_m2 = reinterpret_cast<uint32_t *>(act + plane); p.act_d = act + plane + cap * 8;
+    const size_t cap = (size_t)((M + tc::TM - 1) / tc::TM) * tc::TM;
+    p.act_dh1 = act_dh1; p.act_m2 = reinterpret_cast<uint32_t *>(act); p.act_d = act + cap * 8;
+    p.gW0 = grads->gW0; p.gb0 = grads->gb0;
     if (int rc = tc::launch<true, true>(p, stream)) return rc;
     static NlPerDevice configured;
     const cudaError_t e = configured.once([] { return cudaFuncSetAttribute(tc::k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::WG_SMEM); });
@@ -995,8 +1064,7 @@ extern "C" int nl_mlp_tc_train(int64_t M, const int32_t *d_M_dev, const float *f
             return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_train: could not order the weight-gradient stream behind the decoder kernel");
     }
     const int nsplit = nl_num_sms() / 4 > 0 ? nl_num_sms() / 4 : 1;
-    tc::k_wgrad_tc<<<4 * nsplit, 256, tc::WG_SMEM, ws>>>(M, d_M_dev, feats, p.act_dh1, p.act_m2, p.act_d, p.panels, b0, W1, b1, w2, *grads,
-                                                          nsplit);
+    tc::k_wgrad_tc<<<4 * nsplit, 256, tc::WG_SMEM, ws>>>(M, d_M_dev, feats, p.act_m2, p.act_d, p.panels, b0, W1, b1, w2, *grads, nsplit);
     NL_CHECK_LAUNCH("nl_mlp_tc_train");
     return NL_OK;
 }

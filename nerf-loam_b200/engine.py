@@ -39,8 +39,8 @@ def mlp_forward(bufs, M_cap, M_dev, feats, sdf):
 
 def mlp_train(bufs, M_cap, M_dev, feats, sdf, dfeats, want_wgrad, act, s_flag=None, s_depth=None, s_ray=None, cos=None, gt_depth=None,
               stats_ptr=None, truncation=0.0, dsdf_ext=None, wgrad_stream=None):
-    """Forward + (loss | external d sdf) + backward.  act: dict with scratch tensors for the weight gradients
-    ('h1','dh2' [cap,W] for simt; one 'buf' of nl_mlp_tc_act_floats(cap) floats for tc).  Accumulates into bufs.grads when want_wgrad."""
+    """Forward + (loss | external d sdf) + backward.  act: dict with scratch tensors for the weight gradients from alloc_act
+    ('h1','dh2' [cap,W] for simt; 'buf' = ['dh1' plane or nothing | 'act'] for tc).  Accumulates into bufs.grads when want_wgrad."""
     lib, st = _capi.lib(), _capi.stream_ptr()
     gs = bufs.grads_struct() if want_wgrad else None
     gp = C.byref(gs) if want_wgrad else None
@@ -49,7 +49,8 @@ def mlp_train(bufs, M_cap, M_dev, feats, sdf, dfeats, want_wgrad, act, s_flag=No
         _capi.check(lib.nl_mlp_tc_train(M_cap, M_dev, _capi.ptr(feats), _capi.ptr(bufs.tc_panels), _capi.ptr(p[2]), _capi.ptr(p[1]), _capi.ptr(p[3]),
                                         _capi.ptr(p[4]), _capi.ptr(p[5]), _capi.ptr(s_flag), _capi.ptr(s_depth), _capi.ptr(s_ray),
                                         _capi.ptr(cos), _capi.ptr(gt_depth), stats_ptr, float(truncation), _capi.ptr(sdf),
-                                        _capi.ptr(dfeats), gp, _capi.ptr(act["buf"]) if want_wgrad else None, _capi.ptr(dsdf_ext),
+                                        _capi.ptr(dfeats), gp, _capi.ptr(act["act"]) if want_wgrad else None,
+                                        _capi.ptr(act["dh1"]) if want_wgrad else None, _capi.ptr(dsdf_ext),
                                         C.c_void_p(wgrad_stream.cuda_stream) if (want_wgrad and wgrad_stream is not None) else None, st),
                     "nl_mlp_tc_train")
         _capi.LAUNCHES += 2 if want_wgrad else 1
@@ -62,11 +63,14 @@ def mlp_train(bufs, M_cap, M_dev, feats, sdf, dfeats, want_wgrad, act, s_flag=No
         _capi.LAUNCHES += 2 if want_wgrad else 1
 
 
-def alloc_act(width, M_cap, device):
-    """Scratch for the decoder weight gradients, sized for M_cap samples."""
+def alloc_act(width, M_cap, device, dh1=True):
+    """Scratch for the decoder weight gradients, sized for M_cap samples.  tc: one buffer [dh1 plane | relu'(h2) words | d sdf]
+    (1060 B per sample); with dh1=False the dh1 plane, which no gradient reads, is left out and not written (36 B per sample)."""
     if mlp_impl(width) == "tc":
-        n = int(_capi.lib().nl_mlp_tc_act_floats(int(M_cap)))
-        return {"buf": torch.empty(n, dtype=torch.float32, device=device)}
+        lib = _capi.lib()
+        nd = int(lib.nl_mlp_tc_dh1_floats(int(M_cap))) if dh1 else 0
+        buf = torch.empty(nd + int(lib.nl_mlp_tc_act_floats(int(M_cap))), dtype=torch.float32, device=device)
+        return {"buf": buf, "dh1": buf[:nd] if dh1 else None, "act": buf[nd:]}
     return {k: torch.empty((int(M_cap), width), dtype=torch.float32, device=device) for k in ("h1", "dh2")}
 
 
@@ -374,7 +378,7 @@ class SDFEngine:
     def _ensure_act(self, width):
         key = (width, mlp_impl(width))
         if self.act is None or self._act_key != key:
-            self.act = alloc_act(width, self.max_samples, self.device)
+            self.act = alloc_act(width, self.max_samples, self.device, dh1=False)
             self._act_key = key
 
     # ------------------------------------------------------------------ stages

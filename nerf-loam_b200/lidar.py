@@ -47,7 +47,7 @@ class _DecoderFn(torch.autograd.Function):
         sdf = torch.empty(M, dtype=torch.float32, device=x.device)
         dx = torch.empty((M, 16), dtype=torch.float32, device=x.device)
         need_w = any(ctx.needs_input_grad[2:])
-        act = alloc_act(W, M, x.device) if need_w else None
+        act = alloc_act(W, M, x.device, dh1=False) if need_w else None
         g = gout.reshape(-1).contiguous().float()
         bufs.gradflat.zero_()                       # the buffers are cached per decoder (DecoderBuffers.of): start from zero ...
         mlp_train(bufs, M, None, x, sdf, dx, need_w, act, dsdf_ext=g)

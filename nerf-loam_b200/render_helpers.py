@@ -108,7 +108,7 @@ class _RenderSDF(torch.autograd.Function):
         W = bufs.width
         sdf = torch.empty(M, dtype=torch.float32, device=dev)
         dfeats = torch.empty((M, 16), dtype=torch.float32, device=dev)
-        act = alloc_act(W, M, dev) if need_dec else None
+        act = alloc_act(W, M, dev, dh1=False) if need_dec else None
         g = gsdf.contiguous().float()
         lib, st = _capi.lib(), _capi.stream_ptr()
         mlp_train(bufs, M, None, s["feats"], sdf, dfeats, need_dec, act, dsdf_ext=g)
