@@ -563,6 +563,52 @@ NL_API int nl_mc_emit(int32_t n_vox, int32_t res, float voxel_size, const float 
  * SDF at corner i is negative.  The table is derived (face tracing), not hand-made; see csrc/mc.cu. */
 NL_API int nl_mc_case_table(uint8_t *h_tri, uint8_t *h_ntri, uint8_t *h_edge_corner);
 
+/* ============================================================================================
+ * 11. Reconstruction evaluation: a mesh against a reference point cloud -- replaces the evaluation protocol of Readme.md
+ *     ("Evaluation": the external SHINE-Mapping script, an Open3D mesh sampled on the host and a CPU KD-tree in both directions).
+ *     csrc/eval.cu; nerf-loam_b200/evaluate.py composes the calls.  Every sum is fp64 in a fixed order (tiles of
+ *     NL_EVAL_TILE elements, then the tiles in order), so two calls give the same bits on any device and launch shape.
+ * ============================================================================================ */
+#define NL_EVAL_KEY_BITS 21    /* per axis: voxel and cell keys are 3 x 21 bits; coordinates floor((p - o) / h) in [0, 2^21) */
+#define NL_EVAL_TILE 2048      /* elements per fixed-order partial sum */
+/* NL_EVAL_KEY_BITS, NL_EVAL_TILE: lets a binding check the constants it relies on */
+NL_API void nl_abi_sizes_eval(int32_t out[2]);
+/* d_bounds f32[6] = (min x, y, z, max x, y, z) over the finite rows of d_pts f32[n,3] (+inf / -inf when there is none),
+ * d_nonfinite i64[1] = number of rows with a NaN or inf coordinate.  n may be 0. */
+NL_API int nl_eval_bounds(int64_t n, const float *d_pts, float *d_bounds, int64_t *d_nonfinite, void *stream);
+/* Surface sampling, uniform by area.  nl_eval_surface_prepare: fp64 area of every triangle of d_faces i32[n_faces,3] over
+ * d_verts f32[n_verts,3] and their fp64 inclusive prefix sum, kept in the workspace; d_info f64[2] = (total area, > 0 when a face
+ * index is outside [0, n_verts)).  nl_eval_sample_surface then draws sample i from Philox4x32-10 keyed on `seed` with counter i:
+ * the triangle by inverse CDF over the prefix sum (zero-area triangles are never chosen), the point by the square-root barycentric
+ * formula, computed in fp64 and rounded to d_out f32[n_samples,3]; d_face i32[n_samples] (may be NULL) gets the triangle. */
+NL_API int64_t nl_eval_surface_workspace_bytes(int64_t n_faces);
+NL_API int nl_eval_surface_prepare(int64_t n_verts, const float *d_verts, int64_t n_faces, const int32_t *d_faces, void *d_ws, int64_t ws_bytes,
+                                   double *d_info, void *stream);
+NL_API int nl_eval_sample_surface(int64_t n_verts, const float *d_verts, int64_t n_faces, const int32_t *d_faces, int64_t n_samples, uint64_t seed,
+                                  const void *d_ws, int64_t ws_bytes, float *d_out, int32_t *d_face, void *stream);
+/* Voxel down-sampling on the grid with origin (ox, oy, oz) and side res: key = floor((p - o) / res) per axis in fp64.  Rows
+ * outside the box d_crop f32[6] (min, max as nl_eval_bounds writes it) padded by res are dropped (d_crop may be NULL); rows whose
+ * key does not fit NL_EVAL_KEY_BITS are dropped too and counted apart.  Each occupied voxel becomes the centroid of its rows: a
+ * stable radix sort by key, then one fp64 sum per voxel in that order.  d_out f32[n,3] (capacity n) gets the centroids in key
+ * order, d_keys u64[n] (may be NULL) their keys (x << 42 | y << 21 | z), d_counts i64[3] = (cropped rows, rows outside the key
+ * range, voxels). */
+NL_API int64_t nl_eval_voxel_workspace_bytes(int64_t n_points);
+NL_API int nl_eval_voxel_down_sample(int64_t n, const float *d_pts, double ox, double oy, double oz, double res, const float *d_crop, void *d_ws,
+                                     int64_t ws_bytes, float *d_out, uint64_t *d_keys, int64_t *d_counts, void *stream);
+/* Truncated nearest distance: d_dist[i] = min(truncation, min_j |q_i - t_j|) in fp32, exact below the truncation.  The target
+ * is sorted into cells of side `cell` from origin o (keys as above; d_bad i64[1] counts target rows outside the key range, which
+ * are never searched) and every occupied cell's run goes into a hash table.  A query walks Chebyshev rings of cells around its
+ * own cell; after ring k every unvisited target is at least k * cell away, so it stops when its best distance is <= k * cell or
+ * k * cell >= truncation (max_ring * cell >= truncation is required; max_ring <= 64).  Workspace for n_target rows, about 100
+ * bytes per row. */
+NL_API int64_t nl_eval_nn_workspace_bytes(int64_t n_target);
+NL_API int nl_eval_nearest(int64_t n_query, const float *d_query, int64_t n_target, const float *d_target, double ox, double oy, double oz,
+                           double cell, int32_t max_ring, float truncation, void *d_ws, int64_t ws_bytes, float *d_dist, int64_t *d_bad,
+                           void *stream);
+/* d_out f64[3] = (sum d, sum d^2, number of d < threshold) over d_dist f32[n] */
+NL_API int64_t nl_eval_sums_workspace_bytes(int64_t n);
+NL_API int nl_eval_distance_sums(int64_t n, const float *d_dist, float threshold, void *d_ws, int64_t ws_bytes, double *d_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

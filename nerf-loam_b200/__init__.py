@@ -15,13 +15,15 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     score_poses / relocalise (= render_helpers.*, score)  the loss of up to 65 535 pose hypotheses of one scan; recovering a lost scan
     mapping.MapUpdater              <- Mapping.create_voxels / update_grid_features / get_embeddings (src/mapping.py)
     mesh.extract_mesh / marching_cubes  <- MeshExtractor.create_mesh / marching_cubes (src/utils/mesh_util.py)
+    evaluate.eval_mesh / sample_surface / voxel_down_sample / nearest_distances  <- the map evaluation of Readme.md ("Evaluation"):
+                                    accuracy, completeness, Chamfer distance and F-score of a mesh against a reference cloud, on the GPU
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
 no CPU or eager-PyTorch fallback for the kernels.
 """
 from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
-           "track_batch", "track_frames", "score", "score_poses", "relocalise"]
+           "evaluate", "track_batch", "track_frames", "score", "score_poses", "relocalise"]
 
 
 def __getattr__(name):

@@ -149,6 +149,19 @@ _SIGNATURES = {
     "nl_abi_sizes_score": (None, [C.POINTER(C.c_int32 * 1)]),
     "nl_mlp_tc_score_batch": (C.c_int, [C.c_int64] + [vp] * 13 + [C.c_int32, C.c_float, vp, vp]),
     "nl_loss_finalize_batch": (C.c_int, [C.c_int, vp, C.c_float, C.c_float, vp, vp]),
+    # reconstruction evaluation (include/nerfloam_b200.h section 11)
+    "nl_abi_sizes_eval": (None, [C.POINTER(C.c_int32 * 2)]),
+    "nl_eval_bounds": (C.c_int, [C.c_int64, vp, vp, vp, vp]),
+    "nl_eval_surface_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "nl_eval_surface_prepare": (C.c_int, [C.c_int64, vp, C.c_int64, vp, vp, C.c_int64, vp, vp]),
+    "nl_eval_sample_surface": (C.c_int, [C.c_int64, vp, C.c_int64, vp, C.c_int64, C.c_uint64, vp, C.c_int64, vp, vp, vp]),
+    "nl_eval_voxel_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "nl_eval_voxel_down_sample": (C.c_int, [C.c_int64, vp, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp, C.c_int64, vp, vp, vp, vp]),
+    "nl_eval_nn_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "nl_eval_nearest": (C.c_int, [C.c_int64, vp, C.c_int64, vp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int32, C.c_float, vp,
+                                  C.c_int64, vp, vp, vp]),
+    "nl_eval_sums_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "nl_eval_distance_sums": (C.c_int, [C.c_int64, vp, C.c_float, vp, C.c_int64, vp, vp]),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)
@@ -156,6 +169,8 @@ CTL_ERROR, CTL_SKIPPED, CTL_SKIP_NOW, CTL_ADAM_STEP, CTL_MIN_HIT, CTL_ITERS, CTL
 CTL_STOPPED = 7              # batched control blocks only (nl_iter_status_batch)
 BATCH_MAX_PROBLEMS = 31      # NL_BATCH_MAX_PROBLEMS
 SCORE_MAX_PROBLEMS = 65535   # NL_SCORE_MAX_PROBLEMS
+EVAL_KEY_BITS = 21           # NL_EVAL_KEY_BITS
+EVAL_TILE = 2048             # NL_EVAL_TILE
 STATS_PACK_FIXED = 10
 # node-array checks, bit i = 1 << i (NL_TREE_* in include/nerfloam_b200.h section 1)
 TREE_CHECKS = ("ROOT", "RANGE", "LINK", "PARENTS", "SHAPE", "ROWS", "VERTICES")
@@ -201,6 +216,10 @@ def lib():
         L.nl_abi_sizes_score(C.byref(ssizes))
         if list(ssizes) != [SCORE_MAX_PROBLEMS]:
             raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (score): {list(ssizes)} vs {[SCORE_MAX_PROBLEMS]}")
+        esizes = (C.c_int32 * 2)()
+        L.nl_abi_sizes_eval(C.byref(esizes))
+        if list(esizes) != [EVAL_KEY_BITS, EVAL_TILE]:
+            raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (eval): {list(esizes)} vs {[EVAL_KEY_BITS, EVAL_TILE]}")
         _lib = L
     return _lib
 

@@ -2,7 +2,8 @@
 drop-in API: per scan  track_frame (captured graph) -> bundle_adjust_frames over the keyframe window (captured graph) -> incremental
 map update (MapUpdater) -> publication to the tracker (share.SharedMap); at the end GPU marching cubes.
 BASELINE.json config 2 ("KITTI seq 00 tracking+mapping incremental loop") / config 3 ("... + marching cubes") in spirit; prints a
-JSON summary (per-stage ms per scan, trajectory error against the synthetic ground truth).
+JSON summary (per-stage ms per scan, trajectory error against the synthetic ground truth, and under `reconstruction` the final mesh
+scored by evaluate.eval_mesh against the scans' noise-free returns at the true poses).
 
     python scripts/demo_slam.py [--scans 12] [--spacing 0.5] [--octree host|device] [--json out.json]
 """
@@ -84,13 +85,23 @@ def main():
     t0 = tick()
     verts, faces = nl.mesh.extract_mesh(dec, ms, vs, res=8)
     t_mesh = (tick() - t0) * 1e3
-    err = [float((e[:3, 3] - g[:3, 3]).norm()) for e, g in zip(est, gt)]
+    # the map against the scans' noise-free returns at the true poses, in world coordinates (with the 2000 m offset, like the mesh)
+    clean = []
+    for i in range(a.scans):
+        p, _, pose = syn.make_scan(seed=1000 + i, sensor_xyz=(a.spacing * i, 0.05 * np.sin(0.7 * i), 0.0), yaw=0.01 * np.sin(0.5 * i), noise_std=0.0)
+        clean.append(p.astype(np.float64) @ pose[:3, :3].T.astype(np.float64) + pose[:3, 3])
+    t0 = tick()
+    recon = nl.evaluate.eval_mesh(verts, faces, np.concatenate(clean).astype(np.float32), n_samples=1_000_000, res=0.05, threshold=0.1,
+                                  truncation=0.5, seed=0)
+    recon["ms"] = (tick() - t0) * 1e3
+    err =[float((e[:3, 3] - g[:3, 3]).norm()) for e, g in zip(est, gt)]
     rot = [float(torch.linalg.matrix_norm(e[:3, :3] - g[:3, :3])) for e, g in zip(est, gt)]
     out = {"scans": a.scans, "spacing_m": a.spacing, "octree": a.octree, "translation_error_m": {"mean": float(np.mean(err[1:])), "max": float(np.max(err[1:])), "last": err[-1]},
            "rotation_error_fro": {"mean": float(np.mean(rot[1:])), "max": float(np.max(rot[1:]))},
            "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0, "init_mapping_ms": t_init,
            "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
            "map": {"nodes": ms.n_nodes, "embedding_rows": int(mu.n_rows), "last_update": mu.last_update},
+           "reconstruction": recon,
            "per_scan_translation_error_m": [round(e, 4) for e in err]}
     print(json.dumps(out))
     if a.json:
