@@ -609,6 +609,28 @@ NL_API int nl_eval_nearest(int64_t n_query, const float *d_query, int64_t n_targ
 NL_API int64_t nl_eval_sums_workspace_bytes(int64_t n);
 NL_API int nl_eval_distance_sums(int64_t n, const float *d_dist, float threshold, void *d_ws, int64_t ws_bytes, double *d_out, void *stream);
 
+/* ============================================================================================
+ * 12. Keyframe overlap: the voxels one scan shares with each of K keyframes -- the counts behind the mapper's 'overlap' window
+ *     (Mapping.select_optimize_targets, src/mapping.py:205-225, which declares that method and raises NotImplementedError).
+ *     csrc/overlap.cu; nerf-loam_b200/keyframes.py composes the calls.
+ * ============================================================================================ */
+#define NL_OVERLAP_MAX_CHUNK 1023                   /* keyframes per pass over the table (chunk-local index in the key's top 10 bits) */
+#define NL_OVERLAP_MAX_SLOTS ((int64_t)1 << 32)   /* largest table_slots */
+/* Voxel of a point p (sensor frame) under the pose row Rt f32[12] (as nl_pose_matrices writes it: R row-major, then t): per axis
+ * w_i = ((R_i0 p_x + R_i1 p_y) + R_i2 p_z) + t_i in fp64, v_i = floor(w_i / voxel_size) in fp64.  A point with a v_i outside
+ * [0, grid_dim) (grid_dim a power of two <= 2^18), or not finite, is counted as outside and nowhere else.
+ * Inputs: the scan d_frame_pts f32[n_frame,3] under row 0 of d_Rt12 f32[n_kf+1,12]; keyframe k has d_kf_n[k] points at d_kf_pts[k]
+ * (device arrays of n_kf pointers and counts) under row k + 1, and h_kf_n[k] is the same count on the host: it plans the passes.
+ * Output d_out i64[3 n_kf + 1] = (shared[n_kf] = |V_k n V_c|, kf_voxels[n_kf] = |V_k|, outside[n_kf], frame_voxels = |V_c|), with
+ * V the set of distinct voxels.  Keyframes go through a table of table_slots slots (a power of two >= 2^10) in passes of up to
+ * NL_OVERLAP_MAX_CHUNK keyframes and table_slots / 2 points; a keyframe with more than table_slots / 2 points is an error.  The
+ * workspace (256-byte aligned) holds that table and the scan's set.  No host synchronisation; the counts are exact integers, so two
+ * calls give identical results. */
+NL_API int64_t nl_keyframe_overlap_workspace_bytes(int64_t n_frame, int64_t table_slots);
+NL_API int nl_keyframe_overlap(int64_t n_frame, const float *d_frame_pts, int32_t n_kf, const float *const *d_kf_pts, const int64_t *d_kf_n,
+                               const int64_t *h_kf_n, const float *d_Rt12, double voxel_size, int64_t grid_dim, int64_t table_slots, void *d_ws,
+                               int64_t ws_bytes, int64_t *d_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

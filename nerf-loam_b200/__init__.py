@@ -17,13 +17,15 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     mesh.extract_mesh / marching_cubes  <- MeshExtractor.create_mesh / marching_cubes (src/utils/mesh_util.py)
     evaluate.eval_mesh / sample_surface / voxel_down_sample / nearest_distances  <- the map evaluation of Readme.md ("Evaluation"):
                                     accuracy, completeness, Chamfer distance and F-score of a mesh against a reference cloud, on the GPU
+    keyframes.KeyframeGraph / keyframe_overlap / rank_by_overlap  <- Mapping.insert_keyframe / select_optimize_targets (src/mapping.py),
+                                    with the 'overlap' window the reference leaves unimplemented (voxel IoU with the scan, on the GPU)
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
 no CPU or eager-PyTorch fallback for the kernels.
 """
 from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
-           "evaluate", "track_batch", "track_frames", "score", "score_poses", "relocalise"]
+           "evaluate", "keyframes", "track_batch", "track_frames", "score", "score_poses", "relocalise"]
 
 
 def __getattr__(name):

@@ -162,6 +162,9 @@ _SIGNATURES = {
                                   C.c_int64, vp, vp, vp]),
     "nl_eval_sums_workspace_bytes": (C.c_int64, [C.c_int64]),
     "nl_eval_distance_sums": (C.c_int, [C.c_int64, vp, C.c_float, vp, C.c_int64, vp, vp]),
+    # keyframe overlap (include/nerfloam_b200.h section 12)
+    "nl_keyframe_overlap_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
+    "nl_keyframe_overlap": (C.c_int, [C.c_int64, vp, C.c_int32, vp, vp, vp, vp, C.c_double, C.c_int64, C.c_int64, vp, C.c_int64, vp, vp]),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)

@@ -24,6 +24,7 @@
 #include <cstdio>
 
 #include "../../include/nerfloam_b200.h"
+#include "hash.cuh"
 #include "nl_cuda.cuh"
 
 namespace {
@@ -34,7 +35,6 @@ constexpr int kTile = kThreads * kItems;           // fixed: the fp64 sums' orde
 constexpr int kKeyBits = 21;                       // per axis; NL_EVAL_KEY_BITS
 constexpr int64_t kKeyDim = int64_t(1) << kKeyBits;
 constexpr uint64_t kSentinel = uint64_t(1) << 63;  // cropped point: sorts after every real key (3 x 21 = 63 bits)
-constexpr uint64_t kEmpty = ~uint64_t(0);
 constexpr int64_t kMaxN = INT32_MAX;
 
 size_t take(size_t &at, size_t bytes) {
@@ -78,12 +78,6 @@ __device__ __forceinline__ uint4 philox(uint4 c, uint2 k) {
         k.y += 0xBB67AE85u;
     }
     return c;
-}
-
-__device__ __forceinline__ uint64_t mix64(uint64_t z) {      // splitmix64 finaliser: hash-table slot of a cell key
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
 }
 
 // floor((x - o) / h) in fp64; false when it is outside [0, 2^21)
@@ -378,7 +372,7 @@ __global__ void k_cell_keys(int n, const float *__restrict__ p, double ox, doubl
 }
 
 __global__ void k_hash_clear(int64_t cap, uint64_t *hkey) {
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < cap; i += (int64_t)gridDim.x * blockDim.x) hkey[i] = kEmpty;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < cap; i += (int64_t)gridDim.x * blockDim.x) hkey[i] = NL_HASH_EMPTY;
 }
 
 __global__ void k_hash_build(int n, const float *__restrict__ p, const uint64_t *__restrict__ key, const uint32_t *__restrict__ idx,
@@ -390,17 +384,17 @@ __global__ void k_hash_build(int n, const float *__restrict__ p, const uint64_t 
     pts[i] = make_float4(p[3 * j], p[3 * j + 1], p[3 * j + 2], 0.f);
     if (!flag[i]) return;
     const uint64_t k = key[i];
-    for (uint64_t s = mix64(k) & mask;; s = (s + 1) & mask) {
-        const unsigned long long prev = atomicCAS((unsigned long long *)&hkey[s], (unsigned long long)kEmpty, (unsigned long long)k);
-        if (prev == kEmpty) { hrun[s] = rid[i]; return; }
+    for (uint64_t s = nl_hash_mix(k) & mask;; s = (s + 1) & mask) {
+        const unsigned long long prev = atomicCAS((unsigned long long *)&hkey[s], (unsigned long long)NL_HASH_EMPTY, (unsigned long long)k);
+        if (prev == NL_HASH_EMPTY) { hrun[s] = rid[i]; return; }
     }
 }
 
 __device__ __forceinline__ int hash_find(const uint64_t *__restrict__ hkey, const int32_t *__restrict__ hrun, uint64_t mask, uint64_t k) {
-    for (uint64_t s = mix64(k) & mask;; s = (s + 1) & mask) {
+    for (uint64_t s = nl_hash_mix(k) & mask;; s = (s + 1) & mask) {
         const uint64_t h = hkey[s];
         if (h == k) return hrun[s];
-        if (h == kEmpty) return -1;
+        if (h == NL_HASH_EMPTY) return -1;
     }
 }
 

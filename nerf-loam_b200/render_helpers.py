@@ -281,37 +281,52 @@ class _few_threads:
 
 
 _FRAME_ARRAYS = weakref.WeakKeyDictionary()
+_FRAME_POINTS = weakref.WeakKeyDictionary()
+
+
+def _per_frame(table, f, src, dev, make):
+    """make(dev) -> tuple of device arrays derived from the frame's tensors `src`, computed once per frame OBJECT and kept in the
+    weak-key side table `table`, tied to the identity of the tensors in `src` (a frame whose tensors are REPLACED is uploaded again).
+    Nothing is attached to the frame itself, so pickling a frame (the reference passes frames between its processes through queues)
+    does not drag device memory along."""
+    dev = torch.device(dev)
+    n = len(src)
+    try:
+        c = table.get(f)
+    except TypeError:          # an unhashable / non-weakrefable frame type: no caching
+        c = False
+    if c and all(a is b for a, b in zip(c[:n], src)) and c[n].device.type == dev.type and \
+            (dev.index is None or dev.index == c[n].device.index):
+        return c[n:]
+    out = make(dev)
+    if out[0].is_cuda:
+        # the arrays outlive this call and may next be read on another stream (tracker and mapper run on different ones): make
+        # them complete now -- once per frame, and the uploads from pageable memory have stalled the host anyway
+        torch.cuda.current_stream(out[0].device).synchronize()
+    if c is not False:
+        try:
+            table[f] = src + out
+        except TypeError:
+            pass
+    return out
 
 
 def _frame_arrays(f, dev):
     """Device copies of a scan's per-point data: unit directions f32[n,3], incidence cosines f32[n], cosine-corrected ranges f32[n]
-    (criterion.py:30-32).  Computed once per frame OBJECT and kept in a weak-key side table: a keyframe stays in the optimisation
-    window for many calls (window_size 4-8) and the tracked frame goes straight into the next mapping call, while re-uploading
-    5 x 1.3 MB from pageable memory was ~10 % of a captured mapping call.  Tied to the identity of the frame's tensors (a frame whose
-    points / cosines / directions are REPLACED is uploaded again); nothing is attached to the frame itself, so pickling a frame
-    (the reference passes frames between its processes through queues) does not drag device memory along."""
-    dev = torch.device(dev)
-    src = (f.rays_d, f.pointsCos, f.points)
-    try:
-        c = _FRAME_ARRAYS.get(f)
-    except TypeError:          # an unhashable / non-weakrefable frame type: no caching
-        c = False
-    if c and c[0] is src[0] and c[1] is src[1] and c[2] is src[2] and c[3].device.type == dev.type and \
-            (dev.index is None or dev.index == c[3].device.index):
-        return c[3], c[4], c[5]
-    dirs = src[0].reshape(-1, 3).float().to(dev).contiguous()
-    cos = src[1].float().view(-1).to(dev).contiguous()
-    gt = torch.norm(src[2].float().to(dev), 2, -1) * cos
-    if gt.is_cuda:
-        # the arrays outlive this call and may next be read on another stream (tracker and mapper run on different ones): make
-        # them complete now -- once per frame, and the uploads from pageable memory have stalled the host anyway
-        torch.cuda.current_stream(gt.device).synchronize()
-    if c is not False:
-        try:
-            _FRAME_ARRAYS[f] = src + (dirs, cos, gt)
-        except TypeError:
-            pass
-    return dirs, cos, gt
+    (criterion.py:30-32), kept per frame object (_per_frame): a keyframe stays in the optimisation window for many calls
+    (window_size 4-8) and the tracked frame goes straight into the next mapping call, while re-uploading 5 x 1.3 MB from pageable
+    memory was ~10 % of a captured mapping call."""
+    def make(dev):
+        dirs = f.rays_d.reshape(-1, 3).float().to(dev).contiguous()
+        cos = f.pointsCos.float().view(-1).to(dev).contiguous()
+        return dirs, cos, torch.norm(f.points.float().to(dev), 2, -1) * cos
+    return _per_frame(_FRAME_ARRAYS, f, (f.rays_d, f.pointsCos, f.points), dev, make)
+
+
+def _frame_points(f, dev):
+    """Device copy of a scan's sensor-frame points f32[n,3], kept per frame object like _frame_arrays: the keyframe selection
+    (keyframes.keyframe_overlap) reads every keyframe's points in every mapping call."""
+    return _per_frame(_FRAME_POINTS, f, (f.points,), dev, lambda dev: (f.points.float().reshape(-1, 3).to(dev).contiguous(),))[0]
 
 
 class _FrameBatch:

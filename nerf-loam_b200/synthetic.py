@@ -41,6 +41,15 @@ def make_scan(n_beams=64, n_az=1563, seed=777, min_depth=5.0, max_depth=40.0, se
     return pts.astype(np.float32), cos.astype(np.float32), pose.astype(np.float32)
 
 
+def path_pose(i, n_scans, spacing, path="line"):
+    """(sensor_xyz, yaw) of scan i of scripts/demo_slam.py's drive.  "line": out along +x, spacing metres per scan.  "loop": out
+    along +x for the first half and back over the same ground in the second, so the last scan is taken where the first was."""
+    if path not in ("line", "loop"):
+        raise ValueError(f"path must be 'line' or 'loop', got {path!r}")
+    s = i if path == "line" else min(i, n_scans - 1 - i)
+    return (spacing * s, 0.05 * np.sin(0.7 * i), 0.0), 0.01 * np.sin(0.5 * i)
+
+
 def voxelize(points, pose, voxel_size):
     """src/mapping.py:283-290: sensor points -> world -> floor(/voxel_size) -> int32 voxel coords."""
     R = pose[:3, :3].astype(np.float32)

@@ -5,7 +5,12 @@ BASELINE.json config 2 ("KITTI seq 00 tracking+mapping incremental loop") / conf
 JSON summary (per-stage ms per scan, trajectory error against the synthetic ground truth, and under `reconstruction` the final mesh
 scored by evaluate.eval_mesh against the scans' noise-free returns at the true poses).
 
-    python scripts/demo_slam.py [--scans 12] [--spacing 0.5] [--octree host|device] [--json out.json]
+The mapping window goes through keyframes.KeyframeGraph (a keyframe every second scan, window_size 4): `--selection previous` (the
+default) optimises the last four keyframes, `--selection overlap` the four whose voxels overlap the tracked scan's most.  `--path loop`
+drives out along +x and back over the same ground (fresh noise seeds), so the last scans revisit the first ones' place.
+
+    python scripts/demo_slam.py [--scans 12] [--spacing 0.5] [--octree host|device] [--selection previous|overlap] [--path line|loop]
+                                [--json out.json]
 """
 import argparse, json, os, sys, time
 from types import SimpleNamespace
@@ -21,6 +26,8 @@ def main():
     ap.add_argument("--init-calls", type=int, default=12); ap.add_argument("--json", default=None)
     ap.add_argument("--ray-selection", default="device", choices=["device", "host"])
     ap.add_argument("--octree", default="host", choices=["host", "device"], help="where MapUpdater keeps the octree (the `update` stage)")
+    ap.add_argument("--selection", default="previous", choices=["previous", "overlap"], help="KeyframeGraph.select_optimize_targets method")
+    ap.add_argument("--path", default="line", choices=["line", "loop"], help="line: out along +x; loop: out and back over the same ground")
     a = ap.parse_args()
     dev = torch.device("cuda"); syn, rh = nl.synthetic, nl.render_helpers
     vs, md, trunc = 0.3, 40.0, 0.3
@@ -31,7 +38,8 @@ def main():
     mu = nl.mapping.MapUpdater(vs, device=dev, reserve_nodes=400_000, reserve_rows=400_000, octree=a.octree)   # embeddings start at zero like the reference
     shared = nl.share.SharedMap(lambda: nl.lidar.Decoder(depth=2, width=256, in_dim=16, skips=[], embedder="none", multires=0).to(dev))
     mu.readers = shared
-    scans = [syn.make_scan(seed=1000 + i, sensor_xyz=(a.spacing * i, 0.05 * np.sin(0.7 * i), 0.0), yaw=0.01 * np.sin(0.5 * i)) for i in range(a.scans)]
+    drive = [syn.path_pose(i, a.scans, a.spacing, a.path) for i in range(a.scans)]
+    scans = [syn.make_scan(seed=1000 + i, sensor_xyz=xyz, yaw=yaw) for i, (xyz, yaw) in enumerate(drive)]
     gt = [torch.from_numpy(s[2]) for s in scans]
     T = {k: [] for k in ("track", "map", "update", "publish")}
     def tick():
@@ -46,7 +54,10 @@ def main():
     t0 = tick()
     ms = mu.create_voxels(scans[0][0], gt[0])
     t_update0 = (tick() - t0) * 1e3
-    keyframes, est = [f0], [gt[0].clone()]
+    # key_distance = max_depth: every return of these scans lies inside it, so a keyframe holds the whole scan
+    kg = nl.keyframes.KeyframeGraph(window_size=4, keyframe_gap=2 * a.spacing, key_distance=md, n_rays=2048, voxel_size=vs)
+    kg.insert_keyframe(f0)
+    est, window = [gt[0].clone()], []
     t0 = tick()
     for _ in range(a.init_calls):
         ba([f0], True)
@@ -69,7 +80,8 @@ def main():
             pose = nl.se3pose.OptimizablePose.from_matrix(guess.clone())
         fr.pose = nl.se3pose.OptimizablePose(pose.data.detach().cpu().clone())
         t0 = tick()
-        ba(keyframes[-4:] + [fr], upd_dec=(i < 5))                                          # window_size 4 + the tracked frame, freeze_frame 5
+        window = kg.select_optimize_targets(fr, a.selection)                               # window_size 4 + the tracked frame
+        ba(window, upd_dec=(i < 5))                                                          # freeze_frame 5
         T["map"].append((tick() - t0) * 1e3)
         t0 = tick()
         ms = mu.create_voxels(scans[i][0], fr.get_pose().detach())
@@ -81,14 +93,14 @@ def main():
         rel = torch.linalg.inv(last) @ cur
         est.append(cur)
         if i % 2 == 0:
-            keyframes.append(fr)
+            kg.insert_keyframe(fr)
     t0 = tick()
     verts, faces = nl.mesh.extract_mesh(dec, ms, vs, res=8)
     t_mesh = (tick() - t0) * 1e3
     # the map against the scans' noise-free returns at the true poses, in world coordinates (with the 2000 m offset, like the mesh)
     clean = []
-    for i in range(a.scans):
-        p, _, pose = syn.make_scan(seed=1000 + i, sensor_xyz=(a.spacing * i, 0.05 * np.sin(0.7 * i), 0.0), yaw=0.01 * np.sin(0.5 * i), noise_std=0.0)
+    for i, (xyz, yaw) in enumerate(drive):
+        p, _, pose = syn.make_scan(seed=1000 + i, sensor_xyz=xyz, yaw=yaw, noise_std=0.0)
         clean.append(p.astype(np.float64) @ pose[:3, :3].T.astype(np.float64) + pose[:3, 3])
     t0 = tick()
     recon = nl.evaluate.eval_mesh(verts, faces, np.concatenate(clean).astype(np.float32), n_samples=1_000_000, res=0.05, threshold=0.1,
@@ -96,7 +108,8 @@ def main():
     recon["ms"] = (tick() - t0) * 1e3
     err =[float((e[:3, 3] - g[:3, 3]).norm()) for e, g in zip(est, gt)]
     rot = [float(torch.linalg.matrix_norm(e[:3, :3] - g[:3, :3])) for e, g in zip(est, gt)]
-    out = {"scans": a.scans, "spacing_m": a.spacing, "octree": a.octree, "translation_error_m": {"mean": float(np.mean(err[1:])), "max": float(np.max(err[1:])), "last": err[-1]},
+    out = {"scans": a.scans, "spacing_m": a.spacing, "octree": a.octree, "selection": a.selection, "path": a.path,
+           "last_window_scans": [f.index for f in window], "translation_error_m": {"mean": float(np.mean(err[1:])), "max": float(np.max(err[1:])), "last": err[-1]},
            "rotation_error_fro": {"mean": float(np.mean(rot[1:])), "max": float(np.max(rot[1:]))},
            "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0, "init_mapping_ms": t_init,
            "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
