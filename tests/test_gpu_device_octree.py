@@ -180,8 +180,10 @@ def test_bundle_adjust_on_device_map_equals_host_map(nl):
     bundle_adjust_frames itself is not reproducible bit for bit even on one map: the embedding, decoder and pose gradients are summed
     with fp32 atomics, and Adam turns last-bit differences of near-zero gradients into steps of up to the learning rate.  So three
     calls start from the same state -- two on the host map, one on the device map -- and the device run may differ from the first
-    host run no more than the second host run does (mean absolute difference; the floors are far below what a different map or
-    different embedding rows produce, ~1e-2)."""
+    host run no more than the second host run does, plus a floor (mean absolute difference).  The pose floor covers what that
+    mechanism does to the 18 pose components over the 15 Adam steps: two runs on the same map land ~7e-6 apart about as often as
+    ~1e-7 apart.  A fourth call from embeddings moved by 1e-2 must land farther from the first run than every floor, so the floors
+    still tell a different map state apart."""
     import copy
     rh = nl.render_helpers
     maps = {}
@@ -211,9 +213,10 @@ def test_bundle_adjust_on_device_map_equals_host_map(nl):
     emb0 = mh.embeddings.clone()
     N = min(s[0].shape[0] for s in scans)
     out = []
-    for octree in ("host", "host", "device"):
+    moved = (emb0.float() + 1e-2 * torch.randn(emb0.shape, generator=torch.Generator().manual_seed(5)).to(emb0.device)).to(emb0.dtype)
+    for octree, start in (("host", emb0), ("host", emb0), ("device", emb0), ("host", moved)):
         mu, ms = maps[octree]
-        mu.embeddings.copy_(emb0)
+        mu.embeddings.copy_(start)
         dec = copy.deepcopy(dec0)
         torch.manual_seed(11)                             # the device ray selection draws its seed from torch's generator
         frames = [nl.frame.LidarFrame(i + 1, torch.from_numpy(p[:N]), torch.from_numpy(c[:N]), nl.se3pose.OptimizablePose.from_matrix(torch.from_numpy(T.copy())),
@@ -224,12 +227,15 @@ def test_bundle_adjust_on_device_map_equals_host_map(nl):
         torch.cuda.synchronize()
         out.append((mu.embeddings.float().cpu(), torch.cat([p.detach().cpu().reshape(-1) for p in dec.parameters()]),
                     torch.cat([f.pose.data.detach().cpu().reshape(-1) for f in frames])))
-    (a, b, c) = out
-    for i, (k, floor) in enumerate(zip(("embeddings", "decoder", "poses"), (1e-5, 1e-6, 1e-6))):
+    (a, b, c, d) = out
+    for i, (k, floor) in enumerate(zip(("embeddings", "decoder", "poses"), (1e-5, 1e-6, 3e-5))):
         assert a[i].shape == c[i].shape and bool(torch.isfinite(c[i]).all()), k
         same_map = float((b[i] - a[i]).abs().mean())
         other_map = float((c[i] - a[i]).abs().mean())
+        other_start = float((d[i] - a[i]).abs().mean())
+        print(f"{k}: host vs host {same_map:.2e}, device vs host {other_map:.2e}, moved embeddings vs host {other_start:.2e}")
         assert other_map <= 4 * same_map + floor, (k, other_map, same_map)
+        assert other_start > 4 * same_map + floor, (k, other_start, same_map)
 
 
 def test_device_map_update_moves_no_bulk_data(nl):

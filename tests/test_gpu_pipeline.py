@@ -303,12 +303,27 @@ def test_fullsize_loss_and_ids_vs_oracle(nl, fullscan):
 def test_single_iteration_gradients_vs_oracle_autograd(nl):
     """One mapping iteration over 3 frames: loss and every gradient (embedding table, all decoder tensors, the
     6-vector of each frame pose) against autograd through the oracle's fp32 restatement of the reference."""
-    from oracle import chain as OC
     z = golden("mapping_tracking.npz")
+    single_iteration_vs_oracle(nl, z, load_decoder(z, "map_dec0_"))
+
+
+@pytest.mark.parametrize("width", [64, 128])
+def test_single_iteration_gradients_vs_oracle_autograd_cuda_core_widths(nl, width):
+    """The same iteration with a seeded decoder of width 64 or 128, which runs on the fp32 CUDA-core decoder (csrc/mlp.cu)."""
+    z = golden("mapping_tracking.npz")
+    torch.manual_seed(2000 + width)
+    dec = nl.lidar.Decoder(depth=2, width=width, in_dim=16, skips=[], embedder="none", multires=0).cuda()
+    single_iteration_vs_oracle(nl, z, dec)
+
+
+def single_iteration_vs_oracle(nl, z, dec):
+    """forward_backward over the first 3 scans of mapping_tracking.npz with decoder `dec` (any width), against the oracle's
+    mapping_iteration in fp32 and fp64: loss within 1e-5 and every gradient within 1e-4 of fp64 (norm-wise); prints the report."""
+    from oracle import chain as OC
     vs, md = float(z["voxel_size"]), float(z["max_distance"])
     pm = product_map(z["vox"], vs, z["id2emb"], z["emb_bf16"])
     m = pm["state"]
-    dec = load_decoder(z, "map_dec0_")
+    width = dec.pts_linears[0].weight.shape[0]
     crit = nl.criterion.Criterion(Args())
     dev = m.emb.device
     dirs, gts, coss, fids, frames_o = [], [], [], [], []
@@ -339,7 +354,7 @@ def test_single_iteration_gradients_vs_oracle_autograd(nl):
     # both oracle runs take the kernels' fp32 rays (nl_rays_from_poses vs torch's matmul may differ in the last bit of a direction)
     res, rays = {}, (eng.ray_o[:R].cpu().numpy().copy(), eng.ray_d[:R].cpu().numpy().copy())
     for dt in (torch.float32, torch.float64):
-        dec_o = OC.Decoder(depth=2, width=256, in_dim=16)
+        dec_o = OC.Decoder(depth=2, width=width, in_dim=16)
         dec_o.load_state_dict({k: v.cpu() for k, v in dec.state_dict().items()})
         dec_o = dec_o.to(dt)
         fr = [dict(pose=f["pose"].detach().clone().to(dt).requires_grad_(), dirs=f["dirs"].to(dt), points=f["points"].to(dt), cos=f["cos"].to(dt))
@@ -369,7 +384,7 @@ def test_single_iteration_gradients_vs_oracle_autograd(nl):
         assert report[f"pose{f}"][0] <= 1e-4, report
     report["emb"] = (rel(eng.grad_emb, r64["emb"]), rel(r32["emb"], r64["emb"]))
     assert report["emb"][0] <= 1e-4, report
-    print("gradient parity (kernels vs fp64, torch-fp32 vs fp64):", report)
+    print(f"gradient parity, width {width} (kernels vs fp64, torch-fp32 vs fp64):", report)
 
 
 def test_tensor_core_mlp_forward_matches_fp32_kernel(nl):
