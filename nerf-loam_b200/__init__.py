@@ -19,13 +19,15 @@ Public surface (mirrors the reference, see INTEGRATION.md):
                                     accuracy, completeness, Chamfer distance and F-score of a mesh against a reference cloud, on the GPU
     keyframes.KeyframeGraph / keyframe_overlap / rank_by_overlap  <- Mapping.insert_keyframe / select_optimize_targets (src/mapping.py),
                                     with the 'overlap' window the reference leaves unimplemented (voxel IoU with the scan, on the GPU)
+    ground.points_and_cos / segment_ground  <- the Patchwork++ ground segmentation and pointsCos of src/dataset/kitti.py:40-70, on the GPU
+    dataset.kitti / dataset.maicity .DataLoader  <- src/dataset/kitti.py, maicity.py (seam: sys.modules["dataset"] = nerfloam_b200.dataset)
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
 no CPU or eager-PyTorch fallback for the kernels.
 """
 from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
-           "evaluate", "keyframes", "track_batch", "track_frames", "score", "score_poses", "relocalise"]
+           "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise"]
 
 
 def __getattr__(name):

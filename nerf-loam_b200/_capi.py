@@ -47,6 +47,18 @@ class BatchArgs(C.Structure):
                 ("d_problem_base", vp)]
 
 
+class GroundParams(C.Structure):
+    """nl_ground_params (include/nerfloam_b200.h section 13)."""
+    _fields_ = [("sensor_height", C.c_double), ("min_range", C.c_double), ("max_range", C.c_double),
+                ("num_rings_each_zone", C.c_int32 * 4), ("num_sectors_each_zone", C.c_int32 * 4), ("uprightness_thr", C.c_double),
+                ("elevation_thr", C.c_double * 4), ("flatness_thr", C.c_double * 4), ("num_iter", C.c_int32), ("num_lpr", C.c_int32),
+                ("num_min_pts", C.c_int32), ("_pad", C.c_int32), ("th_seeds", C.c_double), ("th_dist", C.c_double),
+                ("adaptive_seed_margin", C.c_double)]
+
+
+GROUND_PATCH_BYTES = 80      # sizeof(nl_ground_patch): mean[3], normal[3], d, lambda_min (f64), n_points, n_ground, ground, ring (i32)
+
+
 class MlpWeights(C.Structure):
     _fields_ = [("width", C.c_int32), ("W0", vp), ("b0", vp), ("W1", vp), ("b1", vp), ("W2", vp), ("b2", vp),
                 ("W0t", vp), ("W1t", vp)]
@@ -165,6 +177,11 @@ _SIGNATURES = {
     # keyframe overlap (include/nerfloam_b200.h section 12)
     "nl_keyframe_overlap_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
     "nl_keyframe_overlap": (C.c_int, [C.c_int64, vp, C.c_int32, vp, vp, vp, vp, C.c_double, C.c_int64, C.c_int64, vp, C.c_int64, vp, vp]),
+    # ground segmentation (include/nerfloam_b200.h section 13)
+    "nl_abi_sizes_ground": (None, [C.POINTER(C.c_int32 * 3)]),
+    "nl_ground_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "nl_ground_segment": (C.c_int, [C.c_int64, vp, C.c_int32, C.POINTER(GroundParams), vp, C.c_int64, vp, vp, vp, vp, vp, vp]),
+    "nl_ground_partition": (C.c_int, [C.c_int64, vp, C.c_int32, vp, vp, vp, C.c_int64, vp, vp, vp, vp]),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)
@@ -174,6 +191,7 @@ BATCH_MAX_PROBLEMS = 31      # NL_BATCH_MAX_PROBLEMS
 SCORE_MAX_PROBLEMS = 65535   # NL_SCORE_MAX_PROBLEMS
 EVAL_KEY_BITS = 21           # NL_EVAL_KEY_BITS
 EVAL_TILE = 2048             # NL_EVAL_TILE
+GROUND_MAX_PATCHES = 1024    # NL_GROUND_MAX_PATCHES
 STATS_PACK_FIXED = 10
 # node-array checks, bit i = 1 << i (NL_TREE_* in include/nerfloam_b200.h section 1)
 TREE_CHECKS = ("ROOT", "RANGE", "LINK", "PARENTS", "SHAPE", "ROWS", "VERTICES")
@@ -223,6 +241,11 @@ def lib():
         L.nl_abi_sizes_eval(C.byref(esizes))
         if list(esizes) != [EVAL_KEY_BITS, EVAL_TILE]:
             raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (eval): {list(esizes)} vs {[EVAL_KEY_BITS, EVAL_TILE]}")
+        gsizes = (C.c_int32 * 3)()
+        L.nl_abi_sizes_ground(C.byref(gsizes))
+        gmine = [C.sizeof(GroundParams), GROUND_MAX_PATCHES, GROUND_PATCH_BYTES]
+        if list(gsizes) != gmine:
+            raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (ground): {list(gsizes)} vs {gmine}")
         _lib = L
     return _lib
 

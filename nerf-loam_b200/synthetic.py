@@ -5,7 +5,8 @@ spinning LiDAR (elevation -24.8 .. +2.0 deg) x n_az azimuths inside a box-shaped
 ground plane z = -1.73 m, walls |y| = 8 m and |x| = 30 m, range noise N(0, 0.02^2) m, range gate
 (min_depth, max_depth).  `points` are in the sensor frame like the reference data loaders return
 them (src/dataset/kitti.py:75-81), `pointsCos` is |n.d| for ground returns and 1 elsewhere (the
-reference computes it with patchwork++ ground segmentation, src/dataset/kitti.py:40-70).
+reference computes it with patchwork++ ground segmentation, src/dataset/kitti.py:40-70; ground.points_and_cos computes it from
+the points alone, as dataset.kitti / dataset.maicity do for recorded scans).
 """
 import numpy as np
 

@@ -11,6 +11,11 @@ drives out along +x and back over the same ground (fresh noise seeds), so the la
 
     python scripts/demo_slam.py [--scans 12] [--spacing 0.5] [--octree host|device] [--selection previous|overlap] [--path line|loop]
                                 [--json out.json]
+
+`--data DIR --dataset kitti|maicity` runs the same loop on a recorded sequence through dataset.<name>.DataLoader (points and pointsCos
+from the GPU ground segmentation, ground.py): the first scan takes the loader's get_init_pose, every later one is tracked; the
+trajectory error is reported against the pose file when it exists, and the `reconstruction` block (synthetic scans only) is left out.
+`--scans` then caps the number of scans (default: all).
 """
 import argparse, json, os, sys, time
 from types import SimpleNamespace
@@ -20,14 +25,46 @@ sys.path.insert(0, ROOT)
 import nerfloam_b200 as nl
 
 
+def load_sequence(a):
+    """(scans [(points, pointsCos)] as numpy, true poses or None, the first scan's pose) of --data through its DataLoader; poses carry
+    the offset LidarFrame adds to a supplied pose."""
+    import importlib
+    loader = importlib.import_module("nerf-loam_b200.dataset." + a.dataset).DataLoader
+    has_poses = os.path.exists(os.path.join(a.data, loader.pose_file))
+    data = loader(a.data, use_gt=has_poses)
+    a.scans = len(data) if a.scans is None else min(a.scans, len(data))
+    if a.scans < 2:
+        raise SystemExit(f"{a.data}: need at least 2 scans, found {len(data)}")
+    scans = []
+    for i in range(a.scans):
+        _, points, pointcos, _ = data[i]
+        scans.append((points.numpy(), pointcos.numpy()))
+    def shifted(pose):
+        pose = np.array(pose, dtype=np.float32)
+        pose[:3, 3] += nl.frame.POSE_OFFSET
+        return torch.from_numpy(pose)
+    gt = [shifted(data.get_init_pose(i)) for i in range(a.scans)] if has_poses else None
+    return scans, gt, shifted(data.get_init_pose(0))
+
+
+def trajectory_errors(est, gt):
+    err = [float((e[:3, 3] - g[:3, 3]).norm()) for e, g in zip(est, gt)]
+    rot = [float(torch.linalg.matrix_norm(e[:3, :3] - g[:3, :3])) for e, g in zip(est, gt)]
+    return {"translation_error_m": {"mean": float(np.mean(err[1:])), "max": float(np.max(err[1:])), "last": err[-1]},
+            "rotation_error_fro": {"mean": float(np.mean(rot[1:])), "max": float(np.max(rot[1:]))},
+            "per_scan_translation_error_m": [round(e, 4) for e in err]}
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--scans", type=int, default=12); ap.add_argument("--spacing", type=float, default=0.5)
+    ap.add_argument("--scans", type=int, default=None, help="number of scans (default 12, or the whole sequence with --data)"); ap.add_argument("--spacing", type=float, default=0.5)
     ap.add_argument("--init-calls", type=int, default=12); ap.add_argument("--json", default=None)
     ap.add_argument("--ray-selection", default="device", choices=["device", "host"])
     ap.add_argument("--octree", default="host", choices=["host", "device"], help="where MapUpdater keeps the octree (the `update` stage)")
     ap.add_argument("--selection", default="previous", choices=["previous", "overlap"], help="KeyframeGraph.select_optimize_targets method")
     ap.add_argument("--path", default="line", choices=["line", "loop"], help="line: out along +x; loop: out and back over the same ground")
+    ap.add_argument("--data", default=None, help="a KITTI- or MaiCity-layout sequence directory instead of synthetic scans")
+    ap.add_argument("--dataset", default="kitti", choices=["kitti", "maicity"], help="layout of --data")
     a = ap.parse_args()
     dev = torch.device("cuda"); syn, rh = nl.synthetic, nl.render_helpers
     vs, md, trunc = 0.3, 40.0, 0.3
@@ -38,9 +75,14 @@ def main():
     mu = nl.mapping.MapUpdater(vs, device=dev, reserve_nodes=400_000, reserve_rows=400_000, octree=a.octree)   # embeddings start at zero like the reference
     shared = nl.share.SharedMap(lambda: nl.lidar.Decoder(depth=2, width=256, in_dim=16, skips=[], embedder="none", multires=0).to(dev))
     mu.readers = shared
-    drive = [syn.path_pose(i, a.scans, a.spacing, a.path) for i in range(a.scans)]
-    scans = [syn.make_scan(seed=1000 + i, sensor_xyz=xyz, yaw=yaw) for i, (xyz, yaw) in enumerate(drive)]
-    gt = [torch.from_numpy(s[2]) for s in scans]
+    if a.data is None:
+        a.scans = 12 if a.scans is None else a.scans
+        drive = [syn.path_pose(i, a.scans, a.spacing, a.path) for i in range(a.scans)]
+        scans = [syn.make_scan(seed=1000 + i, sensor_xyz=xyz, yaw=yaw) for i, (xyz, yaw) in enumerate(drive)]
+        gt = [torch.from_numpy(s[2]) for s in scans]
+        init = gt[0]
+    else:
+        scans, gt, init = load_sequence(a)
     T = {k: [] for k in ("track", "map", "update", "publish")}
     def tick():
         torch.cuda.synchronize(); return time.perf_counter()
@@ -50,14 +92,14 @@ def main():
                                                             max_voxel_hit=20, max_distance=md, learning_rate=lr, update_pose=True, update_decoder=upd_dec,
                                                             ray_selection=a.ray_selection)
     # ---- first scan: map it, then train on it while "waiting for the tracker" (mapping.py:100-108) ----
-    f0 = mk(0, nl.se3pose.OptimizablePose.from_matrix(gt[0].clone()))
+    f0 = mk(0, nl.se3pose.OptimizablePose.from_matrix(init.clone()))
     t0 = tick()
-    ms = mu.create_voxels(scans[0][0], gt[0])
+    ms = mu.create_voxels(scans[0][0], init)
     t_update0 = (tick() - t0) * 1e3
     # key_distance = max_depth: every return of these scans lies inside it, so a keyframe holds the whole scan
     kg = nl.keyframes.KeyframeGraph(window_size=4, keyframe_gap=2 * a.spacing, key_distance=md, n_rays=2048, voxel_size=vs)
     kg.insert_keyframe(f0)
-    est, window = [gt[0].clone()], []
+    est, window = [init.clone()], []
     t0 = tick()
     for _ in range(a.init_calls):
         ba([f0], True)
@@ -97,6 +139,18 @@ def main():
     t0 = tick()
     verts, faces = nl.mesh.extract_mesh(dec, ms, vs, res=8)
     t_mesh = (tick() - t0) * 1e3
+    if a.data is not None:
+        out = {"data": a.data, "dataset": a.dataset, "scans": a.scans, "octree": a.octree, "selection": a.selection,
+               "last_window_scans": [f.index for f in window], "ground_points": [int((s[1] < 1).sum()) for s in scans],
+               "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0,
+               "init_mapping_ms": t_init, "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
+               "map": {"nodes": ms.n_nodes, "embedding_rows": int(mu.n_rows), "last_update": mu.last_update}}
+        if gt is not None:
+            out.update(trajectory_errors(est, gt))
+        print(json.dumps(out))
+        if a.json:
+            json.dump(out, open(a.json, "w"), indent=1)
+        return
     # the map against the scans' noise-free returns at the true poses, in world coordinates (with the 2000 m offset, like the mesh)
     clean = []
     for i, (xyz, yaw) in enumerate(drive):
@@ -106,16 +160,15 @@ def main():
     recon = nl.evaluate.eval_mesh(verts, faces, np.concatenate(clean).astype(np.float32), n_samples=1_000_000, res=0.05, threshold=0.1,
                                   truncation=0.5, seed=0)
     recon["ms"] = (tick() - t0) * 1e3
-    err =[float((e[:3, 3] - g[:3, 3]).norm()) for e, g in zip(est, gt)]
-    rot = [float(torch.linalg.matrix_norm(e[:3, :3] - g[:3, :3])) for e, g in zip(est, gt)]
+    errors = trajectory_errors(est, gt)
     out = {"scans": a.scans, "spacing_m": a.spacing, "octree": a.octree, "selection": a.selection, "path": a.path,
-           "last_window_scans": [f.index for f in window], "translation_error_m": {"mean": float(np.mean(err[1:])), "max": float(np.max(err[1:])), "last": err[-1]},
-           "rotation_error_fro": {"mean": float(np.mean(rot[1:])), "max": float(np.max(rot[1:]))},
+           "last_window_scans": [f.index for f in window], "translation_error_m": errors["translation_error_m"],
+           "rotation_error_fro": errors["rotation_error_fro"],
            "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0, "init_mapping_ms": t_init,
            "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
            "map": {"nodes": ms.n_nodes, "embedding_rows": int(mu.n_rows), "last_update": mu.last_update},
            "reconstruction": recon,
-           "per_scan_translation_error_m": [round(e, 4) for e in err]}
+           "per_scan_translation_error_m": errors["per_scan_translation_error_m"]}
     print(json.dumps(out))
     if a.json:
         json.dump(out, open(a.json, "w"), indent=1)

@@ -1,0 +1,85 @@
+"""Time ground.points_and_cos (csrc/ground.cu) and dataset.kitti.DataLoader.__getitem__ against the NumPy restatement of
+tests/ground_ref.py on the host, on synthetic 64 x 1563 scans (synthetic.make_scan, ~10^5 returns) and, with --data, on the scans of a
+KITTI-layout sequence.  The kernel and the restatement run alternately in one process; every GPU call ends in a device synchronise.
+Prints the card, its power limit and one line per case (median and min-max in ms), and checks that the labels agree.
+
+    python scripts/time_ground.py [--reps 9] [--numpy-reps 3] [--scans 4] [--data DIR] [--json out.json]
+"""
+import argparse, json, os, subprocess, sys, tempfile, time
+import numpy as np, torch
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import nerfloam_b200 as nl
+import ground_ref as GR
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True,
+                           timeout=30).stdout.strip()
+        return q or torch.cuda.get_device_name(0)
+    except (OSError, subprocess.SubprocessError):
+        return torch.cuda.get_device_name(0) + ", power limit unknown"
+
+
+def timed(fn):
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    out = fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) * 1e3, out
+
+
+def stats(v):
+    return {"median_ms": float(np.median(v)), "min_ms": float(np.min(v)), "max_ms": float(np.max(v)), "runs": len(v)}
+
+
+def write_kitti(root, scans):
+    os.makedirs(os.path.join(root, "velodyne"), exist_ok=True)
+    for i, p in enumerate(scans):
+        np.concatenate([p, np.zeros((len(p), 1), np.float32)], 1).tofile(os.path.join(root, "velodyne", f"{i:06d}.bin"))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=9); ap.add_argument("--numpy-reps", type=int, default=3)
+    ap.add_argument("--scans", type=int, default=4); ap.add_argument("--data", default=None); ap.add_argument("--json", default=None)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("time_ground.py needs a CUDA device")
+    info = card()
+    print(f"card: {info}")
+    params = nl.ground.GroundParams()
+    rows = []
+    with tempfile.TemporaryDirectory() as tmp:
+        synthetic = [nl.synthetic.make_scan(seed=2000 + i, sensor_xyz=(0.5 * i, 0.0, 0.0))[0] for i in range(a.scans)]
+        write_kitti(tmp, synthetic)
+        sources = [("synthetic 64x1563", tmp)] + ([("data " + a.data, a.data)] if a.data else [])
+        for name, path in sources:
+            loader = nl.dataset.kitti.DataLoader(path)
+            for i in range(min(a.scans, len(loader))):
+                raw = loader.read_points(i)
+                dev = torch.from_numpy(raw).cuda()
+                ref = GR.segment(raw, params)
+                kern = lambda: nl.ground.points_and_cos(dev, params)
+                timed(kern); timed(lambda: loader[i])                    # warm-up
+                t = {"points_and_cos (device input)": [], "__getitem__ (file to CPU tensors)": [], "restatement (host)": []}
+                for r in range(a.reps):
+                    ms, out = timed(kern); t["points_and_cos (device input)"].append(ms)
+                    ms, item = timed(lambda: loader[i]); t["__getitem__ (file to CPU tensors)"].append(ms)
+                    if r < a.numpy_reps:
+                        ms, _ = timed(lambda: GR.segment(raw, params)); t["restatement (host)"].append(ms)
+                g = int((ref["label"] == 1).sum())
+                agree = float((nl.ground.segment_ground(dev, params).label.cpu().numpy() == ref["label"]).mean())
+                row = {"source": name, "scan": i, "points": int(len(raw)), "ground": g, "label_agreement": agree}
+                row.update({k: stats(v) for k, v in t.items()})
+                rows.append(row)
+                print(f"{name} scan {i}: {len(raw)} points, {g} ground, labels agree {agree:.6f}  " + "  ".join(
+                    f"{k} {row[k]['median_ms']:.3f} ms ({row[k]['min_ms']:.3f}-{row[k]['max_ms']:.3f})" for k in t), flush=True)
+    if a.json:
+        json.dump({"card": info, "rows": rows}, open(a.json, "w"), indent=1)
+
+
+if __name__ == "__main__":
+    main()
