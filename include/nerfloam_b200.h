@@ -638,6 +638,10 @@ NL_API int nl_keyframe_overlap(int64_t n_frame, const float *d_frame_pts, int32_
  *     points of each patch, num_iter principal-component plane fits, an uprightness and elevation verdict, and for a ground point
  *     cos = |n.p| / |p| with n the normal of the ground patch whose mean is nearest.  csrc/ground.cu; nerf-loam_b200/ground.py
  *     composes the calls.  Every sum is fp64 in a fixed order, so two calls give identical bytes.
+ *     Opt-in vertical-structure filter (DESIGN.md section 12.1; vertical_cell > 0): a row inside the ranges whose xy column
+ *     (floor(x / vertical_cell), floor(y / vertical_cell)) holds returns spread over more than vertical_height in z is vertical:
+ *     never a seed candidate nor in a fit, labelled non-ground with cos 1.  The columns' z extents come from a hash table with
+ *     integer atomics on order-preserving keys, so they are exact and two calls still give identical bytes.
  * ============================================================================================ */
 #define NL_GROUND_MAX_PATCHES 1024   /* sum over the zones of rings x sectors */
 #define NL_GROUND_MAX_LPR 1024       /* largest num_lpr */
@@ -649,22 +653,33 @@ typedef struct nl_ground_params {     /* Patchwork++'s parameter names; ranges a
     double flatness_thr[4];           /* carried for completeness; not used by the verdict */
     int32_t num_iter, num_lpr, num_min_pts, _pad;
     double th_seeds, th_dist, adaptive_seed_margin;
+    double vertical_cell;             /* column width of the vertical-structure filter in metres; 0 = off */
+    double vertical_height;           /* a column whose z extent exceeds it (strictly) is vertical; > 0 when the filter is on */
 } nl_ground_params;
 typedef struct nl_ground_patch {      /* one patch; the doubles are NaN when the patch has no complete fit */
     double mean[3], normal[3];        /* the last fit: mean, unit normal with normal[2] >= 0 */
     double d, lambda_min;             /* plane n.p + d = 0, smallest covariance eigenvalue */
-    int32_t n_points, n_ground, ground, ring;   /* points in the patch, points labelled ground, verdict, global ring */
+    int32_t n_points, n_ground, ground, ring;   /* points in the patch (vertical ones included), points labelled ground, verdict, global ring */
+    int32_t n_vertical, _pad;         /* vertical points in the patch (0 with the filter off) */
 } nl_ground_patch;
 /* out = (sizeof(nl_ground_params), NL_GROUND_MAX_PATCHES, sizeof(nl_ground_patch)) */
 NL_API void nl_abi_sizes_ground(int32_t out[3]);
 NL_API int64_t nl_ground_workspace_bytes(int64_t n);
+/* The vertical filter's column table: 16 bytes per slot (8-byte key, u32 z min and max) and a power of two >= 2n slots. */
+NL_API int64_t nl_ground_vertical_workspace_bytes(int64_t n);
 /* d_points f32 rows of `stride` (3, or 4 with the intensity ignored) floats, n >= 0.  Writes d_label u8[n] (1 = ground),
  * d_cos f32[n] (1 for every non-ground point), d_patch i32[n] (patch id, -1 outside the ranges or not finite; may be NULL),
  * d_patches (one record per patch, zone by zone, ring by ring, sector by sector; may be NULL) and d_counts i64[4] = (ground,
  * non-ground, outside, non-finite); non-ground counts the outside and non-finite rows too.  The workspace (256-byte aligned) has
- * nl_ground_workspace_bytes(n) bytes.  No host synchronisation. */
+ * nl_ground_workspace_bytes(n) bytes.  No host synchronisation.  The vertical filter needs nl_ground_segment_vertical. */
 NL_API int nl_ground_segment(int64_t n, const float *d_points, int32_t stride, const nl_ground_params *params, void *d_ws, int64_t ws_bytes,
                              uint8_t *d_label, float *d_cos, int32_t *d_patch, nl_ground_patch *d_patches, int64_t *d_counts, void *stream);
+/* nl_ground_segment with the vertical filter.  With params->vertical_cell > 0 it needs d_vws (256-byte aligned,
+ * nl_ground_vertical_workspace_bytes(n) bytes) and writes d_vertical u8[n] (1 = vertical); with vertical_cell = 0 both may be NULL,
+ * no extra kernel runs, the results are nl_ground_segment's, and a non-NULL d_vertical is zeroed. */
+NL_API int nl_ground_segment_vertical(int64_t n, const float *d_points, int32_t stride, const nl_ground_params *params, void *d_ws,
+                                      int64_t ws_bytes, void *d_vws, int64_t vws_bytes, uint8_t *d_label, float *d_cos, int32_t *d_patch,
+                                      nl_ground_patch *d_patches, uint8_t *d_vertical, int64_t *d_counts, void *stream);
 /* Stable partition by d_label: the ground rows first, then the rest, each in input order.  d_out_points f32[n,3], d_out_cos f32[n]
  * and d_out_index i32[n] (the input row of each output row). */
 NL_API int nl_ground_partition(int64_t n, const float *d_points, int32_t stride, const uint8_t *d_label, const float *d_cos, void *d_ws,

@@ -53,10 +53,10 @@ class GroundParams(C.Structure):
                 ("num_rings_each_zone", C.c_int32 * 4), ("num_sectors_each_zone", C.c_int32 * 4), ("uprightness_thr", C.c_double),
                 ("elevation_thr", C.c_double * 4), ("flatness_thr", C.c_double * 4), ("num_iter", C.c_int32), ("num_lpr", C.c_int32),
                 ("num_min_pts", C.c_int32), ("_pad", C.c_int32), ("th_seeds", C.c_double), ("th_dist", C.c_double),
-                ("adaptive_seed_margin", C.c_double)]
+                ("adaptive_seed_margin", C.c_double), ("vertical_cell", C.c_double), ("vertical_height", C.c_double)]
 
 
-GROUND_PATCH_BYTES = 80      # sizeof(nl_ground_patch): mean[3], normal[3], d, lambda_min (f64), n_points, n_ground, ground, ring (i32)
+GROUND_PATCH_BYTES = 88      # sizeof(nl_ground_patch): mean[3], normal[3], d, lambda_min (f64), n_points, n_ground, ground, ring, n_vertical, pad (i32)
 
 
 class MlpWeights(C.Structure):
@@ -181,6 +181,9 @@ _SIGNATURES = {
     "nl_abi_sizes_ground": (None, [C.POINTER(C.c_int32 * 3)]),
     "nl_ground_workspace_bytes": (C.c_int64, [C.c_int64]),
     "nl_ground_segment": (C.c_int, [C.c_int64, vp, C.c_int32, C.POINTER(GroundParams), vp, C.c_int64, vp, vp, vp, vp, vp, vp]),
+    "nl_ground_vertical_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "nl_ground_segment_vertical": (C.c_int, [C.c_int64, vp, C.c_int32, C.POINTER(GroundParams), vp, C.c_int64, vp, C.c_int64, vp, vp, vp, vp,
+                                             vp, vp, vp]),
     "nl_ground_partition": (C.c_int, [C.c_int64, vp, C.c_int32, vp, vp, vp, C.c_int64, vp, vp, vp, vp]),
 }
 

@@ -11,6 +11,12 @@
 //               thread runs the same cyclic Jacobi eigen-solve on the result.  Then the verdict and the labels.
 //   cosine    : one thread per point; every CTA compacts the ground patches (mean, normal) into shared memory in id order.
 //   partition : flags -> exclusive scan -> scatter; both halves keep input order (cub::DevicePartition reverses the rejected half).
+//   vertical  : only with vertical_cell > 0 (DESIGN.md section 12.1), between binning and the sort.  Column pass: one thread per
+//               row inside the ranges inserts its cell key into an open-addressing table (hash.cuh) and folds its z into the slot's
+//               min and max with integer atomicMin / atomicMax on order-preserving u32 keys.  Flag pass: one thread per row marks it
+//               vertical from its slot's extent.  The gather carries the flag in the float4's .w, and k_fit<true> leaves flagged
+//               rows out of the candidates, every S and the labels.  With the filter off none of this runs and k_fit<false> is the
+//               unfiltered fit.
 // No floating-point atomics anywhere, so two calls give identical bytes.
 #include <cub/cub.cuh>
 
@@ -20,6 +26,7 @@
 #include <cstdio>
 
 #include "../../include/nerfloam_b200.h"
+#include "hash.cuh"
 #include "nl_cuda.cuh"
 
 namespace {
@@ -45,6 +52,19 @@ struct Fit {
     double seed_floor, th_seeds, th_dist, upright, sensor_height, elevation[4];
     int num_iter, num_lpr, num_min_pts;
 };
+
+struct Vert {
+    double cell = 0.0, height = 0.0;   // cell 0: the filter is off
+};
+
+constexpr double kMaxCells = 1073741824.0;                     // max_range / vertical_cell <= 2^30 keeps the cell indices in int32
+constexpr int64_t kMinColumnSlots = 256;
+
+int64_t column_slots(int64_t n) {                              // a power of two >= 2n
+    int64_t c = kMinColumnSlots;
+    while (c < 2 * n) c <<= 1;
+    return c;
+}
 
 size_t take(size_t &at, size_t bytes) {
     const size_t o = (at + 255) & ~size_t(255);
@@ -129,12 +149,13 @@ __global__ void __launch_bounds__(kThreads) k_bin(int n, const float *__restrict
     if (bad) atomicAdd((unsigned long long *)&counts[3], (unsigned long long)bad);
 }
 
+// .w = 1 for a vertical row (vert: the flag pass's u8[n], nullptr with the filter off), else 0
 __global__ void k_gather(int n, const float *__restrict__ p, int stride, const uint32_t *__restrict__ idx, const int32_t *__restrict__ start,
-                         int n_patches, float4 *pts) {
+                         int n_patches, const uint8_t *__restrict__ vert, float4 *pts) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= start[n_patches]) return;                         // the sorted tail is the outside and non-finite rows
     const int64_t i = (int64_t)stride * idx[j];
-    pts[j] = make_float4(p[i], p[i + 1], p[i + 2], 0.f);
+    pts[j] = make_float4(p[i], p[i + 1], p[i + 2], vert && vert[idx[j]] ? 1.f : 0.f);
 }
 
 // ---- fit ------------------------------------------------------------------------------------------------------------------
@@ -214,6 +235,8 @@ __device__ __forceinline__ int global_ring(const Geo &g, int id) {
     return g.ring_off[z] + (id - g.patch_off[z]) / g.sectors[z];
 }
 
+// V: the vertical filter is on, and a row with .w != 0 takes no part in the seeds, the fits or the labels
+template <bool V>
 __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *__restrict__ start, const float4 *__restrict__ pts,
                                                   const uint32_t *__restrict__ idx, uint8_t *label, nl_ground_patch *rec, int64_t *counts) {
     __shared__ double red[6][kWarps];
@@ -228,12 +251,21 @@ __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *_
     double mean[3] = {nan, nan, nan}, nrm[3] = {nan, nan, nan}, d = nan, lam = nan;
     int ground = 0;
     double n_ground = 0.0;
-    // candidates: every point, except zone 0's below adaptive_seed_margin * sensor_height
-    auto cand = [&](float z) { return !(zone0 && (double)z < f.seed_floor); };
+    // candidates: every point, except zone 0's below adaptive_seed_margin * sensor_height (and the vertical ones)
+    auto cand = [&](int j, float z) { return !(V && P[j].w != 0.f) && !(zone0 && (double)z < f.seed_floor); };
+    auto kept = [](float4 q) { return !(V && q.w != 0.f); };
+    int n_vert = 0;
+    if (V && cnt > 0) {
+        double nv[1] = {0.0};
+        for (int j = threadIdx.x; j < cnt; j += kThreads) nv[0] += P[j].w != 0.f ? 1.0 : 0.0;
+        block_sum<1>(nv, red);
+        n_vert = (int)nv[0];
+    }
+    const int n_fit = cnt - n_vert;                            // num_min_pts counts the rows a fit may use
     bool fitted = false;
-    if (cnt >= f.num_min_pts && cnt > 0) {
+    if (n_fit >= f.num_min_pts && n_fit > 0) {
         double nc[1] = {0.0};
-        for (int j = threadIdx.x; j < cnt; j += kThreads) nc[0] += cand(P[j].z) ? 1.0 : 0.0;
+        for (int j = threadIdx.x; j < cnt; j += kThreads) nc[0] += cand(j, P[j].z) ? 1.0 : 0.0;
         block_sum<1>(nc, red);
         const int n_cand = (int)nc[0];
         if (n_cand > 0) {
@@ -246,7 +278,7 @@ __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *_
                 for (int j = threadIdx.x; j < cnt; j += kThreads) {
                     const float z = P[j].z;
                     const uint32_t o = ord_of(z);
-                    if (cand(z) && (o & mask) == prefix) atomicAdd(&hist[(o >> shift) & 255u], 1u);
+                    if (cand(j, z) && (o & mask) == prefix) atomicAdd(&hist[(o >> shift) & 255u], 1u);
                 }
                 __syncthreads();
                 if (threadIdx.x == 0) {
@@ -266,7 +298,7 @@ __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *_
             __syncthreads();
             for (int j = threadIdx.x; j < cnt; j += kThreads) {
                 const float z = P[j].z;
-                if (cand(z) && ord_of(z) < prefix) low[atomicAdd(&n_low, 1u)] = z;
+                if (cand(j, z) && ord_of(z) < prefix) low[atomicAdd(&n_low, 1u)] = z;
             }
             __syncthreads();
             const int m = (int)n_low;
@@ -292,7 +324,7 @@ __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *_
                 double s[4] = {0.0, 0.0, 0.0, 0.0};
                 for (int j = threadIdx.x; j < cnt; j += kThreads) {
                     const float4 q = P[j];
-                    const bool in = t == 0 ? (cand(q.z) && (double)q.z < cut) : plane_dist(nrm, d, q) < f.th_dist;
+                    const bool in = t == 0 ? (cand(j, q.z) && (double)q.z < cut) : kept(q) && plane_dist(nrm, d, q) < f.th_dist;
                     if (in) { s[0] += 1.0; s[1] += q.x; s[2] += q.y; s[3] += q.z; }
                 }
                 block_sum<4>(s, red);
@@ -301,7 +333,7 @@ __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *_
                 double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
                 for (int j = threadIdx.x; j < cnt; j += kThreads) {
                     const float4 q = P[j];
-                    const bool in = t == 0 ? (cand(q.z) && (double)q.z < cut) : plane_dist(nrm, d, q) < f.th_dist;
+                    const bool in = t == 0 ? (cand(j, q.z) && (double)q.z < cut) : kept(q) && plane_dist(nrm, d, q) < f.th_dist;
                     if (in) {
                         const double dx = q.x - mu[0], dy = q.y - mu[1], dz = q.z - mu[2];
                         c[0] += dx * dx; c[1] += dx * dy; c[2] += dx * dz; c[3] += dy * dy; c[4] += dy * dz; c[5] += dz * dz;
@@ -323,7 +355,7 @@ __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *_
         if (ground) {
             double ng[1] = {0.0};
             for (int j = threadIdx.x; j < cnt; j += kThreads)
-                if (plane_dist(nrm, d, P[j]) < f.th_dist) { label[idx[b + j]] = 1; ng[0] += 1.0; }
+                if (kept(P[j]) && plane_dist(nrm, d, P[j]) < f.th_dist) { label[idx[b + j]] = 1; ng[0] += 1.0; }
             block_sum<1>(ng, red);
             n_ground = ng[0];
         }
@@ -335,8 +367,45 @@ __global__ void __launch_bounds__(kThreads) k_fit(Geo g, Fit f, const int32_t *_
         for (int k = 0; k < 3; ++k) { o.mean[k] = mean[k]; o.normal[k] = nrm[k]; }
         o.d = d; o.lambda_min = lam;
         o.n_points = cnt; o.n_ground = (int32_t)n_ground; o.ground = ground; o.ring = ring;
+        o.n_vertical = n_vert; o._pad = 0;
         rec[id] = o;
         if (o.n_ground) atomicAdd((unsigned long long *)&counts[0], (unsigned long long)o.n_ground);
+    }
+}
+
+// ---- vertical filter ------------------------------------------------------------------------------------------------------
+// The cell (floor(x / cell), floor(y / cell)), fp64 from the fp32 row, packed with each index biased by 2^31.  A row inside the
+// ranges has |x|, |y| < max_range <= 2^30 cells, so each biased half lies in [2^30, 3 * 2^30]: never NL_HASH_EMPTY.
+__device__ __forceinline__ uint64_t column_key(float fx, float fy, double cell) {
+    const int32_t cx = (int32_t)floor((double)fx / cell), cy = (int32_t)floor((double)fy / cell);
+    return ((uint64_t)((uint32_t)cx + 0x80000000u) << 32) | (uint64_t)((uint32_t)cy + 0x80000000u);
+}
+
+// Column pass: every row inside the ranges (patch >= 0) folds its z into its cell's slot.  zlo starts at ~0, zhi at 0.
+__global__ void __launch_bounds__(kThreads) k_columns(int n, const float *__restrict__ p, int stride, const int32_t *__restrict__ patch,
+                                                      double cell, uint64_t mask, uint64_t *keys, uint32_t *zlo, uint32_t *zhi) {
+    for (int i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+        if (patch[i] < 0) continue;
+        const int64_t r = (int64_t)stride * i;
+        const uint64_t s = nl_hash_insert_slot(keys, mask, column_key(p[r], p[r + 1], cell));
+        const uint32_t o = ord_of(p[r + 2]);
+        atomicMin(&zlo[s], o);
+        atomicMax(&zhi[s], o);
+    }
+}
+
+// Flag pass: vertical = the row's cell spreads over more than `height` in z (the extent of two floats in fp64 is exact).
+__global__ void __launch_bounds__(kThreads) k_vertical(int n, const float *__restrict__ p, int stride, const int32_t *__restrict__ patch,
+                                                       double cell, double height, uint64_t mask, const uint64_t *__restrict__ keys,
+                                                       const uint32_t *__restrict__ zlo, const uint32_t *__restrict__ zhi, uint8_t *vert) {
+    for (int i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+        uint8_t v = 0;
+        if (patch[i] >= 0) {
+            const int64_t r = (int64_t)stride * i;
+            const uint64_t s = nl_hash_slot_of(keys, mask, column_key(p[r], p[r + 1], cell));
+            v = (double)float_of(zhi[s]) - (double)float_of(zlo[s]) > height;
+        }
+        vert[i] = v;
     }
 }
 
@@ -395,7 +464,7 @@ __global__ void k_scatter(int n, const float *__restrict__ p, int stride, const 
     out_idx[o] = i;
 }
 
-int check_params(const char *what, const nl_ground_params *q, Geo &g, Fit &f, int &n_patches) {
+int check_params(const char *what, const nl_ground_params *q, Geo &g, Fit &f, Vert &v, int &n_patches) {
     char buf[192];
     if (!q) { std::snprintf(buf, sizeof(buf), "%s: null params", what); return nl_set_error(buf); }
     if (!(std::isfinite(q->min_range) && std::isfinite(q->max_range) && q->min_range > 0.0 && q->min_range < q->max_range)) {
@@ -424,6 +493,22 @@ int check_params(const char *what, const nl_ground_params *q, Geo &g, Fit &f, in
     for (double v : th) finite = finite && std::isfinite(v);
     for (int k = 0; k < 4; ++k) finite = finite && std::isfinite(q->elevation_thr[k]);
     if (!finite) { std::snprintf(buf, sizeof(buf), "%s: thresholds and sensor_height must be finite", what); return nl_set_error(buf); }
+    if (!(std::isfinite(q->vertical_cell) && q->vertical_cell >= 0.0)) {
+        std::snprintf(buf, sizeof(buf), "%s: vertical_cell must be finite and >= 0 (0 = off)", what);
+        return nl_set_error(buf);
+    }
+    if (q->vertical_cell > 0.0) {
+        if (!(std::isfinite(q->vertical_height) && q->vertical_height > 0.0)) {
+            std::snprintf(buf, sizeof(buf), "%s: vertical_height must be positive and finite when vertical_cell > 0", what);
+            return nl_set_error(buf);
+        }
+        if (!(q->max_range / q->vertical_cell <= kMaxCells)) {
+            std::snprintf(buf, sizeof(buf), "%s: vertical_cell too small: the cell keys need max_range / vertical_cell <= 2^30", what);
+            return nl_set_error(buf);
+        }
+    }
+    v.cell = q->vertical_cell;
+    v.height = q->vertical_height;
     const double lo = q->min_range, hi = q->max_range;
     const double e[5] = {lo, (7.0 * lo + hi) / 8.0, (3.0 * lo + hi) / 4.0, (lo + hi) / 2.0, hi};
     g.patch_off[0] = 0;
@@ -480,16 +565,41 @@ int64_t nl_ground_workspace_bytes(int64_t n) {
     return (int64_t)l.total;
 }
 
-int nl_ground_segment(int64_t n, const float *d_points, int32_t stride, const nl_ground_params *params, void *d_ws, int64_t ws_bytes,
-                      uint8_t *d_label, float *d_cos, int32_t *d_patch, nl_ground_patch *d_patches, int64_t *d_counts, void *stream) {
-    const char *what = "nl_ground_segment";
-    if (n < 0 || n > kMaxN) return nl_set_error("nl_ground_segment: n must be in [0, 2^31)");
-    if (stride != 3 && stride != 4) return nl_set_error("nl_ground_segment: stride must be 3 or 4");
+int64_t nl_ground_vertical_workspace_bytes(int64_t n) {
+    if (n < 0 || n > kMaxN) return nl_set_error("nl_ground_vertical_workspace_bytes: n must be in [0, 2^31)");
+    return 16 * column_slots(n);
+}
+
+static int ground_segment(const char *what, int64_t n, const float *d_points, int32_t stride, const nl_ground_params *params, void *d_ws,
+                          int64_t ws_bytes, void *d_vws, int64_t vws_bytes, uint8_t *d_label, float *d_cos, int32_t *d_patch,
+                          nl_ground_patch *d_patches, uint8_t *d_vertical, int64_t *d_counts, void *stream) {
+    char buf[192];
+    if (n < 0 || n > kMaxN) { std::snprintf(buf, sizeof(buf), "%s: n must be in [0, 2^31)", what); return nl_set_error(buf); }
+    if (stride != 3 && stride != 4) { std::snprintf(buf, sizeof(buf), "%s: stride must be 3 or 4", what); return nl_set_error(buf); }
     Geo g;
     Fit f;
+    Vert v;
     int n_patches = 0, rc;
-    if ((rc = check_params(what, params, g, f, n_patches)) != NL_OK) return rc;
-    if (!d_counts || (n > 0 && (!d_points || !d_label || !d_cos))) return nl_set_error("nl_ground_segment: null pointer");
+    if ((rc = check_params(what, params, g, f, v, n_patches)) != NL_OK) return rc;
+    if (!d_counts || (n > 0 && (!d_points || !d_label || !d_cos))) { std::snprintf(buf, sizeof(buf), "%s: null pointer", what); return nl_set_error(buf); }
+    const bool vertical = v.cell > 0.0;
+    const int64_t slots = column_slots(n);
+    if (vertical && n > 0) {
+        if (!d_vws || !d_vertical) {
+            std::snprintf(buf, sizeof(buf), "%s: null pointer: vertical_cell > 0 needs the vertical workspace and d_vertical "
+                          "(nl_ground_segment_vertical)", what);
+            return nl_set_error(buf);
+        }
+        if (vws_bytes < 16 * slots) {
+            std::snprintf(buf, sizeof(buf), "%s: vertical workspace of %lld bytes, nl_ground_vertical_workspace_bytes asks for %lld", what,
+                          (long long)vws_bytes, (long long)(16 * slots));
+            return nl_set_error(buf);
+        }
+        if (((uintptr_t)d_vws & 255u) != 0) {
+            std::snprintf(buf, sizeof(buf), "%s: the vertical workspace must be 256-byte aligned", what);
+            return nl_set_error(buf);
+        }
+    }
     Layout l;
     if ((rc = check_ws(what, n, d_ws, ws_bytes, l)) != NL_OK) return rc;
 
@@ -508,6 +618,19 @@ int nl_ground_segment(int64_t n, const float *d_points, int32_t stride, const nl
         k_bin<<<grid_for(n), kThreads, 0, s>>>(ni, d_points, stride, g, n_patches, key_a, val_a, patch, pcount, d_label, d_cos, d_counts);
         NL_CHECK_LAUNCH(what);
     }
+    if (vertical && ni > 0) {                                   // the column table: keys, then z min, then z max, `slots` of each
+        uint64_t *keys = at<uint64_t>(d_vws, 0);
+        uint32_t *zlo = at<uint32_t>(d_vws, 8 * slots), *zhi = at<uint32_t>(d_vws, 12 * slots);
+        if ((e = cudaMemsetAsync(keys, 0xff, 12 * slots, s)) != cudaSuccess) return cuda_fail(what, e);   // NL_HASH_EMPTY keys, zlo = ~0
+        if ((e = cudaMemsetAsync(zhi, 0, 4 * slots, s)) != cudaSuccess) return cuda_fail(what, e);
+        const uint64_t mask = (uint64_t)slots - 1;
+        k_columns<<<grid_for(n), kThreads, 0, s>>>(ni, d_points, stride, patch, v.cell, mask, keys, zlo, zhi);
+        NL_CHECK_LAUNCH(what);
+        k_vertical<<<grid_for(n), kThreads, 0, s>>>(ni, d_points, stride, patch, v.cell, v.height, mask, keys, zlo, zhi, d_vertical);
+        NL_CHECK_LAUNCH(what);
+    } else if (d_vertical && ni > 0) {
+        if ((e = cudaMemsetAsync(d_vertical, 0, n, s)) != cudaSuccess) return cuda_fail(what, e);
+    }
     size_t tb = l.tmp_bytes;
     if ((e = cub::DeviceScan::ExclusiveSum(at<void>(d_ws, l.tmp), tb, pcount, start, n_patches + 1, s)) != cudaSuccess) return cuda_fail(what, e);
     const uint32_t *idx = val_a;
@@ -516,10 +639,11 @@ int nl_ground_segment(int64_t n, const float *d_points, int32_t stride, const nl
         tb = l.tmp_bytes;
         if ((e = cub::DeviceRadixSort::SortPairs(at<void>(d_ws, l.tmp), tb, dk, dv, ni, 0, kKeyBits, s)) != cudaSuccess) return cuda_fail(what, e);
         idx = dv.Current();
-        k_gather<<<nl_div_up(n, kThreads), kThreads, 0, s>>>(ni, d_points, stride, idx, start, n_patches, pts);
+        k_gather<<<nl_div_up(n, kThreads), kThreads, 0, s>>>(ni, d_points, stride, idx, start, n_patches, vertical ? d_vertical : nullptr, pts);
         NL_CHECK_LAUNCH(what);
     }
-    k_fit<<<n_patches, kThreads, 0, s>>>(g, f, start, pts, idx, d_label, rec, d_counts);
+    if (vertical) k_fit<true><<<n_patches, kThreads, 0, s>>>(g, f, start, pts, idx, d_label, rec, d_counts);
+    else k_fit<false><<<n_patches, kThreads, 0, s>>>(g, f, start, pts, idx, d_label, rec, d_counts);
     NL_CHECK_LAUNCH(what);
     if (ni > 0) {
         static NlPerDevice opt_in;
@@ -529,6 +653,19 @@ int nl_ground_segment(int64_t n, const float *d_points, int32_t stride, const nl
         NL_CHECK_LAUNCH(what);
     }
     return NL_OK;
+}
+
+int nl_ground_segment(int64_t n, const float *d_points, int32_t stride, const nl_ground_params *params, void *d_ws, int64_t ws_bytes,
+                      uint8_t *d_label, float *d_cos, int32_t *d_patch, nl_ground_patch *d_patches, int64_t *d_counts, void *stream) {
+    return ground_segment("nl_ground_segment", n, d_points, stride, params, d_ws, ws_bytes, nullptr, 0, d_label, d_cos, d_patch, d_patches,
+                          nullptr, d_counts, stream);
+}
+
+int nl_ground_segment_vertical(int64_t n, const float *d_points, int32_t stride, const nl_ground_params *params, void *d_ws, int64_t ws_bytes,
+                               void *d_vws, int64_t vws_bytes, uint8_t *d_label, float *d_cos, int32_t *d_patch, nl_ground_patch *d_patches,
+                               uint8_t *d_vertical, int64_t *d_counts, void *stream) {
+    return ground_segment("nl_ground_segment_vertical", n, d_points, stride, params, d_ws, ws_bytes, d_vws, vws_bytes, d_label, d_cos, d_patch,
+                          d_patches, d_vertical, d_counts, stream);
 }
 
 int nl_ground_partition(int64_t n, const float *d_points, int32_t stride, const uint8_t *d_label, const float *d_cos, void *d_ws, int64_t ws_bytes,

@@ -1,5 +1,5 @@
-// Open-addressing hash sets of 64-bit keys with linear probing, shared by eval.cu (cell table of the nearest-neighbour search)
-// and overlap.cu (voxel sets of the keyframe overlap).  A slot holds NL_HASH_EMPTY until one atomicCAS claims it, and is never
+// Open-addressing hash sets of 64-bit keys with linear probing, shared by eval.cu (cell table of the nearest-neighbour search),
+// overlap.cu (voxel sets of the keyframe overlap) and ground.cu (column table of the vertical filter).  A slot holds NL_HASH_EMPTY until one atomicCAS claims it, and is never
 // written again, so a plain load that sees a key sees it for good; a stale "empty" is resolved by the CAS.  The caller keeps the
 // capacity a power of two and the load factor below 1 (both users stay at or below 1/2), and never stores NL_HASH_EMPTY as a key.
 #pragma once
@@ -23,6 +23,24 @@ __device__ __forceinline__ bool nl_hash_insert(uint64_t *slots, uint64_t mask, u
         if (prev == NL_HASH_EMPTY) return true;
         if (prev == k) return false;
     }
+}
+
+// Adds k to the set if absent and returns its slot, for callers that keep values beside the keys (ground.cu's column extents).
+__device__ __forceinline__ uint64_t nl_hash_insert_slot(uint64_t *slots, uint64_t mask, uint64_t k) {
+    for (uint64_t s = nl_hash_mix(k) & mask;; s = (s + 1) & mask) {
+        const uint64_t h = slots[s];
+        if (h == k) return s;
+        if (h != NL_HASH_EMPTY) continue;
+        const unsigned long long prev = atomicCAS((unsigned long long *)&slots[s], (unsigned long long)NL_HASH_EMPTY, (unsigned long long)k);
+        if (prev == NL_HASH_EMPTY || prev == k) return s;
+    }
+}
+
+// The slot of k, which must be in the set.
+__device__ __forceinline__ uint64_t nl_hash_slot_of(const uint64_t *__restrict__ slots, uint64_t mask, uint64_t k) {
+    uint64_t s = nl_hash_mix(k) & mask;
+    while (slots[s] != k) s = (s + 1) & mask;
+    return s;
 }
 
 __device__ __forceinline__ bool nl_hash_contains(const uint64_t *__restrict__ slots, uint64_t mask, uint64_t k) {

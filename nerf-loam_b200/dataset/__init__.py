@@ -1,6 +1,7 @@
 """The reference's scan loaders (src/dataset/kitti.py, maicity.py) with the ground segmentation on the GPU (ground.py) in place of
 the external Patchwork++ library.  `dataset.kitti.DataLoader` and `dataset.maicity.DataLoader` keep the reference's constructor and
 methods; __getitem__ returns (index, points f32[N,3], pointcos f32[N], pose 4x4 or None) with CPU tensors, the ground points first.
+The keyword `ground_params` (a ground.GroundParams, e.g. with the vertical filter on) sets the segmentation; None keeps its defaults.
 
 The reference imports them as `import_module("dataset." + name)` (src/utils/import_util.py:4-6), so the seam is one line:
 
@@ -24,8 +25,9 @@ class ScanLoader(Dataset):
     pose_file = None
     remove_abnormal_z = False   # drop rows with z <= -3.0 before the depth gates
 
-    def __init__(self, data_path, use_gt=False, max_depth=-1, min_depth=-1):
+    def __init__(self, data_path, use_gt=False, max_depth=-1, min_depth=-1, ground_params=None):
         self.data_path = data_path
+        self.ground_params = ground_params
         self.num_bin = len(glob(osp.join(self.data_path, "velodyne/*.bin")))
         self.use_gt = use_gt
         self.max_depth = max_depth
@@ -60,7 +62,7 @@ class ScanLoader(Dataset):
     def load_points(self, index):
         """(points f32[N,3], pointcos f32[N]) as numpy: the ground points first, then the rest, each half in scan order."""
         import nerfloam_b200
-        points, pointcos, _ = nerfloam_b200.ground.points_and_cos(self.read_points(index))
+        points, pointcos, _ = nerfloam_b200.ground.points_and_cos(self.read_points(index), self.ground_params)
         return points.cpu().numpy(), pointcos.cpu().numpy()
 
     def __len__(self):

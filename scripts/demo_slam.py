@@ -15,7 +15,8 @@ drives out along +x and back over the same ground (fresh noise seeds), so the la
 `--data DIR --dataset kitti|maicity` runs the same loop on a recorded sequence through dataset.<name>.DataLoader (points and pointsCos
 from the GPU ground segmentation, ground.py): the first scan takes the loader's get_init_pose, every later one is tracked; the
 trajectory error is reported against the pose file when it exists, and the `reconstruction` block (synthetic scans only) is left out.
-`--scans` then caps the number of scans (default: all).
+`--scans` then caps the number of scans (default: all).  `--vertical-cell W` (with --data) turns on the ground segmentation's
+vertical-structure filter with W-metre columns (GroundParams.vertical_cell; 0, the default, leaves it off).
 """
 import argparse, json, os, sys, time
 from types import SimpleNamespace
@@ -31,7 +32,8 @@ def load_sequence(a):
     import importlib
     loader = importlib.import_module("nerf-loam_b200.dataset." + a.dataset).DataLoader
     has_poses = os.path.exists(os.path.join(a.data, loader.pose_file))
-    data = loader(a.data, use_gt=has_poses)
+    gp = nl.ground.GroundParams(vertical_cell=a.vertical_cell) if a.vertical_cell > 0 else None
+    data = loader(a.data, use_gt=has_poses, ground_params=gp)
     a.scans = len(data) if a.scans is None else min(a.scans, len(data))
     if a.scans < 2:
         raise SystemExit(f"{a.data}: need at least 2 scans, found {len(data)}")
@@ -65,7 +67,11 @@ def main():
     ap.add_argument("--path", default="line", choices=["line", "loop"], help="line: out along +x; loop: out and back over the same ground")
     ap.add_argument("--data", default=None, help="a KITTI- or MaiCity-layout sequence directory instead of synthetic scans")
     ap.add_argument("--dataset", default="kitti", choices=["kitti", "maicity"], help="layout of --data")
+    ap.add_argument("--vertical-cell", type=float, default=0.0,
+                    help="with --data: column width (m) of the ground segmentation's vertical-structure filter; 0 = off")
     a = ap.parse_args()
+    if a.vertical_cell != 0.0 and a.data is None:
+        ap.error("--vertical-cell applies to --data")
     dev = torch.device("cuda"); syn, rh = nl.synthetic, nl.render_helpers
     vs, md, trunc = 0.3, 40.0, 0.3
     crit = nl.criterion.Criterion(SimpleNamespace(criteria={"eiko_weight": 0.1, "sdf_weight": 10000.0, "fs_weight": 1.0, "sdf_truncation": trunc},
@@ -141,6 +147,7 @@ def main():
     t_mesh = (tick() - t0) * 1e3
     if a.data is not None:
         out = {"data": a.data, "dataset": a.dataset, "scans": a.scans, "octree": a.octree, "selection": a.selection,
+               **({"vertical_cell": a.vertical_cell} if a.vertical_cell > 0 else {}),
                "last_window_scans": [f.index for f in window], "ground_points": [int((s[1] < 1).sum()) for s in scans],
                "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0,
                "init_mapping_ms": t_init, "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
