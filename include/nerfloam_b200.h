@@ -685,6 +685,47 @@ NL_API int nl_ground_segment_vertical(int64_t n, const float *d_points, int32_t 
 NL_API int nl_ground_partition(int64_t n, const float *d_points, int32_t stride, const uint8_t *d_label, const float *d_cos, void *d_ws,
                                int64_t ws_bytes, float *d_out_points, float *d_out_cos, int32_t *d_out_index, void *stream);
 
+/* ============================================================================================
+ * 14. Key-scan map refinement (the mapper's final_iter pass, src/mapping.py:154-164): P passes of `iters` iterations, each pass one
+ *     bundle_adjust_frames over a random window of keyframes with poses and decoder frozen and a fresh Adam on the embedding table
+ *     (render_helpers.py:341-353).  csrc/refine.cu; render_helpers.refine_map captures one iteration and replays it P x iters times.
+ *     A fresh Adam makes a row-sparse step exact: a row no sample has reached since the pass began has g = m = v = 0, and the bf16
+ *     update leaves it bitwise unchanged, so Adam over the rows touched so far in the pass gives the dense step's table.
+ *     State d_state int32[NL_REFINE_STATE_WORDS], zeroed before the first pass: */
+#define NL_REFINE_ITER 0         /* iterations completed in the call; pass = ITER / iters                                       */
+#define NL_REFINE_LISTED 1       /* rows listed so far in the current pass (length of the row list)                              */
+#define NL_REFINE_PREV 2         /* rows the previous pass listed (still in the row list until the next pass's first nl_mark_rows) */
+#define NL_REFINE_STATE_WORDS 4
+/* Pass boundary, first launch of an iteration.  A no-op unless ITER % iters == 0; then, for pass p = ITER / iters < n_passes:
+ * scans d_windows[p][0..n_frames) (keyframe indices) are copied into the selection buffers d_dirs f32[n_frames,cap,3], d_gt, d_cos
+ * f32[n_frames,cap] and d_n_points i64[n_frames] from the keyframe table (d_kf_arrays i64[K][3] = device addresses of each keyframe's
+ * dirs f32[n,3], cos f32[n], range f32[n]; d_kf_points i64[K] = n <= cap), their poses from d_kf_pose6 f32[K,6] into d_pose6;
+ * *d_sel_seed = d_sel_seeds[p], *d_noise_seed = d_noise_seeds[p] (both may be NULL: deterministic sampling); d_ctl[NL_CTL_ADAM_STEP]
+ * = 0 (a fresh optimiser); and the moments d_m / d_v (bf16 [n_rows,16]) and the flag bits of the PREV rows of d_rows are zeroed.
+ * Replaces the per-call set-up of bundle_adjust_frames (render_helpers.py:341-353: a new optimiser per call) and the upload of its
+ * frames and seeds (render_helpers.py:356-391), once per pass. */
+NL_API int nl_refine_pass_begin(int n_frames, int64_t cap, int n_keyframes, int iters, int n_passes, const int32_t *d_state,
+                                const int32_t *d_windows, const int64_t *d_kf_arrays, const int64_t *d_kf_points, const float *d_kf_pose6,
+                                const int32_t *d_sel_seeds, const int32_t *d_noise_seeds, float *d_dirs, float *d_gt, float *d_cos,
+                                int64_t *d_n_points, float *d_pose6, int32_t *d_sel_seed, int32_t *d_noise_seed, int32_t *d_ctl,
+                                int64_t n_rows, const int32_t *d_rows, uint32_t *d_row_bits, uint16_t *d_m, uint16_t *d_v, void *stream);
+/* Flag the embedding rows that nl_gather_trilinear_bwd scatters into (render_helpers.py:60-93, the backward of the trilinear
+ * gather): for the first min(*d_M, M) samples, the rows d_vox2row[d_vox[i]][0..8) that are >= 0.  A row whose bit in d_row_bits
+ * (u32[ceil(n_rows / 32)]) was clear is set and appended to d_rows at d_state[NL_REFINE_LISTED] (each row once; order unspecified). */
+NL_API int nl_mark_rows(int64_t M, const int32_t *d_M, const int32_t *d_vox, const int32_t *d_vox2row, int64_t n_rows, uint32_t *d_row_bits,
+                        int32_t *d_rows, int32_t *d_state, void *stream);
+/* nl_adam_bf16_ctl (optim.step() on the embedding table, render_helpers.py:421-423) over the first min(*d_n_listed, n_rows) rows of d_rows
+ * only, 16 elements per row, with the same arithmetic; step count and skip flag from d_ctl.  Every listed row's gradient is cleared
+ * after it is read, on a skipped iteration too (its scatter may have run). */
+NL_API int nl_adam_bf16_rows_ctl(int64_t n_rows, const int32_t *d_rows, const int32_t *d_n_listed, uint16_t *d_param, float *d_grad_f32,
+                                 uint16_t *d_m, uint16_t *d_v, double lr, double beta1, double beta2, double eps, const int32_t *d_ctl,
+                                 void *stream);
+/* Last launch of an iteration: *d_sel_seed += sel_inc and *d_noise_seed += noise_inc (wrapping; either may be NULL), as the captured
+ * mapping iteration advances its seeds (the next iteration's frame.sample_rays and sampler noise, render_helpers.py:365-391);
+ * ITER += 1, and at the end of a pass PREV = LISTED, LISTED = 0. */
+NL_API int nl_refine_iter_end(int iters, int32_t *d_state, int32_t *d_sel_seed, int32_t sel_inc, int32_t *d_noise_seed, int32_t noise_inc,
+                              void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,6 +12,7 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     frame.LidarFrame                <- src/lidarFrame.py
     render_helpers.render_rays / bundle_adjust_frames / track_frame / get_scores  <- src/variations/render_helpers.py
     track_frames (= render_helpers.track_frames, track_batch)  K independent track_frame problems in one launch chain
+    refine_map (= render_helpers.refine_map)  the mapper's key-scan refinement (mapper_specs.final_iter, src/mapping.py:154-164)
     score_poses / relocalise (= render_helpers.*, score)  the loss of up to 65 535 pose hypotheses of one scan; recovering a lost scan
     mapping.MapUpdater              <- Mapping.create_voxels / update_grid_features / get_embeddings (src/mapping.py)
     mesh.extract_mesh / marching_cubes  <- MeshExtractor.create_mesh / marching_cubes (src/utils/mesh_util.py)
@@ -27,13 +28,15 @@ no CPU or eager-PyTorch fallback for the kernels.
 from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
-           "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise"]
+           "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise", "refine_map"]
 
 
 def __getattr__(name):
     import importlib
     if name == "track_frames":
         return importlib.import_module(".track_batch", __name__).track_frames
+    if name == "refine_map":
+        return importlib.import_module(".render_helpers", __name__).refine_map
     if name in ("score_poses", "relocalise"):
         return getattr(importlib.import_module(".score", __name__), name)
     if name in __all__:

@@ -185,6 +185,11 @@ _SIGNATURES = {
     "nl_ground_segment_vertical": (C.c_int, [C.c_int64, vp, C.c_int32, C.POINTER(GroundParams), vp, C.c_int64, vp, C.c_int64, vp, vp, vp, vp,
                                              vp, vp, vp]),
     "nl_ground_partition": (C.c_int, [C.c_int64, vp, C.c_int32, vp, vp, vp, C.c_int64, vp, vp, vp, vp]),
+    # key-scan map refinement (include/nerfloam_b200.h section 14)
+    "nl_refine_pass_begin": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int] + [vp] * 15 + [C.c_int64] + [vp] * 5),
+    "nl_mark_rows": (C.c_int, [C.c_int64, vp, vp, vp, C.c_int64, vp, vp, vp, vp]),
+    "nl_adam_bf16_rows_ctl": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),
+    "nl_refine_iter_end": (C.c_int, [C.c_int, vp, vp, C.c_int32, vp, C.c_int32, vp]),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)
@@ -195,6 +200,8 @@ SCORE_MAX_PROBLEMS = 65535   # NL_SCORE_MAX_PROBLEMS
 EVAL_KEY_BITS = 21           # NL_EVAL_KEY_BITS
 EVAL_TILE = 2048             # NL_EVAL_TILE
 GROUND_MAX_PATCHES = 1024    # NL_GROUND_MAX_PATCHES
+# words of the refinement state block (include/nerfloam_b200.h section 14)
+REFINE_ITER, REFINE_LISTED, REFINE_PREV, REFINE_STATE_WORDS = 0, 1, 2, 4
 STATS_PACK_FIXED = 10
 # node-array checks, bit i = 1 << i (NL_TREE_* in include/nerfloam_b200.h section 1)
 TREE_CHECKS = ("ROOT", "RANGE", "LINK", "PARENTS", "SHAPE", "ROWS", "VERTICES")

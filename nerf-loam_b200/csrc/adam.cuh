@@ -21,3 +21,20 @@ __device__ __forceinline__ void nl_adam_f32_elem(const NlAdamConst &c, float gi,
     m = mi;
     v = vi;
 }
+// The same on the bf16 embedding table (optim.cu's nl_adam_bf16_ctl, refine.cu's row-list step): parameter and moments are bf16,
+// every operation rounds its result to bf16, and the fp32 gradient sum is rounded first.  With g = m = v = 0 it leaves p bitwise
+// unchanged (m = v = +0, and p + (-step_size) * (+0 / d) = p, also for p = -0).
+__device__ __forceinline__ void nl_adam_bf16_elem(const NlAdamConst &c, float g32, uint16_t &p, uint16_t &m, uint16_t &v) {
+    const float gi = nl_round_bf16(g32);
+    float mi = nl_bf16_to_f32(m), vi = nl_bf16_to_f32(v), pi = nl_bf16_to_f32(p);
+    mi = nl_round_bf16(__fadd_rn(mi, __fmul_rn(c.w1, __fsub_rn(gi, mi))));
+    vi = nl_round_bf16(__fmul_rn(vi, c.b2));
+    vi = nl_round_bf16(__fadd_rn(vi, __fmul_rn(__fmul_rn(c.w2, gi), gi)));
+    float d = nl_round_bf16(__fsqrt_rn(vi));
+    d = nl_round_bf16(__fdiv_rn(d, c.bc2_sqrt));
+    d = nl_round_bf16(__fadd_rn(d, c.eps));
+    pi = nl_round_bf16(__fadd_rn(pi, __fmul_rn(-c.step_size, __fdiv_rn(mi, d))));
+    p = nl_f32_to_bf16(pi);
+    m = nl_f32_to_bf16(mi);
+    v = nl_f32_to_bf16(vi);
+}

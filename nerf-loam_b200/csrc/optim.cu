@@ -78,18 +78,7 @@ __global__ void k_adam_ctl(long long n, void *__restrict__ p_, const float *__re
     const float w1 = (float)(1.0 - beta1), b2 = (float)beta2, w2 = (float)(1.0 - beta2), step_size = (float)(lr / bc1), bc2_sqrt = (float)sqrt(bc2);
     if (BF16) {
         uint16_t *p = (uint16_t *)p_, *m = (uint16_t *)m_, *v = (uint16_t *)v_;
-        const float gi = nl_round_bf16(g[i]);
-        float mi = nl_bf16_to_f32(m[i]), vi = nl_bf16_to_f32(v[i]), pi = nl_bf16_to_f32(p[i]);
-        mi = nl_round_bf16(__fadd_rn(mi, __fmul_rn(w1, __fsub_rn(gi, mi))));
-        vi = nl_round_bf16(__fmul_rn(vi, b2));
-        vi = nl_round_bf16(__fadd_rn(vi, __fmul_rn(__fmul_rn(w2, gi), gi)));
-        float d = nl_round_bf16(__fsqrt_rn(vi));
-        d = nl_round_bf16(__fdiv_rn(d, bc2_sqrt));
-        d = nl_round_bf16(__fadd_rn(d, eps));
-        pi = nl_round_bf16(__fadd_rn(pi, __fmul_rn(-step_size, __fdiv_rn(mi, d))));
-        p[i] = nl_f32_to_bf16(pi);
-        m[i] = nl_f32_to_bf16(mi);
-        v[i] = nl_f32_to_bf16(vi);
+        nl_adam_bf16_elem(NlAdamConst{w1, b2, w2, eps, step_size, bc2_sqrt}, g[i], p[i], m[i], v[i]);
     } else {
         float *p = (float *)p_, *m = (float *)m_, *v = (float *)v_;
         nl_adam_f32_elem(NlAdamConst{w1, b2, w2, eps, step_size, bc2_sqrt}, g[i], p[i], m[i], v[i]);

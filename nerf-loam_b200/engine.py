@@ -474,14 +474,16 @@ class SDFEngine:
     def forward_backward(self, m, dec, R, cfg, gt_depth, cos, dir_local=None, ray_frame=None, n_frames=1, ray_o=None,
                          ray_d=None, noise=None, rng_seed=0, reference_compat=True, update_decoder=True, update_emb=True,
                          update_pose=True, pose6=None, group=None, refresh_weights=True, rng_seed_dev=None, defer_wgrad=False, peer=None,
-                         peer_stats=None, pose_step=None):
+                         peer_stats=None, pose_step=None, zero_grads=True):
         """One optimisation iteration without the optimiser step.  Gradients land in
         self.grad_emb (fp32 [V,16]), dec.grads (fp32), self.pose_grad (fp32 [F,6]); the loss in stats.
         defer_wgrad=True: return without waiting for the decoder's weight gradients -- they (and whatever the caller enqueues on
         side_stream(), i.e. the decoder's optimiser step) are joined right before the next iteration's decoder, or by join_side().
         pose_step: dict(mask, m, v, lr, seeds=[(int32 tensor, increment), ...]) -- the pose gradient, the poses' Adam step (rows in
         `mask`, moments m / v f32[F,6]), the loss read-out and the advance of the listed device-side seeds as ONE launch
-        (nl_pose_step) instead of nl_pose_grad + nl_loss_finalize + one Adam launch per pose + one add per seed."""
+        (nl_pose_step) instead of nl_pose_grad + nl_loss_finalize + one Adam launch per pose + one add per seed.
+        zero_grads=False: skip the zero-fill of the gradient table (self.gradflat); the caller clears the rows it used (refine_map's
+        row-list Adam, nl_adam_bf16_rows_ctl), so the scatter finds zeros without a pass over the whole table."""
         lib = _capi.lib()
         st = _capi.stream_ptr()
         self._vs = cfg["voxel_size"]
@@ -518,7 +520,7 @@ class SDFEngine:
         self._mark("t_mlp")
         want_pose = update_pose and dir_local is not None
         if update_emb or want_pose:
-            if not self._ensure_grads(m.emb.shape[0] if update_emb else 0, n_frames):
+            if not self._ensure_grads(m.emb.shape[0] if update_emb else 0, n_frames) and zero_grads:
                 self.gradflat.zero_()
         if update_emb or want_pose:
             _capi.check(lib.nl_gather_trilinear_bwd(

@@ -600,6 +600,210 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
                 f.pose.data.copy_(host[i].to(f.pose.data.device))
 
 
+def refine_schedule(keyframe_graph, passes, deterministic=False, device="cuda"):
+    """What the mapper's final_iter loop (mapping.py:154-164) draws, drawn up front in the loop's order: per pass the window
+    (KeyframeGraph.select_optimize_targets(None, 'random'), as indices into keyframe_graph.keyframe_graph in window order), the sampler
+    noise seed (torch's CPU generator, 0 when deterministic) and the ray-selection seed (torch's generator on `device`: an int32[1]
+    tensor there).  Returns (windows, noise_seeds, selection_seeds)."""
+    index = {id(f): i for i, f in enumerate(keyframe_graph.keyframe_graph)}
+    windows, noise, sel = [], [], []
+    for _ in range(passes):
+        windows.append([index[id(f)] for f in keyframe_graph.select_optimize_targets(None, "random")])
+        noise.append(0 if deterministic else _seed_from_torch())
+        sel.append(_seed_from_cuda(device))
+    return windows, noise, sel
+
+
+class _RefineGraph:
+    """One captured refinement iteration: pass boundary (nl_refine_pass_begin) -> ray selection -> rays -> samples -> gather -> decoder
+    forward/backward -> embedding scatter -> row marking (nl_mark_rows) -> Adam over the listed rows (nl_adam_bf16_rows_ctl) -> seed and
+    counter advance (nl_refine_iter_end).  Poses and decoder are frozen, so only the table moves.  Every per-call input (windows,
+    keyframe table, seeds) sits in static device buffers; a call is passes x num_iterations replays and ONE read-back."""
+
+    _cache = {}
+
+    def __init__(self, key, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, cap, spr, K, P, iters):
+        dev = emb.device
+        R = F * N_rays
+        V = emb.shape[0]
+        eng = SDFEngine(R, R * spr, dev)            # private: captured pointers must stay valid
+        bufs = DecoderBuffers(sdf_network, dev)
+        m = m.replace(emb=emb)
+        self.key, self.eng, self.bufs, self.m, self.emb, self.F, self.K, self.P = key, eng, bufs, m, emb, F, K, P
+        self.packed = m.packed_children()
+        self.dirs = torch.zeros((F, cap, 3), device=dev)
+        self.gt = torch.zeros((F, cap), device=dev)
+        self.cos = torch.zeros((F, cap), device=dev)
+        self.n_dev = torch.zeros((F, 1), dtype=torch.int64, device=dev)
+        self.sel_seed = torch.ones(1, dtype=torch.int32, device=dev)
+        self.seed_dev = None if deterministic else torch.zeros(1, dtype=torch.int32, device=dev)
+        self.sel_out = (torch.empty((R, 3), device=dev), torch.empty(R, device=dev), torch.empty(R, device=dev))
+        self.fid = torch.arange(F, dtype=torch.int32, device=dev).repeat_interleave(N_rays).contiguous()
+        self.pose6 = torch.zeros((F, 6), device=dev)
+        # per-call inputs
+        self.windows = torch.zeros((P, F), dtype=torch.int32, device=dev)
+        self.sel_seeds = torch.ones(P, dtype=torch.int32, device=dev)
+        self.noise_seeds = None if deterministic else torch.zeros(P, dtype=torch.int32, device=dev)
+        self.kf_arrays = torch.zeros((K, 3), dtype=torch.int64, device=dev)
+        self.kf_points = torch.zeros(K, dtype=torch.int64, device=dev)
+        self.kf_pose6 = torch.zeros((K, 6), device=dev)
+        # row list and a fresh optimiser's moments; zero outside the rows a pass lists (nl_refine_pass_begin clears those)
+        self.state = torch.zeros(_capi.REFINE_STATE_WORDS, dtype=torch.int32, device=dev)
+        self.rows = torch.zeros(V, dtype=torch.int32, device=dev)
+        self.row_bits = torch.zeros((V + 31) // 32, dtype=torch.int32, device=dev)
+        self.adam_m, self.adam_v = torch.zeros_like(emb), torch.zeros_like(emb)
+        self.iters, self.lr, self.V, self.cap = iters, float(lr), V, cap
+        self.graph = None
+        self.launches_per_iter = 0
+
+        def body():
+            lib, st = _capi.lib(), _capi.stream_ptr()
+            _capi.check(lib.nl_refine_pass_begin(F, cap, K, iters, P, _capi.ptr(self.state), _capi.ptr(self.windows), _capi.ptr(self.kf_arrays),
+                                                 _capi.ptr(self.kf_points), _capi.ptr(self.kf_pose6), _capi.ptr(self.sel_seeds),
+                                                 _capi.ptr(self.noise_seeds), _capi.ptr(self.dirs), _capi.ptr(self.gt), _capi.ptr(self.cos),
+                                                 _capi.ptr(self.n_dev), _capi.ptr(self.pose6), _capi.ptr(self.sel_seed), _capi.ptr(self.seed_dev),
+                                                 _capi.ptr(eng.ctl), V, _capi.ptr(self.rows), _capi.ptr(self.row_bits), _capi.ptr(self.adam_m),
+                                                 _capi.ptr(self.adam_v), st), "nl_refine_pass_begin")
+            _capi.LAUNCHES += 1
+            dirs, gt, cos = select_rays_device(self.dirs, self.gt, self.cos, N_rays, n_dev=self.n_dev, seed=self.sel_seed, out=self.sel_out)
+            eng.rays_from_poses(self.pose6, dirs, self.fid)
+            eng.forward_backward(m, bufs, R, cfg, gt, cos, dir_local=dirs, ray_frame=self.fid, n_frames=F, update_decoder=False,
+                                 update_emb=True, update_pose=False, pose6=self.pose6, refresh_weights=False, rng_seed_dev=self.seed_dev,
+                                 zero_grads=False)
+            _capi.check(lib.nl_mark_rows(eng.max_samples, eng.n_samples_dev, _capi.ptr(eng.s_vox), _capi.ptr(m.vox2row), V,
+                                         _capi.ptr(self.row_bits), _capi.ptr(self.rows), _capi.ptr(self.state), st), "nl_mark_rows")
+            _capi.check(lib.nl_adam_bf16_rows_ctl(V, _capi.ptr(self.rows), _capi.ptr(self.state[_capi.REFINE_LISTED:]), _capi.ptr(emb),
+                                                  _capi.ptr(eng.grad_emb), _capi.ptr(self.adam_m), _capi.ptr(self.adam_v), self.lr, 0.9, 0.999,
+                                                  1e-8, _capi.ptr(eng.ctl), st), "nl_adam_bf16_rows_ctl")
+            _capi.check(lib.nl_refine_iter_end(iters, _capi.ptr(self.state), _capi.ptr(self.sel_seed), 0x632BE5, _capi.ptr(self.seed_dev),
+                                               0x3779B1, st), "nl_refine_iter_end")    # the increments of _MapGraph's iteration
+            _capi.LAUNCHES += 3
+        self.body = body
+
+    def _capture(self):
+        """One throw-away eager iteration on a side stream (allocations, one-time kernel attributes) on the call's inputs, then the
+        capture; what the throw-away iteration changed (table rows, moments, row list) is put back."""
+        dev = self.emb.device
+        keep = self.emb.clone()
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            self.eng.begin_call()
+            self.body()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        l0 = _capi.LAUNCHES
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self.body()
+        self.launches_per_iter = _capi.LAUNCHES - l0 + 1
+        with torch.no_grad():
+            self.emb.copy_(keep)
+        for t in (self.adam_m, self.adam_v, self.row_bits, self.state, self.eng.grad_emb):
+            t.zero_()
+
+    @classmethod
+    def get(cls, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, n_points, spr, K, P, iters):
+        cap = max(1 << 17, 1 << (int(n_points) - 1).bit_length())
+        key = (F, N_rays, float(lr), bool(deterministic), cap, int(spr), K, P, iters, m.centres.data_ptr(), m.structure.data_ptr(),
+               m.vox2row.data_ptr(), m.packed_children().data_ptr(), emb.data_ptr(), -1 if m.stable else m.n_nodes, int(emb.shape[0]),
+               tuple(p.data_ptr() for p in _decoder_params(sdf_network)), tuple(sorted(cfg.items())))
+        g = cls._cache.get("g")
+        if g is None or g.key != key:
+            cls._cache = {}
+            g = cls(key, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, cap, spr, K, P, iters)
+            cls._cache = {"g": g}
+        return g
+
+    def run(self, arrays, counts, pose6, windows, noise_seeds, sel_seeds):
+        """arrays: per keyframe (dirs, cos, range) device tensors (_frame_arrays); counts, pose6, windows, noise_seeds: host lists;
+        sel_seeds: int32[P] device tensor."""
+        dev = self.emb.device
+        self.kf_arrays.copy_(torch.tensor([[a.data_ptr() for a in arr] for arr in arrays], dtype=torch.int64))
+        self.kf_points.copy_(torch.tensor(counts, dtype=torch.int64))
+        self.kf_pose6.copy_(pose6)
+        self.windows.copy_(torch.tensor(windows, dtype=torch.int32))
+        if self.noise_seeds is not None:
+            self.noise_seeds.copy_(torch.tensor(noise_seeds, dtype=torch.int64).to(torch.int32))
+        self.sel_seeds.copy_(sel_seeds)
+        self.bufs.refresh_transposes()        # the decoder is frozen for the whole call: its kernel-side images once
+        if self.graph is None:
+            self._capture()
+        self.state[_capi.REFINE_ITER].zero_()  # PREV is kept: the first pass clears the rows of the previous call's last pass
+        self.eng.begin_call()
+        for _ in range(self.P * self.iters):
+            self.graph.replay()
+        _capi.LAUNCHES += self.launches_per_iter * self.P * self.iters
+        return self.eng.read_ctl()
+
+
+def refine_map(keyframe_graph, embeddings, map_states, sdf_network, loss_criteria, voxel_size, step_size, N_rays=512, num_iterations=10,
+               truncation=0.1, max_voxel_hit=10, max_distance=10, learning_rate=1e-2, passes=None, deterministic=False):
+    """The mapper's key-scan refinement (`mapper_specs.final_iter`, mapping.py:154-164): `passes` (default len(keyframe_graph) + 1)
+    bundle adjustments of a random window of keyframes with poses and decoder frozen, each with a fresh Adam on the embedding table,
+    i.e. under the same random.seed / torch.manual_seed what
+
+        for _ in range(passes):
+            bundle_adjust_frames(keyframe_graph.select_optimize_targets(None, "random"), embeddings, map_states, sdf_network,
+                                 loss_criteria, voxel_size, step_size, N_rays, num_iterations, ..., learning_rate=[learning_rate, *],
+                                 update_pose=False, update_decoder=False, deterministic=deterministic)
+
+    computes (same windows, rays and sampler noise; the table may differ by the fp32 scatter atomics' summation order).  N_rays is rays
+    per keyframe per iteration (the reference passes 2 x N_rays_each).  Mutates `embeddings` in place and returns None.
+
+    Everything the loop draws is drawn up front (refine_schedule) and uploaded once; one captured iteration (_RefineGraph) is replayed
+    passes x num_iterations times, and Adam steps only the rows the pass has reached, which is exact because the optimiser is fresh in
+    every pass (include/nerfloam_b200.h section 14).  The control block is read once at the end; a call that exceeded the sample
+    capacity is undone and redone with room for its largest iteration."""
+    frames = list(keyframe_graph.keyframe_graph)
+    K = len(frames)
+    if K == 0:
+        raise ValueError("refine_map: the keyframe graph is empty")
+    P = K + 1 if passes is None else int(passes)
+    if int(N_rays) < 1 or int(num_iterations) < 0 or P < 0:
+        raise ValueError("refine_map: N_rays must be >= 1, num_iterations and passes >= 0")
+    small = [f.index for f in frames if f.points.shape[0] < N_rays]
+    if small:
+        raise ValueError(f"refine_map: keyframes {small} have fewer than N_rays = {N_rays} points")
+    emb = embeddings.detach()
+    if not emb.is_cuda:
+        raise ValueError("refine_map: the embedding table must be a CUDA tensor (no CPU fallback)")
+    if not (emb.dtype == torch.bfloat16 and emb.is_contiguous()):
+        raise ValueError("refine_map: embeddings must be a contiguous bf16 CUDA tensor (mapping.py:305-314)")
+    dev = emb.device
+    windows, noise, sel = refine_schedule(keyframe_graph, P, deterministic, dev)
+    if P == 0 or num_iterations == 0:
+        return None
+    m = map_states if isinstance(map_states, MapState) else MapState.from_map_states(map_states, dev)
+    m.emb = emb
+    if m.stable and m.emb_full is not None and emb.data_ptr() == m.emb_full.data_ptr():
+        emb = m.emb_full                 # a MapUpdater map: optimised at its full capacity, like bundle_adjust_frames' graph
+    cfg = _cfg(step_size, voxel_size, max_distance, loss_criteria)
+    F = len(windows[0])
+    R = F * N_rays
+    arrays = [_frame_arrays(f, dev) for f in frames]
+    counts = [int(a[0].shape[0]) for a in arrays]
+    pose6 = torch.stack([f.pose.data.detach().float().reshape(6).cpu() for f in frames]).to(dev)
+    sel_seeds = torch.cat(sel)
+    cap = R * SAMPLES_PER_RAY_MAP
+    snap = None
+    while True:
+        if snap is None:
+            snap = emb.clone()
+        g = _RefineGraph.get(m, emb, sdf_network, cfg, F, N_rays, learning_rate, deterministic, max(counts), -(-cap // R), K, P,
+                             int(num_iterations))
+        ctl = g.run(arrays, counts, pose6, windows, noise, sel_seeds)
+        _check_ctl(ctl, "refine_map")
+        if not (ctl[_capi.CTL_ERROR] & 2):
+            break
+        # sample capacity exceeded somewhere in the call: undo it and redo it with room for the largest iteration seen
+        with torch.no_grad():
+            emb.copy_(snap)
+        cap = _grown_capacity(cap, ctl, "refine_map")
+    for _ in range(ctl[_capi.CTL_SKIPPED]):
+        print("Encouter a bug while Mapping, currently not be fixed, Continue!!")  # render_helpers.py:407-409 (the step was skipped)
+    return None
+
+
 class _TrackGraph:
     """One captured tracking iteration (ray selection -> rays -> traversal -> sampling -> gather -> decoder fwd/bwd -> pose gradient
     -> Adam) with every per-scan input in static device buffers, so that the capture (tens of ms) is paid once per map / decoder

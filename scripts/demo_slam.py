@@ -17,6 +17,11 @@ from the GPU ground segmentation, ground.py): the first scan takes the loader's 
 trajectory error is reported against the pose file when it exists, and the `reconstruction` block (synthetic scans only) is left out.
 `--scans` then caps the number of scans (default: all).  `--vertical-cell W` (with --data) turns on the ground segmentation's
 vertical-structure filter with W-metre columns (GroundParams.vertical_cell; 0, the default, leaves it off).
+
+`--final-iter` runs the mapper's key-scan refinement (mapper_specs.final_iter, src/mapping.py:154-164) before the final mesh:
+render_helpers.refine_map over the keyframe graph with KITTI's values (window 4, 2 x 2048 rays per keyframe, 25 iterations, embedding
+rate 0.01, len(keyframes) + 1 passes).  The JSON then carries `refine_ms` and, for synthetic scans, `reconstruction_before_refine`
+next to `reconstruction` (the refined map's mesh).
 """
 import argparse, json, os, sys, time
 from types import SimpleNamespace
@@ -69,6 +74,7 @@ def main():
     ap.add_argument("--dataset", default="kitti", choices=["kitti", "maicity"], help="layout of --data")
     ap.add_argument("--vertical-cell", type=float, default=0.0,
                     help="with --data: column width (m) of the ground segmentation's vertical-structure filter; 0 = off")
+    ap.add_argument("--final-iter", action="store_true", help="refine the map over every keyframe (refine_map) before the final mesh")
     a = ap.parse_args()
     if a.vertical_cell != 0.0 and a.data is None:
         ap.error("--vertical-cell applies to --data")
@@ -142,6 +148,25 @@ def main():
         est.append(cur)
         if i % 2 == 0:
             kg.insert_keyframe(fr)
+    # the map against the scans' noise-free returns at the true poses, in world coordinates (with the 2000 m offset, like the mesh)
+    def score(verts, faces):
+        clean = []
+        for i, (xyz, yaw) in enumerate(drive):
+            p, _, pose = syn.make_scan(seed=1000 + i, sensor_xyz=xyz, yaw=yaw, noise_std=0.0)
+            clean.append(p.astype(np.float64) @ pose[:3, :3].T.astype(np.float64) + pose[:3, 3])
+        t0 = tick()
+        recon = nl.evaluate.eval_mesh(verts, faces, np.concatenate(clean).astype(np.float32), n_samples=1_000_000, res=0.05, threshold=0.1,
+                                      truncation=0.5, seed=0)
+        recon["ms"] = (tick() - t0) * 1e3
+        return recon
+    refine = {}
+    if a.final_iter:
+        if a.data is None:
+            refine["reconstruction_before_refine"] = score(*nl.mesh.extract_mesh(dec, ms, vs, res=8))
+        t0 = tick()
+        rh.refine_map(kg, mu.embeddings, ms, dec, crit, vs, 0.5 * vs, N_rays=2 * 2048, num_iterations=25, truncation=trunc, max_voxel_hit=20,
+                      max_distance=md, learning_rate=lr[0])
+        refine = {"refine_ms": (tick() - t0) * 1e3, "refine_passes": len(kg.keyframe_graph) + 1, **refine}
     t0 = tick()
     verts, faces = nl.mesh.extract_mesh(dec, ms, vs, res=8)
     t_mesh = (tick() - t0) * 1e3
@@ -151,22 +176,14 @@ def main():
                "last_window_scans": [f.index for f in window], "ground_points": [int((s[1] < 1).sum()) for s in scans],
                "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0,
                "init_mapping_ms": t_init, "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
-               "map": {"nodes": ms.n_nodes, "embedding_rows": int(mu.n_rows), "last_update": mu.last_update}}
+               "map": {"nodes": ms.n_nodes, "embedding_rows": int(mu.n_rows), "last_update": mu.last_update}, **refine}
         if gt is not None:
             out.update(trajectory_errors(est, gt))
         print(json.dumps(out))
         if a.json:
             json.dump(out, open(a.json, "w"), indent=1)
         return
-    # the map against the scans' noise-free returns at the true poses, in world coordinates (with the 2000 m offset, like the mesh)
-    clean = []
-    for i, (xyz, yaw) in enumerate(drive):
-        p, _, pose = syn.make_scan(seed=1000 + i, sensor_xyz=xyz, yaw=yaw, noise_std=0.0)
-        clean.append(p.astype(np.float64) @ pose[:3, :3].T.astype(np.float64) + pose[:3, 3])
-    t0 = tick()
-    recon = nl.evaluate.eval_mesh(verts, faces, np.concatenate(clean).astype(np.float32), n_samples=1_000_000, res=0.05, threshold=0.1,
-                                  truncation=0.5, seed=0)
-    recon["ms"] = (tick() - t0) * 1e3
+    recon = score(verts, faces)
     errors = trajectory_errors(est, gt)
     out = {"scans": a.scans, "spacing_m": a.spacing, "octree": a.octree, "selection": a.selection, "path": a.path,
            "last_window_scans": [f.index for f in window], "translation_error_m": errors["translation_error_m"],
@@ -174,7 +191,7 @@ def main():
            "ms_per_scan": {k: float(np.median(v)) for k, v in T.items()}, "ms_first_tracked_scan": T["track"][0], "ms_first_update": t_update0, "init_mapping_ms": t_init,
            "mesh": {"ms": t_mesh, "vertices": int(verts.shape[0]), "triangles": int(faces.shape[0])},
            "map": {"nodes": ms.n_nodes, "embedding_rows": int(mu.n_rows), "last_update": mu.last_update},
-           "reconstruction": recon,
+           "reconstruction": recon, **refine,
            "per_scan_translation_error_m": errors["per_scan_translation_error_m"]}
     print(json.dumps(out))
     if a.json:
