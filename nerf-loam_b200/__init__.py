@@ -22,13 +22,15 @@ Public surface (mirrors the reference, see INTEGRATION.md):
                                     with the 'overlap' window the reference leaves unimplemented (voxel IoU with the scan, on the GPU)
     ground.points_and_cos / segment_ground  <- the Patchwork++ ground segmentation and pointsCos of src/dataset/kitti.py:40-70, on the GPU
     dataset.kitti / dataset.maicity .DataLoader  <- src/dataset/kitti.py, maicity.py (seam: sys.modules["dataset"] = nerfloam_b200.dataset)
+    slam.NeRFLOAM / Tracking / Mapping  <- src/nerfloam.py, tracking.py, mapping.py: a whole sequence, tracker and mapper concurrent on
+                                    two CUDA streams in a fixed lag-one schedule, writing the trajectory and the meshes
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
 no CPU or eager-PyTorch fallback for the kernels.
 """
 from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
-           "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise", "refine_map"]
+           "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise", "refine_map", "slam"]
 
 
 def __getattr__(name):

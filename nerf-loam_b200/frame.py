@@ -12,12 +12,13 @@ POSE_OFFSET = 2000   # metres added to the translation of externally supplied po
 _TINY = 1e-9
 
 
-def sample_rays(mask, num_samples):
+def sample_rays(mask, num_samples, generator=None):
     """Boolean mask [B,H,W] with exactly `num_samples` True cells per batch entry, drawn without replacement with probability
-    proportional to `mask` (Gumbel top-k, sample_util.py:4-19; the constants 1e-9 / 1e-7 are the reference's)."""
+    proportional to `mask` (Gumbel top-k, sample_util.py:4-19; the constants 1e-9 / 1e-7 are the reference's).  generator: a
+    torch.Generator on the mask's device to draw from instead of torch's (None: the reference's draw, torch.rand_like)."""
     batch, height, width = mask.shape
     weights = (mask / (mask.sum() + _TINY)).reshape(batch, height * width)
-    uniform = torch.rand_like(weights)
+    uniform = torch.rand(weights.shape, dtype=weights.dtype, device=weights.device, generator=generator)
     keys = torch.log(weights + _TINY) - torch.log(1e-7 - torch.log(uniform + 1e-7))
     chosen = keys.topk(num_samples, dim=-1).indices
     picked = torch.zeros_like(weights)
@@ -78,7 +79,8 @@ class LidarFrame(nn.Module):
         return directions
 
     @torch.no_grad()
-    def sample_rays(self, N_rays, track=False):
-        """Draws this iteration's rays: sample_mask bool[N,1] with N_rays True (every point equally likely)."""
+    def sample_rays(self, N_rays, track=False, generator=None):
+        """Draws this iteration's rays: sample_mask bool[N,1] with N_rays True (every point equally likely), from `generator` (a CPU
+        torch.Generator) when one is given."""
         every_point = torch.ones((1, self.num_point, 1))
-        self.sample_mask = sample_rays(every_point, N_rays)[0]
+        self.sample_mask = sample_rays(every_point, N_rays, generator)[0]

@@ -139,10 +139,11 @@ class KeyframeGraph:
         self.keyframe_graph.append(kf)
         return kf
 
-    def select_optimize_targets(self, tracked_frame=None, selection_method="previous"):
+    def select_optimize_targets(self, tracked_frame=None, selection_method="previous", generator=None):
         """mapping.py:205-225 with 'overlap' implemented: the window of keyframes (plus the tracked frame when it is not the current
         keyframe).  'overlap' ranks the keyframes by voxel IoU with tracked_frame, or with the current keyframe when tracked_frame
-        is None.  A graph of at most window_size keyframes returns every keyframe.  An unknown method raises ValueError."""
+        is None.  A graph of at most window_size keyframes returns every keyframe.  An unknown method raises ValueError.
+        generator: a CPU torch.Generator that 'random' draws its window from (torch.randperm) instead of the `random` module."""
         if selection_method not in METHODS:
             raise ValueError(f"selection method {selection_method!r} unknown (one of {', '.join(METHODS)})")
         if selection_method == "current":
@@ -151,6 +152,8 @@ class KeyframeGraph:
             return [tracked_frame]
         if len(self.keyframe_graph) <= self.window_size:
             targets = self.keyframe_graph[:]
+        elif selection_method == "random" and generator is not None:
+            targets = [self.keyframe_graph[i] for i in torch.randperm(len(self.keyframe_graph), generator=generator)[:self.window_size].tolist()]
         elif selection_method == "random":
             targets = random.sample(self.keyframe_graph, self.window_size)
         elif selection_method == "previous":

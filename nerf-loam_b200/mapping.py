@@ -268,10 +268,12 @@ class MapUpdater:
         if not self.incremental:
             return self._update_full()
         n = self.svo.count_export_nodes()
-        self._grow_nodes(n)
-        if self.readers is not None:      # a tracker on another stream may still traverse the arrays that are patched below
+        if self.readers is not None:
+            # a tracker on another stream may still traverse the arrays that are patched below; waiting before the capacity growth
+            # also orders this stream after those reads, so a buffer the growth frees cannot be reused under them
             for ev in self.readers.reader_events():
                 torch.cuda.current_stream(self.device).wait_event(ev)
+        self._grow_nodes(n)
         ids, m, new_rows = self._patch_rows(n)
         self._grow_rows(new_rows)
         self._pack_rows(ids, m)

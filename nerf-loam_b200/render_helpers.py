@@ -13,7 +13,9 @@ Behavioural notes (also in DESIGN.md):
   * the unused autograd.grad(sdf, xyz) of render_helpers.py:293-297 is not computed.
 """
 import os
+import threading
 import weakref
+from contextlib import contextmanager
 from copy import deepcopy
 
 import torch
@@ -31,20 +33,36 @@ _ENGINES = {}
 
 
 def _engine(n_rays, min_samples, device):
-    """Engines are cached by capacity class (power-of-two rays / samples)."""
+    """Engines are cached by capacity class (power-of-two rays / samples) and by the calling thread's current stream: a tracker and a
+    mapper on two streams (slam.NeRFLOAM) must neither share one engine's scratch nor evict (free) the other's while it is in use."""
     r = 1 << max(10, (int(n_rays) - 1).bit_length())
     m = 1 << max(16, (int(min_samples) - 1).bit_length())
-    key = (r, m, str(device))
+    stream = torch.cuda.current_stream(device).cuda_stream
+    key = (r, m, str(device), stream)
     e = _ENGINES.get(key)
     if e is None:
-        for k in [k for k in _ENGINES if k[0] <= r and k[1] <= m and k[2] == str(device)]:
-            del _ENGINES[k]
+        for k in [k for k in list(_ENGINES) if k[0] <= r and k[1] <= m and k[2:] == key[2:]]:
+            _ENGINES.pop(k, None)
         e = _ENGINES[key] = SDFEngine(r, m, device)
     return e
 
 
-def _seed_from_torch():
-    return int(torch.randint(1, 2 ** 31 - 1, (1,)).item())
+_CAPTURE_LOCK = threading.Lock()
+
+
+@contextmanager
+def _graph_capture(graph):
+    """torch.cuda.graph for the captured loops.  capture_error_mode="thread_local": in the default "global" mode a capture on one host
+    thread makes the other thread's stream synchronisations and read-backs fail (slam.NeRFLOAM runs the tracker and the mapper on two
+    threads); a single thread behaves the same in either mode.  The lock keeps two captures from running at once: torch.cuda.graph
+    shares one capture stream between threads, and entering a capture synchronises the device and empties the allocator's cache."""
+    with _CAPTURE_LOCK, torch.cuda.graph(graph, capture_error_mode="thread_local"):
+        yield
+
+
+def _seed_from_torch(generator=None):
+    """A fresh 31-bit seed from torch's CPU generator, or from `generator` (a CPU torch.Generator) when one is given."""
+    return int(torch.randint(1, 2 ** 31 - 1, (1,), generator=generator).item())
 
 
 def _cfg(step_size, voxel_size, max_distance, crit=None):
@@ -237,9 +255,12 @@ def get_scores(sdf_network, map_states, voxel_size, bits=8):
 # ======================================================================================================
 # optimisation loops
 # ======================================================================================================
-def _seed_from_cuda(dev):
-    """A fresh 32-bit seed drawn from torch's CUDA generator without a host round trip being needed later: a 1-element device tensor."""
-    return torch.randint(1, 2 ** 31 - 1, (1,), device=dev, dtype=torch.int32)
+def _seed_from_cuda(dev, generator=None):
+    """A fresh 32-bit seed drawn from torch's CUDA generator without a host round trip being needed later: a 1-element device tensor.
+    With `generator` (a CPU torch.Generator) the seed is drawn from it on the host and uploaded without blocking."""
+    if generator is None:
+        return torch.randint(1, 2 ** 31 - 1, (1,), device=dev, dtype=torch.int32)
+    return torch.randint(1, 2 ** 31 - 1, (1,), dtype=torch.int32, generator=generator).pin_memory().to(dev, non_blocking=True)
 
 
 def select_rays_device(dirs_all, gt_all, cos_all, n_select, n_dev=None, seed=None, out=None):
@@ -339,22 +360,25 @@ class _FrameBatch:
         self.cos = [a[1] for a in arrays]
         self.gt = [a[2] for a in arrays]
 
-    def select(self, N_rays, dev, track=False, mode="host"):
+    def select(self, N_rays, dev, track=False, mode="host", generator=None):
         """mode "host": ray selection like the reference (frame.sample_rays -> boolean mask, CPU torch RNG: the same seed
         picks the same rays as the reference), gathered on the device.  mode "device": the same distribution (uniform
         without replacement = top-k of iid keys, sample_util.py:4-19 with a constant mask) drawn with the CUDA generator,
-        no host round trip; frame.sample_mask is not updated."""
+        no host round trip; frame.sample_mask is not updated.  generator: a CPU torch.Generator to draw from instead of torch's."""
         d, g, c, fid = [], [], [], []
         for i, f in enumerate(self.frames):
             if mode == "device":
                 n = self.dirs[i].shape[0]
                 k = min(N_rays, n)
-                di, gi, ci = select_rays_device(self.dirs[i], self.gt[i], self.cos[i], k, n_dev=None, seed=_seed_from_cuda(dev))
+                di, gi, ci = select_rays_device(self.dirs[i], self.gt[i], self.cos[i], k, n_dev=None, seed=_seed_from_cuda(dev, generator))
                 d.append(di); g.append(gi); c.append(ci)
                 fid.append(torch.full((k,), i, dtype=torch.int32, device=dev))
                 continue
             with _few_threads():
-                f.sample_rays(N_rays, track=True) if track else f.sample_rays(N_rays)
+                if generator is not None:          # the reference's own LidarFrame has no generator argument
+                    f.sample_rays(N_rays, track=track, generator=generator)
+                else:
+                    f.sample_rays(N_rays, track=True) if track else f.sample_rays(N_rays)
                 idx = f.sample_mask.view(-1).nonzero().view(-1).to(dev, non_blocking=True)
             d.append(self.dirs[i][idx]); g.append(self.gt[i][idx]); c.append(self.cos[i][idx])
             fid.append(torch.full((idx.shape[0],), i, dtype=torch.int32, device=dev))
@@ -436,7 +460,7 @@ class _MapGraph:
         torch.cuda.current_stream(dev).wait_stream(side)
         l0 = _capi.LAUNCHES
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        with _graph_capture(self.graph):
             body()
         self.launches_per_iter = _capi.LAUNCHES - l0 + 1
         self.opt = state["opt"]
@@ -475,12 +499,12 @@ class _MapGraph:
             self.gt[i, :n].copy_(g)
             self.n_dev[i].fill_(n)
 
-    def run(self, frames, pose6_init, num_iterations, seed):
+    def run(self, frames, pose6_init, num_iterations, seed, generator=None):
         dev = self.dirs.device
         self._upload(frames)
         self.pose6.copy_(pose6_init)
         self.seed_dev.fill_(seed if seed < 2 ** 31 else seed - 2 ** 32)
-        self.sel_seed.copy_(_seed_from_cuda(dev))          # ray selection follows torch's CUDA generator (torch.manual_seed reproduces it)
+        self.sel_seed.copy_(_seed_from_cuda(dev, generator))   # ray selection follows torch's CUDA generator (torch.manual_seed reproduces it)
         for g in self.opt.groups:
             g["m"].zero_(); g["v"].zero_()
         self.pose_m.zero_(); self.pose_v.zero_()
@@ -494,7 +518,8 @@ class _MapGraph:
 def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, loss_criteria, voxel_size, step_size,
                          N_rays=512, num_iterations=10, truncation=0.1, max_voxel_hit=10, max_distance=10,
                          learning_rate=[1e-2, 1e-2, 5e-3], update_pose=True, update_decoder=True, profiler=None,
-                         deterministic=False, noise_per_iter=None, loss_log=None, ray_selection="device", cuda_graph=None):
+                         deterministic=False, noise_per_iter=None, loss_log=None, ray_selection="device", cuda_graph=None,
+                         generator=None):
     """render_helpers.py:321-425.  Mutates `embeddings` (bf16 CUDA table), the decoder parameters and the
     frame poses in place, like the reference.  Returns None.  ray_selection: see _FrameBatch.select ("device" by default;
     "host" reproduces the reference's CPU RNG stream ray for ray).  cuda_graph (default: on whenever ray_selection="device" and no
@@ -503,7 +528,10 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
     No host synchronisation per iteration: kernel error bits, "nothing was hit" iterations (which the reference skips,
     :405-409) and Adam's step count are tracked in a device-side control block that the Adam kernels read; the host looks at it
     once at the end of the call.  If the sample capacity was exceeded in any iteration the parameters and the RNG state are
-    restored and the whole call is redone with a larger engine, so a truncated sample set never reaches the parameters."""
+    restored and the whole call is redone with a larger engine, so a truncated sample set never reaches the parameters.
+
+    generator: a CPU torch.Generator that every random draw of the call (ray selection, sampler seeds) comes from instead of torch's
+    global generators, which it then leaves untouched -- two threads each with their own generator draw reproducibly."""
     if ray_selection not in ("host", "device"):
         raise ValueError("ray_selection must be 'host' or 'device'")
     dev = embeddings.device
@@ -538,10 +566,10 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
             groups += [dict(param=p.data, grad=g, lr=learning_rate[1], side=True) for p, g in zip(bufs.params, bufs.grads)]
         opt = None
         for it in range(num_iterations):
-            dirs, gt, cos, fid = batch.select(N_rays, dev, mode=ray_selection)
+            dirs, gt, cos, fid = batch.select(N_rays, dev, mode=ray_selection, generator=generator)
             eng.rays_from_poses(pose6, dirs, fid)
             noise = noise_per_iter[it] if noise_per_iter is not None else None
-            seed = 0 if (deterministic or noise is not None) else _seed_from_torch()
+            seed = 0 if (deterministic or noise is not None) else _seed_from_torch(generator)
             eng.forward_backward(m, bufs, dirs.shape[0], cfg, gt, cos, dir_local=dirs, ray_frame=fid, n_frames=F, noise=noise,
                                  rng_seed=seed, update_decoder=update_decoder, update_emb=True, update_pose=any(pose_opt), pose6=pose6,
                                  defer_wgrad=pipeline)
@@ -567,13 +595,13 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
         raise ValueError("cuda_graph=True needs ray_selection='device', no per-iteration host inputs/outputs and >= N_rays points per scan")
     cap = R * SAMPLES_PER_RAY_MAP
     while True:
-        snap = (emb.clone(), [p.data.clone() for p in bufs.params] if update_decoder else None, pose6.clone(),
-                torch.get_rng_state(), torch.cuda.get_rng_state(dev))
+        rng = (generator.get_state(),) if generator is not None else (torch.get_rng_state(), torch.cuda.get_rng_state(dev))
+        snap = (emb.clone(), [p.data.clone() for p in bufs.params] if update_decoder else None, pose6.clone(), rng)
         n_log = len(loss_log) if loss_log is not None else 0
         if cuda_graph:
             g = _MapGraph.get(m, emb, sdf_network, cfg, F, N_rays, learning_rate, update_decoder, pose_rows, deterministic,
                               max(f.points.shape[0] for f in frames), -(-cap // R))
-            ctl = g.run(frames, pose6, num_iterations, 0 if deterministic else _seed_from_torch())
+            ctl = g.run(frames, pose6, num_iterations, 0 if deterministic else _seed_from_torch(generator), generator)
             pose6.copy_(g.pose6)
         else:
             eng = _engine(R, cap, dev)
@@ -587,7 +615,10 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
             if snap[1] is not None:
                 for p, q in zip(bufs.params, snap[1]):
                     p.data.copy_(q)
-        torch.set_rng_state(snap[3]); torch.cuda.set_rng_state(snap[4], dev)
+        if generator is not None:
+            generator.set_state(snap[3][0])
+        else:
+            torch.set_rng_state(snap[3][0]); torch.cuda.set_rng_state(snap[3][1], dev)
         if loss_log is not None:
             del loss_log[n_log:]
         cap = _grown_capacity(cap, ctl, "bundle_adjust_frames")
@@ -600,17 +631,17 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
                 f.pose.data.copy_(host[i].to(f.pose.data.device))
 
 
-def refine_schedule(keyframe_graph, passes, deterministic=False, device="cuda"):
+def refine_schedule(keyframe_graph, passes, deterministic=False, device="cuda", generator=None):
     """What the mapper's final_iter loop (mapping.py:154-164) draws, drawn up front in the loop's order: per pass the window
     (KeyframeGraph.select_optimize_targets(None, 'random'), as indices into keyframe_graph.keyframe_graph in window order), the sampler
     noise seed (torch's CPU generator, 0 when deterministic) and the ray-selection seed (torch's generator on `device`: an int32[1]
-    tensor there).  Returns (windows, noise_seeds, selection_seeds)."""
+    tensor there), all from `generator` (a CPU torch.Generator) instead when one is given.  Returns (windows, noise_seeds, selection_seeds)."""
     index = {id(f): i for i, f in enumerate(keyframe_graph.keyframe_graph)}
     windows, noise, sel = [], [], []
     for _ in range(passes):
-        windows.append([index[id(f)] for f in keyframe_graph.select_optimize_targets(None, "random")])
-        noise.append(0 if deterministic else _seed_from_torch())
-        sel.append(_seed_from_cuda(device))
+        windows.append([index[id(f)] for f in keyframe_graph.select_optimize_targets(None, "random", generator=generator)])
+        noise.append(0 if deterministic else _seed_from_torch(generator))
+        sel.append(_seed_from_cuda(device, generator))
     return windows, noise, sel
 
 
@@ -693,7 +724,7 @@ class _RefineGraph:
         torch.cuda.current_stream(dev).wait_stream(side)
         l0 = _capi.LAUNCHES
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        with _graph_capture(self.graph):
             self.body()
         self.launches_per_iter = _capi.LAUNCHES - l0 + 1
         with torch.no_grad():
@@ -737,7 +768,7 @@ class _RefineGraph:
 
 
 def refine_map(keyframe_graph, embeddings, map_states, sdf_network, loss_criteria, voxel_size, step_size, N_rays=512, num_iterations=10,
-               truncation=0.1, max_voxel_hit=10, max_distance=10, learning_rate=1e-2, passes=None, deterministic=False):
+               truncation=0.1, max_voxel_hit=10, max_distance=10, learning_rate=1e-2, passes=None, deterministic=False, generator=None):
     """The mapper's key-scan refinement (`mapper_specs.final_iter`, mapping.py:154-164): `passes` (default len(keyframe_graph) + 1)
     bundle adjustments of a random window of keyframes with poses and decoder frozen, each with a fresh Adam on the embedding table,
     i.e. under the same random.seed / torch.manual_seed what
@@ -753,7 +784,7 @@ def refine_map(keyframe_graph, embeddings, map_states, sdf_network, loss_criteri
     Everything the loop draws is drawn up front (refine_schedule) and uploaded once; one captured iteration (_RefineGraph) is replayed
     passes x num_iterations times, and Adam steps only the rows the pass has reached, which is exact because the optimiser is fresh in
     every pass (include/nerfloam_b200.h section 14).  The control block is read once at the end; a call that exceeded the sample
-    capacity is undone and redone with room for its largest iteration."""
+    capacity is undone and redone with room for its largest iteration.  generator: a CPU torch.Generator for every draw (refine_schedule)."""
     frames = list(keyframe_graph.keyframe_graph)
     K = len(frames)
     if K == 0:
@@ -770,7 +801,7 @@ def refine_map(keyframe_graph, embeddings, map_states, sdf_network, loss_criteri
     if not (emb.dtype == torch.bfloat16 and emb.is_contiguous()):
         raise ValueError("refine_map: embeddings must be a contiguous bf16 CUDA tensor (mapping.py:305-314)")
     dev = emb.device
-    windows, noise, sel = refine_schedule(keyframe_graph, P, deterministic, dev)
+    windows, noise, sel = refine_schedule(keyframe_graph, P, deterministic, dev, generator)
     if P == 0 or num_iterations == 0:
         return None
     m = map_states if isinstance(map_states, MapState) else MapState.from_map_states(map_states, dev)
@@ -853,7 +884,7 @@ class _TrackGraph:
         torch.cuda.current_stream(dev).wait_stream(side)
         l0 = _capi.LAUNCHES
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        with _graph_capture(self.graph):
             body()
         self.launches_per_iter = _capi.LAUNCHES - l0 + 1
 
@@ -885,13 +916,13 @@ class _TrackGraph:
         self.gt[:n].copy_(g)
         self.n_dev.fill_(n)
 
-    def run(self, frame, pose6_init, num_iterations, seed):
+    def run(self, frame, pose6_init, num_iterations, seed, generator=None):
         dev = self.dirs.device
         self.bufs.refresh_transposes()        # the decoder may have been updated in place since the capture (same pointers, new values)
         self._upload(frame)
         self.pose6.copy_(pose6_init)
         self.seed_dev.fill_(seed if seed < 2 ** 31 else seed - 2 ** 32)
-        self.sel_seed.copy_(_seed_from_cuda(dev))          # ray selection follows torch's CUDA generator (torch.manual_seed reproduces it)
+        self.sel_seed.copy_(_seed_from_cuda(dev, generator))          # ray selection follows torch's CUDA generator (torch.manual_seed reproduces it)
         self.adam_m.zero_(); self.adam_v.zero_()
         self.eng.begin_call()
         for _ in range(num_iterations):
@@ -901,7 +932,7 @@ class _TrackGraph:
 
 
 def _track_frame_graph(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, voxel_size, N_rays, step_size, num_iterations,
-                       learning_rate, max_distance, deterministic):
+                       learning_rate, max_distance, deterministic, generator):
     dev = torch.device("cuda")
     m = map_states if isinstance(map_states, MapState) else MapState.from_map_states(map_states, dev)
     cfg = _cfg(step_size, voxel_size, max_distance, loss_criteria)
@@ -911,12 +942,12 @@ def _track_frame_graph(frame_pose, curr_frame, map_states, sdf_network, loss_cri
     n_points = curr_frame.points.shape[0]
     if n_points < N_rays:
         raise ValueError("cuda_graph=True needs at least N_rays points in the scan")
-    seed = 0 if deterministic else _seed_from_torch()
+    seed = 0 if deterministic else _seed_from_torch(generator)
     spr = SAMPLES_PER_RAY_TRACK
     while True:
         g = _TrackGraph.get(m, sdf_network, cfg, N_rays, lr, deterministic, n_points, spr)
         eng = g.eng
-        st, ctl = g.run(curr_frame, init_pose.data.detach().reshape(1, 6), num_iterations, seed)
+        st, ctl = g.run(curr_frame, init_pose.data.detach().reshape(1, 6), num_iterations, seed, generator)
         _check_ctl(ctl, "track_frame")
         if not (ctl[_capi.CTL_ERROR] & 2):
             break
@@ -932,13 +963,14 @@ def _track_frame_graph(frame_pose, curr_frame, map_states, sdf_network, loss_cri
 def track_frame(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, voxel_size, N_rays=512, step_size=0.05,
                 num_iterations=10, truncation=0.1, learning_rate=1e-3, max_voxel_hit=10, max_distance=10, profiler=None,
                 depth_variance=False, deterministic=False, noise_per_iter=None, loss_log=None, ray_selection="device",
-                cuda_graph=None):
+                cuda_graph=None, generator=None):
     """render_helpers.py:428-514: optimise the 6-vector pose of one scan against a frozen map.
     Returns (OptimizablePose on the GPU, hit_mask bool[N_rays]) or (pose, None) if nothing was hit.
     ray_selection: see _FrameBatch.select.  cuda_graph=True (needs ray_selection="device"): the iteration -- ray selection,
     rays, traversal, sampling, gather, decoder forward/backward, pose gradient, Adam -- is captured once and replayed, with
     the sampler seed and the Adam step count in device memory; the host looks at the statistics once at the end instead of
-    every iteration (an iteration without hits makes the call return (pose, None) like the reference, just later)."""
+    every iteration (an iteration without hits makes the call return (pose, None) like the reference, just later).
+    generator: a CPU torch.Generator that the call's draws come from instead of torch's global generators (bundle_adjust_frames)."""
     if ray_selection not in ("host", "device"):
         raise ValueError("ray_selection must be 'host' or 'device'")
     graph_ok = ray_selection == "device" and noise_per_iter is None and loss_log is None and curr_frame.points.shape[0] >= N_rays
@@ -950,7 +982,7 @@ def track_frame(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, 
         if not graph_ok:
             raise ValueError("cuda_graph=True needs ray_selection='device', no per-iteration host inputs/outputs and >= N_rays points")
         return _track_frame_graph(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, voxel_size, N_rays, step_size,
-                                  num_iterations, learning_rate, max_distance, deterministic)
+                                  num_iterations, learning_rate, max_distance, deterministic, generator)
     dev = torch.device("cuda")
     m = map_states if isinstance(map_states, MapState) else MapState.from_map_states(map_states, dev)
     cfg = _cfg(step_size, voxel_size, max_distance, loss_criteria)
@@ -968,9 +1000,9 @@ def track_frame(frame_pose, curr_frame, map_states, sdf_network, loss_criteria, 
     n_last = 0
     bufs.refresh_transposes()           # the decoder is frozen while tracking: derive the kernel-side weight images once
     for it in range(num_iterations):
-        dirs, gt, cos, fid = batch.select(N_rays, dev, track=True, mode=ray_selection)
+        dirs, gt, cos, fid = batch.select(N_rays, dev, track=True, mode=ray_selection, generator=generator)
         noise = noise_per_iter[it] if noise_per_iter is not None else None
-        seed = 0 if (deterministic or noise is not None) else _seed_from_torch()
+        seed = 0 if (deterministic or noise is not None) else _seed_from_torch(generator)
         while True:
             eng.rays_from_poses(pose6, dirs, None)
             eng.forward_backward(m, bufs, dirs.shape[0], cfg, gt, cos, dir_local=dirs, ray_frame=None, n_frames=1, noise=noise,

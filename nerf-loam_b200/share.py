@@ -93,11 +93,20 @@ class SharedMap:
         self._front = self._slots.index(s)
         return s.version
 
-    def acquire(self):
-        """Called on the tracker's stream: (map_state, decoder, slot).  The stream waits for the publication, not the host."""
+    def acquire(self, version=None):
+        """Called on the tracker's stream: (map_state, decoder, slot).  The stream waits for the publication, not the host.
+        version: None takes the latest publication; a number takes that publication (publish()'s return value), which must still
+        be in one of the two slots -- a reader that lags by at most one publication and releases before the mapper publishes again
+        (slam.NeRFLOAM's schedule) always finds it there.  A version that is not (any more, or not yet) held raises RuntimeError."""
         if self._front < 0:
             raise RuntimeError("nothing has been published yet")
-        s = self._slots[self._front]
+        if version is None:
+            s = self._slots[self._front]
+        else:
+            held = [t for t in self._slots if t.version == version]
+            if not held:
+                raise RuntimeError(f"map version {version} is not held (the slots hold {sorted(t.version for t in self._slots if t.version >= 0)})")
+            s = held[0]
         torch.cuda.current_stream().wait_event(s.published)
         if s.decoder is None:
             s.decoder = self._factory()

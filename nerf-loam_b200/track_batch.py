@@ -214,7 +214,7 @@ class _TrackBatchGraph:
         torch.cuda.current_stream(dev).wait_stream(side)
         l0 = _capi.LAUNCHES
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        with rh._graph_capture(self.graph):
             body()
         self.launches_per_iter = _capi.LAUNCHES - l0 + 1
 
