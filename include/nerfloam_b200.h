@@ -726,6 +726,57 @@ NL_API int nl_adam_bf16_rows_ctl(int64_t n_rows, const int32_t *d_rows, const in
 NL_API int nl_refine_iter_end(int iters, int32_t *d_state, int32_t *d_sel_seed, int32_t sel_inc, int32_t *d_noise_seed, int32_t noise_inc,
                               void *stream);
 
+/* ============================================================================================
+ * 15. Global localisation, coarse stage (DESIGN.md section 3.4; csrc/globalloc.cu): for every placement of a scan over a lattice of
+ *     positions x headings around anchor poses, how many of M scan points fall in an occupied map voxel, and the n highest counts.
+ *     Occupied set: the map's leaf voxels (structure[i][8] == 1, Octree.get_leaf_voxels()), key floor(centre / voxel_size) per axis
+ *     packed as vx << 36 | vy << 18 | vz, in an open-addressing set (hash.cuh) of nl_globalloc_occupied_slots(n_leaves) u64 slots.
+ *     Anchors: A >= 1 poses, f64[A][12] = the 3x4 matrix row-major (host copy h_anchors for the checks, device copy d_anchors).
+ *     Cells: lattice points (i, j) x xy_step within radius (fp64 xy distance) of an anchor, with the nearest anchor (lower index on a
+ *     tie of the fp32 distance), numbered in ascending (i, j); d_cells i32[n_cells][3] = (i, j, anchor).
+ *     Placement id = cell x yaw_steps + k: rotation Rz(2 pi k / yaw_steps - atan2(R_a10, R_a00)) R_a, translation (i xy_step,
+ *     j xy_step, t_a,z), formed in fp64 and rounded to fp32; ids are int32, so n_cells x yaw_steps < 2^31.
+ *     Count: the points whose world point ((R0 x + R1 y) + R2 z) + t (fp64 from fp32) has voxel floor(w / voxel_size) inside
+ *     [0, grid_dim)^3 and in the set (the arithmetic of section 12).  Every result is an exact integer or a function of integers,
+ *     independent of atomics order and launch shape.  Bad arguments return an error code; no entry point aborts.
+ * ============================================================================================ */
+#define NL_GLOBALLOC_MAX_POINTS 8192   /* M: the scan points are staged in shared memory (12 B each) */
+/* out = (NL_GLOBALLOC_MAX_POINTS, ints per cell row) */
+NL_API void nl_abi_sizes_globalloc(int32_t out[2]);
+/* *d_n_leaves = the rows of d_structure i32[n_nodes][9] with side 1.  n_nodes >= 1. */
+NL_API int nl_globalloc_count_leaves(int64_t n_nodes, const int32_t *d_structure, int64_t *d_n_leaves, void *stream);
+/* Slots of the occupied set: a power of two >= max(2^10, 2 n_leaves); an error for n_leaves < 1 (an empty map). */
+NL_API int64_t nl_globalloc_occupied_slots(int64_t n_leaves);
+/* Clears d_set u64[slots] and inserts the key of every leaf row whose voxel lies in [0, grid_dim)^3.  grid_dim a power of two
+ * <= 2^18; slots a power of two >= 2 x the leaf count. */
+NL_API int nl_globalloc_occupied(int64_t n_nodes, const float *d_centres, const int32_t *d_structure, double voxel_size, int64_t grid_dim,
+                                 int64_t slots, uint64_t *d_set, void *stream);
+/* Workspace of nl_globalloc_cells / _finish: a hash of (i, j) and a key list sized from the lattice points the anchors' boxes can
+ * hold.  Checks A >= 1, finite anchors, radius finite and >= 0, xy_step finite and > 0, and the lattice size. */
+NL_API int64_t nl_globalloc_cells_workspace_bytes(int32_t n_anchors, const double *h_anchors, double radius, double xy_step);
+/* First half of the cell table: inserts every cell with its nearest anchor and writes *d_n_cells (int64, device).  The caller reads
+ * the count back and passes it to nl_globalloc_cells_finish with the same workspace. */
+NL_API int nl_globalloc_cells(int32_t n_anchors, const double *h_anchors, const double *d_anchors, double radius, double xy_step, void *d_ws,
+                              int64_t ws_bytes, int64_t *d_n_cells, void *stream);
+/* Sorts the cells by (i, j) and writes d_cells i32[n_cells][3]. */
+NL_API int nl_globalloc_cells_finish(int32_t n_anchors, const double *h_anchors, double radius, double xy_step, int64_t n_cells, void *d_ws,
+                                     int64_t ws_bytes, int32_t *d_cells, void *stream);
+/* d_Rt12 f32[n][12] (R row-major, then t) of the placements d_ids i64[n]: the device function the scorer uses.  An id outside
+ * [0, n_cells x yaw_steps) gets a matrix of NaN. */
+NL_API int nl_globalloc_matrices(int64_t n, const int64_t *d_ids, int64_t n_cells, const int32_t *d_cells, const double *d_anchors,
+                                 int32_t yaw_steps, double xy_step, float *d_Rt12, void *stream);
+/* d_counts[h] for the placements h in [p0, p0 + n): how many of d_points f32[n_points][3] (sensor frame, 1 <= n_points <=
+ * NL_GLOBALLOC_MAX_POINTS) land in the occupied set d_set u64[slots]. */
+NL_API int nl_globalloc_score(int64_t p0, int64_t n, int64_t n_cells, const int32_t *d_cells, const double *d_anchors, int32_t yaw_steps,
+                              double xy_step, int32_t n_points, const float *d_points, const uint64_t *d_set, int64_t slots, double voxel_size,
+                              int64_t grid_dim, int32_t *d_counts, void *stream);
+NL_API int64_t nl_globalloc_select_workspace_bytes(int64_t n_placements, int32_t n_points, int64_t n_select);
+/* The n_select placements of highest d_counts i32[n_placements] ranked by (count desc, id asc): d_ids i32[n_select] and their counts
+ * d_sel_counts i32[n_select].  A count outside [0, n_points] is ignored; when fewer than n_select counts are valid, the remaining
+ * entries of both outputs are -1.  1 <= n_select <= n_placements; workspace 256-byte aligned. */
+NL_API int nl_globalloc_select(int64_t n_placements, const int32_t *d_counts, int32_t n_points, int64_t n_select, void *d_ws, int64_t ws_bytes,
+                               int32_t *d_ids, int32_t *d_sel_counts, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

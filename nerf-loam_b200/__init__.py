@@ -14,6 +14,8 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     track_frames (= render_helpers.track_frames, track_batch)  K independent track_frame problems in one launch chain
     refine_map (= render_helpers.refine_map)  the mapper's key-scan refinement (mapper_specs.final_iter, src/mapping.py:154-164)
     score_poses / relocalise (= render_helpers.*, score)  the loss of up to 65 535 pose hypotheses of one scan; recovering a lost scan
+    relocalise_global (globalloc)   a scan placed anywhere within a radius of anchor poses with no guess: millions of placements
+                                    scored by occupied-voxel counts on the GPU, the best refined with score_poses and relocalise
     mapping.MapUpdater              <- Mapping.create_voxels / update_grid_features / get_embeddings (src/mapping.py)
     mesh.extract_mesh / marching_cubes  <- MeshExtractor.create_mesh / marching_cubes (src/utils/mesh_util.py)
     evaluate.eval_mesh / sample_surface / voxel_down_sample / nearest_distances  <- the map evaluation of Readme.md ("Evaluation"):
@@ -30,7 +32,8 @@ no CPU or eager-PyTorch fallback for the kernels.
 from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
-           "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise", "refine_map", "slam"]
+           "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise", "refine_map", "slam",
+           "globalloc", "relocalise_global"]
 
 
 def __getattr__(name):
@@ -41,6 +44,8 @@ def __getattr__(name):
         return importlib.import_module(".render_helpers", __name__).refine_map
     if name in ("score_poses", "relocalise"):
         return getattr(importlib.import_module(".score", __name__), name)
+    if name == "relocalise_global":
+        return importlib.import_module(".globalloc", __name__).relocalise_global
     if name in __all__:
         return importlib.import_module("." + name, __name__)
     raise AttributeError(name)

@@ -190,6 +190,19 @@ _SIGNATURES = {
     "nl_mark_rows": (C.c_int, [C.c_int64, vp, vp, vp, C.c_int64, vp, vp, vp, vp]),
     "nl_adam_bf16_rows_ctl": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),
     "nl_refine_iter_end": (C.c_int, [C.c_int, vp, vp, C.c_int32, vp, C.c_int32, vp]),
+    # global localisation, coarse stage (include/nerfloam_b200.h section 15)
+    "nl_abi_sizes_globalloc": (None, [C.POINTER(C.c_int32 * 2)]),
+    "nl_globalloc_count_leaves": (C.c_int, [C.c_int64, vp, vp, vp]),
+    "nl_globalloc_occupied_slots": (C.c_int64, [C.c_int64]),
+    "nl_globalloc_occupied": (C.c_int, [C.c_int64, vp, vp, C.c_double, C.c_int64, C.c_int64, vp, vp]),
+    "nl_globalloc_cells_workspace_bytes": (C.c_int64, [C.c_int32, vp, C.c_double, C.c_double]),
+    "nl_globalloc_cells": (C.c_int, [C.c_int32, vp, vp, C.c_double, C.c_double, vp, C.c_int64, vp, vp]),
+    "nl_globalloc_cells_finish": (C.c_int, [C.c_int32, vp, C.c_double, C.c_double, C.c_int64, vp, C.c_int64, vp, vp]),
+    "nl_globalloc_matrices": (C.c_int, [C.c_int64, vp, C.c_int64, vp, vp, C.c_int32, C.c_double, vp, vp]),
+    "nl_globalloc_score": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, vp, vp, C.c_int32, C.c_double, C.c_int32, vp, vp, C.c_int64, C.c_double,
+                                     C.c_int64, vp, vp]),
+    "nl_globalloc_select_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int64]),
+    "nl_globalloc_select": (C.c_int, [C.c_int64, vp, C.c_int32, C.c_int64, vp, C.c_int64, vp, vp, vp]),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)
@@ -200,6 +213,7 @@ SCORE_MAX_PROBLEMS = 65535   # NL_SCORE_MAX_PROBLEMS
 EVAL_KEY_BITS = 21           # NL_EVAL_KEY_BITS
 EVAL_TILE = 2048             # NL_EVAL_TILE
 GROUND_MAX_PATCHES = 1024    # NL_GROUND_MAX_PATCHES
+GLOBALLOC_MAX_POINTS = 8192  # NL_GLOBALLOC_MAX_POINTS
 # words of the refinement state block (include/nerfloam_b200.h section 14)
 REFINE_ITER, REFINE_LISTED, REFINE_PREV, REFINE_STATE_WORDS = 0, 1, 2, 4
 STATS_PACK_FIXED = 10
@@ -256,6 +270,10 @@ def lib():
         gmine = [C.sizeof(GroundParams), GROUND_MAX_PATCHES, GROUND_PATCH_BYTES]
         if list(gsizes) != gmine:
             raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (ground): {list(gsizes)} vs {gmine}")
+        lsizes = (C.c_int32 * 2)()
+        L.nl_abi_sizes_globalloc(C.byref(lsizes))
+        if list(lsizes) != [GLOBALLOC_MAX_POINTS, 3]:
+            raise ImportError(f"ABI mismatch between _capi.py and libnerfloam_b200.so (globalloc): {list(lsizes)} vs {[GLOBALLOC_MAX_POINTS, 3]}")
         _lib = L
     return _lib
 

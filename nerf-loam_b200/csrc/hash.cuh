@@ -1,7 +1,8 @@
 // Open-addressing hash sets of 64-bit keys with linear probing, shared by eval.cu (cell table of the nearest-neighbour search),
-// overlap.cu (voxel sets of the keyframe overlap) and ground.cu (column table of the vertical filter).  A slot holds NL_HASH_EMPTY until one atomicCAS claims it, and is never
+// overlap.cu (voxel sets of the keyframe overlap), ground.cu (column table of the vertical filter) and globalloc.cu (occupied
+// voxels and lattice cells of the global localisation).  A slot holds NL_HASH_EMPTY until one atomicCAS claims it, and is never
 // written again, so a plain load that sees a key sees it for good; a stale "empty" is resolved by the CAS.  The caller keeps the
-// capacity a power of two and the load factor below 1 (both users stay at or below 1/2), and never stores NL_HASH_EMPTY as a key.
+// capacity a power of two and the load factor below 1 (every user here stays at or below 1/2), and never stores NL_HASH_EMPTY as a key.
 #pragma once
 #include <cstdint>
 

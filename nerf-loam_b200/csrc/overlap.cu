@@ -1,8 +1,8 @@
 // Voxel overlap of one scan with K keyframes (include/nerfloam_b200.h section 12): the counts behind the mapper's 'overlap'
 // keyframe window (src/mapping.py:205-225 declares that method and leaves it unimplemented).
 //
-//   world point : w_i = ((R_i0 x + R_i1 y) + R_i2 z) + t_i in fp64 from the fp32 matrix and point.  The products are exact in
-//                 fp64, so FMA contraction cannot change the result; the parentheses fix the order of the additions.
+//   world point : w_i = ((R_i0 x + R_i1 y) + R_i2 z) + t_i in fp64 from the fp32 matrix and point (voxel.cuh, shared with
+//                 globalloc.cu).
 //   voxel       : floor(w / voxel_size) in fp64 per axis; a point whose voxel leaves [0, grid_dim)^3 (or is not finite) is not
 //                 counted.  Key = vx << 36 | vy << 18 | vz (grid_dim <= 2^18, so 54 bits).
 //   frame set   : every point of the scan goes into an open-addressing set (capacity a power of two >= 2N); a first insertion
@@ -24,11 +24,12 @@
 #include "../../include/nerfloam_b200.h"
 #include "hash.cuh"
 #include "nl_cuda.cuh"
+#include "voxel.cuh"
 
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kAxisBits = 18;                            // log2 of the largest grid_dim (MapUpdater's default, 256 * 256 * 4)
+constexpr int kAxisBits = NL_VOXEL_AXIS_BITS;
 constexpr int kKfShift = 3 * kAxisBits;                  // composite key: keyframe << 54 | voxel key
 constexpr int kMaxChunk = NL_OVERLAP_MAX_CHUNK;          // keyframes per chunk: local index <= 1022 in the top 10 bits
 constexpr int64_t kMinSlots = 1024;
@@ -43,20 +44,6 @@ int64_t pow2_at_least(int64_t v) {
 int64_t frame_slots(int64_t n) { return std::max(kMinSlots, pow2_at_least(2 * n)); }
 
 bool is_pow2(int64_t v) { return v > 0 && (v & (v - 1)) == 0; }
-
-__device__ __forceinline__ bool voxel_key(const float (&Rt)[12], float x, float y, float z, double vs, double gd, uint64_t &key) {
-    uint64_t k = 0;
-    #pragma unroll
-    for (int i = 0; i < 3; ++i) {
-        const double w = (((double)Rt[3 * i] * (double)x + (double)Rt[3 * i + 1] * (double)y) + (double)Rt[3 * i + 2] * (double)z) +
-                         (double)Rt[9 + i];
-        const double v = floor(w / vs);
-        if (!(v >= 0.0 && v < gd)) return false;
-        k = (k << kAxisBits) | (uint64_t)v;
-    }
-    key = k;
-    return true;
-}
 
 __device__ __forceinline__ void load_rt(const float *__restrict__ row, float (&Rt)[12]) {
     #pragma unroll
@@ -87,7 +74,7 @@ __global__ void __launch_bounds__(kThreads) k_frame_set(int64_t n, const float *
     for (int64_t base = blockIdx.x * (int64_t)kThreads + (threadIdx.x & ~31); base < n; base += (int64_t)gridDim.x * kThreads) {
         const int64_t i = base + lane;
         uint64_t key = 0;
-        const bool ok = i < n && voxel_key(Rt, p[3 * i], p[3 * i + 1], p[3 * i + 2], vs, gd, key);
+        const bool ok = i < n && nl_voxel_key(Rt, p[3 * i], p[3 * i + 1], p[3 * i + 2], vs, gd, key);
         const bool dup = repeats_previous(ok, key);
         if (ok && !dup && nl_hash_insert(set, mask, key)) ++added;
     }
@@ -111,7 +98,7 @@ __global__ void __launch_bounds__(kThreads) k_keyframes(int k0, const float *con
     for (int64_t base = blockIdx.x * (int64_t)kThreads + (threadIdx.x & ~31); base < n; base += (int64_t)gridDim.x * kThreads) {
         const int64_t i = base + lane;
         uint64_t key = 0;
-        const bool ok = i < n && voxel_key(Rt, p[3 * i], p[3 * i + 1], p[3 * i + 2], vs, gd, key);
+        const bool ok = i < n && nl_voxel_key(Rt, p[3 * i], p[3 * i + 1], p[3 * i + 2], vs, gd, key);
         out += (i < n && !ok);
         const bool dup = repeats_previous(ok, key);
         if (ok && !dup && nl_hash_insert(set, mask, tag | key)) {
