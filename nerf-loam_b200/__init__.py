@@ -25,7 +25,10 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     ground.points_and_cos / segment_ground  <- the Patchwork++ ground segmentation and pointsCos of src/dataset/kitti.py:40-70, on the GPU
     dataset.kitti / dataset.maicity .DataLoader  <- src/dataset/kitti.py, maicity.py (seam: sys.modules["dataset"] = nerfloam_b200.dataset)
     slam.NeRFLOAM / Tracking / Mapping  <- src/nerfloam.py, tracking.py, mapping.py: a whole sequence, tracker and mapper concurrent on
-                                    two CUDA streams in a fixed lag-one schedule, writing the trajectory and the meshes
+                                    two CUDA streams in a fixed lag-one schedule, writing the trajectory and the meshes;
+                                    NeRFLOAM.save_map / slam.load_map: the finished run's map, decoder and trajectory as one file
+    localise.Localiser              a sequence localised in a saved map: the first scan placed by relocalise_global with no guess,
+                                    the rest tracked by slam.Tracking against the frozen map
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
 no CPU or eager-PyTorch fallback for the kernels.
 """
@@ -33,7 +36,7 @@ from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
            "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise", "refine_map", "slam",
-           "globalloc", "relocalise_global"]
+           "globalloc", "relocalise_global", "localise"]
 
 
 def __getattr__(name):

@@ -16,7 +16,8 @@ fixed (the lag-one schedule, DESIGN.md section 11.3):
 Outputs under out_dir, in the reference's layout (loggers.py:17-29, 56-71): mesh/mesh_{index:05d}.ply, mesh/final_mesh_noreplay.ply,
 mesh/final_mesh.ply (binary little-endian PLY, float32 xyz and int32 faces, with the -2000 m offset removed as mesh_util.py:139
 does) and misc/frame_poses_{index:05d}.txt, misc/frame_poses.txt (one scan per line, the top 3 x 4 of its pose row-major: KITTI's
-format, loggers.py:144-159).
+format, loggers.py:144-159).  NeRFLOAM.save_map(path) writes the finished run's map, decoder, trajectory and settings to one file
+(write_map); load_map reads it back onto either octree, and localise.Localiser localises later scans in it.
 
 Deviations from the reference (also in DESIGN.md section 11.3):
   * end_frame is clamped to len - 1: the reference's min(end_frame, len) and range(..., end_frame + 1) index past the last scan
@@ -33,6 +34,7 @@ import queue
 import random
 import threading
 import time
+from collections import namedtuple
 from types import SimpleNamespace
 
 import numpy as np
@@ -46,7 +48,7 @@ from .lidar import Decoder
 from .mapping import MapUpdater
 from .mesh import extract_mesh
 from .se3pose import OptimizablePose
-from .share import SharedMap
+from .share import SharedMap, _flat_decoder_state, load_flat_decoder_state
 
 SELECTIONS = ("current", "previous", "overlap")
 
@@ -318,6 +320,7 @@ class Mapping(_Timed):
         os.makedirs(self.mesh_dir, exist_ok=True)
         os.makedirs(self.misc_dir, exist_ok=True)
         self.first_frame_id = None
+        self.scan_ids = []                  # frame.index of each trajectory entry, in the trajectory's order
         self.times, self.streams = {}, set()
 
     # -- the steps ---------------------------------------------------------------------------------------------------------
@@ -371,6 +374,7 @@ class Mapping(_Timed):
     # -- helpers -----------------------------------------------------------------------------------------------------------
     def _end_step(self, frame):
         self.trajectory.record(self.kg, frame)
+        self.scan_ids.append(frame.index)
         if self.mesh_freq > 0 and frame.index % self.mesh_freq == 0:
             big = self.final_iter and len(self.kg.keyframe_graph) > 20
             if big:
@@ -562,6 +566,152 @@ def run_pipeline(tracker, mapper, streams=None, schedule=None):
 
 
 # ----------------------------------------------------------------------------------------------------------------------------
+# map files
+# ----------------------------------------------------------------------------------------------------------------------------
+MAP_FORMAT = "nerfloam_b200.map/1"
+MAP_KEYS = ("format", "map", "decoder", "trajectory", "scan_ids", "config")
+CONFIG_KEYS = ("criteria", "tracker_specs", "voxel_size", "data_specs", "dataset")
+
+SavedMap = namedtuple("SavedMap", ["map", "decoder", "decoder_specs", "trajectory", "scan_ids", "config"])
+SavedMap.__doc__ = """A run's map: map (mapping.MapUpdater), decoder (lidar.Decoder), decoder_specs (dict), trajectory f64[S,4,4] (the
+poses of frame_poses.txt, without POSE_OFFSET), scan_ids i64[S] and config (criteria, tracker_specs, voxel_size, data_specs, dataset
+as plain types).  write_map takes one, load_map returns one."""
+
+
+def _plain(v, where):
+    """`v` as built-in types (what torch.load(weights_only=True) reads back); anything else raises ValueError naming `where`."""
+    if v is None or isinstance(v, (bool, int, float, str)):
+        return v
+    if isinstance(v, np.integer):
+        return int(v)
+    if isinstance(v, np.floating):
+        return float(v)
+    if isinstance(v, (list, tuple)):
+        return [_plain(x, f"{where}[{i}]") for i, x in enumerate(v)]
+    if isinstance(v, dict):
+        return {str(k): _plain(x, f"{where}.{k}") for k, x in v.items()}
+    raise ValueError(f"write_map: {where} is a {type(v).__name__}, not a plain type")
+
+
+def map_config(args):
+    """What a map file keeps of a run's configuration (load_config's namespace): criteria, tracker_specs, the mapper's voxel_size,
+    data_specs and dataset, as plain types."""
+    return _plain({"criteria": args.criteria, "tracker_specs": args.tracker_specs, "voxel_size": args.mapper_specs["voxel_size"],
+                   "data_specs": args.data_specs, "dataset": args.dataset}, "config")
+
+
+def write_map(path, saved):
+    """One torch.save file of `saved` (SavedMap) that torch.load(..., weights_only=True) reads: format, map (MapUpdater.state_dict()),
+    decoder ({"params": the flat fp32 parameters in state_dict() order, "decoder_specs"}), trajectory f64[S,4,4], scan_ids i64[S]
+    and config.  The file is written next to `path` and renamed over it, so a failed write leaves no partial map behind."""
+    traj = torch.as_tensor(np.asarray(saved.trajectory, dtype=np.float64)).clone()
+    ids = torch.as_tensor(np.asarray(saved.scan_ids, dtype=np.int64)).clone()
+    if traj.dim() != 3 or traj.shape[1:] != (4, 4) or traj.shape[0] < 1 or ids.shape != (traj.shape[0],):
+        raise ValueError(f"write_map: need trajectory [S,4,4] and scan_ids [S] with S >= 1, got {list(traj.shape)} and {list(ids.shape)}")
+    if not bool(torch.isfinite(traj).all()):
+        raise ValueError("write_map: the trajectory has non-finite poses")
+    config = _plain(dict(saved.config), "config")
+    missing = [k for k in CONFIG_KEYS if k not in config]
+    if missing:
+        raise ValueError(f"write_map: config lacks {', '.join(missing)}")
+    if float(config["voxel_size"]) != saved.map.voxel_size:
+        raise ValueError(f"write_map: config voxel_size {config['voxel_size']} is not the map's {saved.map.voxel_size}")
+    obj = {"format": MAP_FORMAT, "map": saved.map.state_dict(),
+           "decoder": {"params": _flat_decoder_state(saved.decoder).to("cpu", copy=True), "decoder_specs": _plain(dict(saved.decoder_specs), "decoder_specs")},
+           "trajectory": traj, "scan_ids": ids, "config": config}
+    tmp = f"{os.fspath(path)}.part"
+    torch.save(obj, tmp)
+    os.replace(tmp, path)
+
+
+def _decoder_size(specs):
+    """Number of parameters of Decoder(**specs), built on the meta device (no memory, no draw from torch's generator)."""
+    with torch.device("meta"):
+        return sum(p.numel() for p in Decoder(**specs).state_dict().values())
+
+
+def _check_map_file(obj):
+    """The checks of a map file above the map itself (from_state_dict checks that); the names of the failed ones."""
+    if not isinstance(obj, dict):
+        return ["a dict"]
+    missing = [k for k in MAP_KEYS if k not in obj]
+    if missing:
+        return ["keys " + ", ".join(missing)]
+    bad = []
+    if obj["format"] != MAP_FORMAT:
+        bad.append(f"format {obj['format']!r} (this version reads {MAP_FORMAT!r})")
+    if not isinstance(obj["map"], dict):
+        bad.append("map a dict")
+    dec = obj["decoder"]
+    if not isinstance(dec, dict) or not isinstance(dec.get("decoder_specs"), dict) or not isinstance(dec.get("params"), torch.Tensor):
+        bad.append("decoder a dict of params and decoder_specs")
+    elif dec["params"].dtype != torch.float32 or dec["params"].dim() != 1:
+        bad.append("decoder params a flat float32 tensor")
+    else:
+        try:
+            n = _decoder_size(dec["decoder_specs"])
+        except (TypeError, ValueError, NotImplementedError) as e:
+            bad.append(f"decoder_specs a supported decoder ({e})")
+        else:
+            if dec["params"].numel() != n:
+                bad.append(f"decoder params of {n} values for its decoder_specs (got {dec['params'].numel()})")
+            elif not bool(torch.isfinite(dec["params"]).all()):
+                bad.append("decoder params finite")
+    traj, ids = obj["trajectory"], obj["scan_ids"]
+    if not isinstance(traj, torch.Tensor) or traj.dtype != torch.float64:
+        bad.append("trajectory a float64 tensor")
+    elif traj.dim() != 3 or traj.shape[1:] != (4, 4) or traj.shape[0] < 1:
+        bad.append(f"trajectory of shape [S,4,4] with S >= 1 (got {list(traj.shape)})")
+    elif not bool(torch.isfinite(traj).all()):
+        bad.append("trajectory poses finite")
+    elif not torch.equal(traj[:, 3], torch.tensor([0.0, 0.0, 0.0, 1.0], dtype=torch.float64).expand(traj.shape[0], 4)):
+        bad.append("trajectory poses with last row 0 0 0 1")
+    if not isinstance(ids, torch.Tensor) or ids.dtype != torch.int64:
+        bad.append("scan_ids an int64 tensor")
+    elif isinstance(traj, torch.Tensor) and tuple(ids.shape) != (traj.shape[0],):
+        bad.append(f"scan_ids of shape [{traj.shape[0]}] (one per pose, got {list(ids.shape)})")
+    cfg = obj["config"]
+    if not isinstance(cfg, dict):
+        bad.append("config a dict")
+    else:
+        gone = [k for k in CONFIG_KEYS if k not in cfg]
+        if gone:
+            bad.append("config keys " + ", ".join(gone))
+        else:
+            for k in ("criteria", "tracker_specs", "data_specs"):
+                if not isinstance(cfg[k], dict):
+                    bad.append(f"config {k} a dict")
+            if cfg["dataset"] not in ("kitti", "maicity"):
+                bad.append(f"config dataset kitti or maicity (got {cfg['dataset']!r})")
+            vs = cfg["voxel_size"]
+            if isinstance(obj["map"], dict) and (not isinstance(vs, (int, float)) or vs != obj["map"].get("voxel_size")):
+                bad.append(f"config voxel_size equal to the map's (got {vs!r} and {obj['map'].get('voxel_size')!r})")
+    return bad
+
+
+def load_map(path, octree="host", device="cuda"):
+    """A map file (write_map, NeRFLOAM.save_map) -> SavedMap: the MapUpdater restored onto `octree` ("host" or "device",
+    MapUpdater.from_state_dict), a Decoder on `device` carrying the saved parameters, and the other fields.  A malformed file raises
+    ValueError naming the failed checks (a missing key, a wrong dtype or shape, a format mismatch, non-finite poses); a malformed map
+    inside it raises NerfLoamError (from_state_dict's checks)."""
+    try:
+        obj = torch.load(path, map_location="cpu", weights_only=True)
+    except (OSError, EOFError) as e:
+        raise ValueError(f"load_map: cannot read {path}: {e}") from e
+    except Exception as e:                  # noqa: BLE001 -- torch.load raises pickle / zip / runtime errors for a foreign file
+        raise ValueError(f"load_map: {path} is not a map file: {e}") from e
+    bad = _check_map_file(obj)
+    if bad:
+        raise ValueError(f"load_map: {path} is a malformed map file, failed checks: " + "; ".join(bad))
+    mu = MapUpdater.from_state_dict(obj["map"], device=device, octree=octree)
+    specs = dict(obj["decoder"]["decoder_specs"])
+    with torch.device("meta"):
+        decoder = Decoder(**specs)
+    decoder = load_flat_decoder_state(decoder.to_empty(device=device), obj["decoder"]["params"].to(device))
+    return SavedMap(mu, decoder, specs, obj["trajectory"], obj["scan_ids"], obj["config"])
+
+
+# ----------------------------------------------------------------------------------------------------------------------------
 # the whole system
 # ----------------------------------------------------------------------------------------------------------------------------
 def load_dataset(args):
@@ -604,6 +754,19 @@ class NeRFLOAM:
         self.schedule = run_pipeline(self.tracker, self.mapper, self.streams)
         torch.cuda.synchronize()
         return self.summary((time.perf_counter() - t0) * 1e3)
+
+    def saved_map(self):
+        """The finished run's map as a SavedMap over the live objects (no copy): the mapper's MapUpdater and decoder after the final
+        refinement (the map final_mesh.ply was made from), the trajectory frame_poses.txt holds and the scans' ids."""
+        m = self.mapper
+        if m.map_state is None or m.trajectory.frame_poses or not m.trajectory.final_poses:
+            raise RuntimeError("save_map: the run has not finished (call run() first)")
+        return SavedMap(m.map, m.decoder, dict(self.args.decoder_specs), np.stack(m.trajectory.final_poses).astype(np.float64),
+                        np.asarray(m.scan_ids, dtype=np.int64), map_config(self.args))
+
+    def save_map(self, path):
+        """Writes the finished run's map to one file (write_map); localise.Localiser and load_map read it."""
+        write_map(path, self.saved_map())
 
     def summary(self, wall_ms):
         times = {**self.tracker.times, **self.mapper.times}

@@ -2,10 +2,12 @@
 CUDA streams (slam.NeRFLOAM), writing mesh/*.ply and misc/frame_poses*.txt under the output directory.
 
     python scripts/run_slam.py CONFIG [--data DIR] [--out DIR] [--selection current|previous|overlap] [--init-calls 12]
+                               [--save-map PATH]
 
 CONFIG is the reference's YAML layout (base_config merged).  --data replaces data_specs.data_path; --out defaults to
 log_dir/exp_name/<time> like src/loggers.py:17-18.  Prints a JSON summary: scans, keyframes, milliseconds per scan per stage (host
-wall-clock of each role's steps), the wall time and the refinement times.
+wall-clock of each role's steps), the wall time and the refinement times.  --save-map also writes the finished run's map, decoder,
+trajectory and settings to PATH (NeRFLOAM.save_map), which scripts/localise.py localises later drives in.
 """
 import argparse, json, os, sys
 from datetime import datetime
@@ -21,13 +23,18 @@ def main():
     ap.add_argument("--out", default=None, help="output directory (default: log_dir/exp_name/<time>)")
     ap.add_argument("--selection", default="current", choices=nl.slam.SELECTIONS, help="the mapping window (reference: current)")
     ap.add_argument("--init-calls", type=int, default=12, help="mapping calls on the first scan")
+    ap.add_argument("--save-map", default=None, metavar="PATH", help="write the finished run's map to PATH (slam.NeRFLOAM.save_map)")
     a = ap.parse_args()
     cfg = nl.slam.load_config(a.config)
     if a.data is not None:
         cfg.data_specs["data_path"] = a.data
     out = a.out or os.path.join(getattr(cfg, "log_dir", "./logs"), getattr(cfg, "exp_name", "run"),
                                 datetime.strftime(datetime.now(), "%Y-%m-%d-%H-%M-%S"))
-    summary = nl.slam.NeRFLOAM(cfg, out, selection=a.selection, init_calls=a.init_calls).run()
+    slam = nl.slam.NeRFLOAM(cfg, out, selection=a.selection, init_calls=a.init_calls)
+    summary = slam.run()
+    if a.save_map is not None:
+        slam.save_map(a.save_map)
+        summary["map_file"] = a.save_map
     print(json.dumps(summary))
 
 
