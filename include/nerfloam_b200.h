@@ -464,11 +464,6 @@ NL_API int nl_adam_f32(int64_t n, float *d_param, const float *d_grad, float *d_
                 double beta2, double eps, int step, void *stream);
 NL_API int nl_adam_bf16(int64_t n, uint16_t *d_param, const float *d_grad_f32, uint16_t *d_m, uint16_t *d_v, double lr,
                  double beta1, double beta2, double eps, int step, void *stream);
-/* nl_adam_f32 with the step count in device memory: *d_step is incremented, then used -- so the pair of launches can be
- * captured in a CUDA graph and replayed (the tracking loop, render_helpers.py:452-510, is launch-bound). */
-NL_API int nl_adam_f32_devstep(int64_t n, float *d_param, const float *d_grad, float *d_m, float *d_v, double lr, double beta1,
-                        double beta2, double eps, int32_t *d_step, void *stream);
-
 
 /* ============================================================================================
  * 8. Device-side iteration control: lets a whole optimisation call (render_helpers.py:356-423 / :452-510) run without a

@@ -135,7 +135,6 @@ _SIGNATURES = {
                                vp, C.c_int32, vp, C.c_int32, vp]),
     "nl_select_rays": (C.c_int, [C.c_int, C.c_int, C.c_int, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "nl_adam_f32": (C.c_int, [C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, vp]),
-    "nl_adam_f32_devstep": (C.c_int, [C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),
     "nl_adam_bf16": (C.c_int, [C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, vp]),
     "nl_iter_status": (C.c_int, [vp, vp, vp, vp]),
     "nl_adam_f32_ctl": (C.c_int, [C.c_int64, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),

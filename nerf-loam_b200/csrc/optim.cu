@@ -44,27 +44,6 @@ __global__ void k_adam_bf16(long long n, uint16_t *__restrict__ p, const float *
     v[i] = nl_f32_to_bf16(vi);
 }
 
-// Same update with the step count read from device memory (a CUDA graph replays the launch with fixed arguments): the bias
-// corrections are evaluated per thread in double like the host path.  *step is advanced by k_step_inc in the same graph.
-__global__ void k_adam_f32_dev(long long n, float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
-                               float *__restrict__ v, double lr, double beta1, double beta2, float eps, const int32_t *__restrict__ step) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int t = *step;
-    const double bc1 = 1.0 - pow(beta1, (double)t), bc2 = 1.0 - pow(beta2, (double)t);
-    const float w1 = (float)(1.0 - beta1), b2 = (float)beta2, w2 = (float)(1.0 - beta2), step_size = (float)(lr / bc1), bc2_sqrt = (float)sqrt(bc2);
-    const float gi = g[i];
-    const float mi = __fadd_rn(m[i], __fmul_rn(w1, __fsub_rn(gi, m[i])));
-    float vi = __fmul_rn(v[i], b2);
-    vi = __fadd_rn(vi, __fmul_rn(__fmul_rn(w2, gi), gi));
-    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vi), bc2_sqrt), eps);
-    p[i] = __fadd_rn(p[i], __fmul_rn(-step_size, __fdiv_rn(mi, denom)));
-    m[i] = mi;
-    v[i] = vi;
-}
-
-__global__ void k_step_inc(int32_t *step) { *step += 1; }
-
 // Adam driven by the device-side iteration control block (nl_iter_status): the step count is ctl[NL_CTL_ADAM_STEP] and the whole
 // update is skipped when ctl[NL_CTL_SKIP_NOW] is set -- the reference `continue`s past optim.step() when an iteration hits nothing
 // (render_helpers.py:405-409), and a skipped step advances neither the moments nor Adam's step count.
@@ -112,17 +91,6 @@ extern "C" int nl_adam_bf16(int64_t n, uint16_t *p, const float *g, uint16_t *m,
                                                                      (float)(1.0 - beta2), (float)eps, (float)(lr / bc1),
                                                                      (float)std::sqrt(bc2));
     NL_CHECK_LAUNCH("nl_adam_bf16");
-    return NL_OK;
-}
-
-extern "C" int nl_adam_f32_devstep(int64_t n, float *p, const float *g, float *m, float *v, double lr, double beta1, double beta2,
-                                   double eps, int32_t *d_step, void *stream) {
-    if (n < 0) return nl_set_error("nl_adam_f32_devstep: bad arguments");
-    if (n == 0) return NL_OK;
-    if (!p || !g || !m || !v || !d_step) return nl_set_error("nl_adam_f32_devstep: null pointer");
-    k_step_inc<<<1, 1, 0, (cudaStream_t)stream>>>(d_step);
-    k_adam_f32_dev<<<nl_div_up(n, 256), 256, 0, (cudaStream_t)stream>>>(n, p, g, m, v, lr, beta1, beta2, (float)eps, d_step);
-    NL_CHECK_LAUNCH("nl_adam_f32_devstep");
     return NL_OK;
 }
 

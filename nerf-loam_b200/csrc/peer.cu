@@ -16,6 +16,7 @@
 // arithmetic is done once instead of W times, and one kernel launch replaces two.  The caller orders it between two
 // symmetric-memory barriers (all scatters finished / all tables written); see dist.PeerReduceAdam.
 #include "nl_cuda.cuh"
+#include "adam.cuh"
 
 namespace {
 
@@ -28,27 +29,6 @@ __device__ __forceinline__ float4 mc_ld_reduce_f32x4(const float *mc) {
 __device__ __forceinline__ void mc_st_b32x4(void *mc, uint4 v) {
     asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(mc), "f"(__uint_as_float(v.x)), "f"(__uint_as_float(v.y)),
                  "f"(__uint_as_float(v.z)), "f"(__uint_as_float(v.w)) : "memory");
-}
-
-struct AdamConst {
-    float w1, b2, w2, eps, step_size, bc2_sqrt;
-};
-__device__ __forceinline__ AdamConst adam_const(double lr, double beta1, double beta2, float eps, int t) {
-    const double bc1 = 1.0 - pow(beta1, (double)t), bc2 = 1.0 - pow(beta2, (double)t);
-    return {(float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), eps, (float)(lr / bc1), (float)sqrt(bc2)};
-}
-// one element of torch.optim.Adam on a bf16 tensor: every intermediate rounded to bf16 where torch's per-op kernels round (optim.cu)
-__device__ __forceinline__ void adam_bf16(const AdamConst &c, float g32, uint16_t &p, uint16_t &m, uint16_t &v) {
-    const float gi = nl_round_bf16(g32);
-    float mi = nl_bf16_to_f32(m), vi = nl_bf16_to_f32(v), pi = nl_bf16_to_f32(p);
-    mi = nl_round_bf16(__fadd_rn(mi, __fmul_rn(c.w1, __fsub_rn(gi, mi))));
-    vi = nl_round_bf16(__fmul_rn(vi, c.b2));
-    vi = nl_round_bf16(__fadd_rn(vi, __fmul_rn(__fmul_rn(c.w2, gi), gi)));
-    float d = nl_round_bf16(__fsqrt_rn(vi));
-    d = nl_round_bf16(__fdiv_rn(d, c.bc2_sqrt));
-    d = nl_round_bf16(__fadd_rn(d, c.eps));
-    pi = nl_round_bf16(__fadd_rn(pi, __fmul_rn(-c.step_size, __fdiv_rn(mi, d))));
-    p = nl_f32_to_bf16(pi); m = nl_f32_to_bf16(mi); v = nl_f32_to_bf16(vi);
 }
 
 // One thread per 8 consecutive elements (half an embedding row): 2 x 16 B of reduced gradient in, 16 B of parameters out.
@@ -89,12 +69,12 @@ __global__ void __launch_bounds__(256) k_reduce_adam_bf16(long long e0, long lon
             g[0] += a.x; g[1] += a.y; g[2] += a.z; g[3] += a.w; g[4] += b.x; g[5] += b.y; g[6] += b.z; g[7] += b.w;
         }
     }
-    const AdamConst c = adam_const(lr, beta1, beta2, eps, ctl[NL_CTL_ADAM_STEP]);
+    const NlAdamConst c = nl_adam_const(lr, beta1, beta2, eps, ctl[NL_CTL_ADAM_STEP]);
     uint4 pw = *reinterpret_cast<const uint4 *>(param_peers[rank] + e);
     uint4 mw = *reinterpret_cast<const uint4 *>(m + e), vw = *reinterpret_cast<const uint4 *>(v + e);
     uint16_t *p16 = reinterpret_cast<uint16_t *>(&pw), *m16 = reinterpret_cast<uint16_t *>(&mw), *v16 = reinterpret_cast<uint16_t *>(&vw);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) adam_bf16(c, g[i], p16[i], m16[i], v16[i]);
+    for (int i = 0; i < 8; ++i) nl_adam_bf16_elem(c, g[i], p16[i], m16[i], v16[i]);
     *reinterpret_cast<uint4 *>(m + e) = mw;
     *reinterpret_cast<uint4 *>(v + e) = vw;
     if (MC) {

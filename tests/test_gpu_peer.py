@@ -1,8 +1,9 @@
 """Single-GPU test of the fused reduce-scatter -> Adam -> all-gather kernel (csrc/peer.cu, dist.PeerReduceAdam) and of the
 symmetric-memory statistics exchange (dist.PeerStats) in a 1-rank process group: the kernels then read / write their "peers"
-through the same pointer tables and must reproduce nl_adam_bf16_ctl and nl_stats_unpack exactly.  The W > 1 behaviour (NVLS
-multicast, bit-identity with NCCL all-reduce + Adam, identical replicas) is checked by scripts/test_peer.py under torchrun
-and by bench.py's strong-scaling block on every multi-GPU run."""
+through the same pointer tables and must reproduce nl_adam_bf16_ctl and nl_stats_unpack exactly.  The plain P2P path at W > 1
+(rank-ordered sums, slices, identical replicas) is checked on one GPU by tests/test_gpu_iteration_tail.py; NVLS multicast and
+bit-identity with NCCL all-reduce + Adam are checked by scripts/test_peer.py under torchrun and by bench.py's strong-scaling block
+on every multi-GPU run."""
 import os
 import socket
 
