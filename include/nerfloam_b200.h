@@ -544,8 +544,10 @@ NL_API int nl_peer_reduce_adam_bf16(int64_t n_elems, int rank, int world, const 
  *     lattice edge); voxels are independent (vertices on shared voxel faces are not merged, exactly like the reference's loop,
  *     which offsets each voxel's faces by the running vertex count, mesh_util.py:160-163).
  *     Two calls: nl_mc_count fills per-voxel counts, their exclusive scans and d_totals = {n_vertices, n_triangles} (int64[2]);
- *     the caller allocates the outputs and calls nl_mc_emit.
- *     vertex = ((lattice position) / (res - 1) - 0.5) * voxel_size + centres[vox_ids ? vox_ids[v] : v]   (mesh_util.py:149-161)
+ *     the caller allocates the outputs and calls nl_mc_emit.  Offsets and vertex ids are int32: when a total exceeds INT32_MAX
+ *     the offsets have wrapped and the mesh cannot be emitted (nl_mc_emit refuses capacities above INT32_MAX).
+ *     vertex = ((lattice position) / (res - 1) - 0.5) * voxel_size + centres[vox_ids ? vox_ids[v] : v]   (mesh_util.py:149-161),
+ *     each of the four steps rounded separately in fp32 (no FMA contraction).  NaN lattice values count as outside (not < 0).
  *     Triangles are wound so that the normal points towards increasing SDF.
  * ============================================================================================ */
 NL_API int nl_mc_count(int32_t n_vox, int32_t res, const float *d_sdf, int32_t *d_nvert, int32_t *d_ntri, int32_t *d_voff, int32_t *d_toff,

@@ -289,14 +289,16 @@ __global__ void __launch_bounds__(MC_THREADS) k_mc_emit(int n_vox, int res, floa
         for (int q = 0; q < w; ++q) pre += s_warp[q];
         const int rank = pre + __popc(bal & ((1u << lane) - 1u));
         if (id < nedge) s_rank[id] = cross ? (int16_t)rank : (int16_t)-1;
-        if (cross && (int64_t)(vbase + rank) < vcap) {
+        if (cross && (int64_t)vbase + rank < vcap) {
             const float tt = s0 / (s0 - s1);                                  // zero crossing between the two lattice points
             float p[3] = {(float)i, (float)j, (float)k};
             p[a] += tt;
             float *o = verts + (size_t)(vbase + rank) * 3;
-            o[0] = (p[0] * inv - 0.5f) * voxel_size + cx;                      // mesh_util.py:149-161: spacing 1/(res-1), -0.5, * voxel_size, + centre
-            o[1] = (p[1] * inv - 0.5f) * voxel_size + cy;
-            o[2] = (p[2] * inv - 0.5f) * voxel_size + cz;
+            // mesh_util.py:149-161: spacing 1/(res-1), -0.5, * voxel_size, + centre -- four separately rounded steps, written
+            // with explicit roundings so that nvcc does not contract them into two FMAs (tests/mesh_ref.py restates them)
+            o[0] = __fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(p[0], inv), 0.5f), voxel_size), cx);
+            o[1] = __fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(p[1], inv), 0.5f), voxel_size), cy);
+            o[2] = __fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(p[2], inv), 0.5f), voxel_size), cz);
         }
         __syncthreads();
         if (t == 0) { int tot = 0; for (int q = 0; q < MC_THREADS / 32; ++q) tot += s_warp[q]; s_carry += tot; }
@@ -325,9 +327,9 @@ __global__ void __launch_bounds__(MC_THREADS) k_mc_emit(int n_vox, int res, floa
         __syncthreads();
         int pre = s_carry;
         for (int q = 0; q < w; ++q) pre += s_warp[q];
-        int out = tbase + pre + incl - nt;
+        int64_t out = (int64_t)tbase + pre + incl - nt;
         for (int q = 0; q < nt; ++q, ++out) {
-            if ((int64_t)out >= tcap) break;
+            if (out >= tcap) break;
 #pragma unroll
             for (int r = 0; r < 3; ++r) {
                 const int e = c_mc.tri[cfg][3 * q + r];
@@ -368,7 +370,8 @@ extern "C" int nl_mc_count(int32_t n_vox, int32_t res, const float *d_sdf, int32
                            int64_t *d_totals, void *stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (n_vox < 0 || res < 2 || res > MC_MAX_RES) return nl_set_error("nl_mc_count: need n_vox >= 0 and 2 <= res <= 16");
-    if (!d_sdf || !d_nvert || !d_ntri || !d_voff || !d_toff || !d_totals) return nl_set_error("nl_mc_count: null pointer");
+    // no voxels (an empty map): nothing is read or written but the totals, so the per-voxel pointers may be null
+    if ((n_vox > 0 && (!d_sdf || !d_nvert || !d_ntri || !d_voff || !d_toff)) || !d_totals) return nl_set_error("nl_mc_count: null pointer");
     if (int rc = upload_tables()) return rc;
     if (n_vox > 0) k_mc_count<<<n_vox, MC_THREADS, 0, stream>>>(n_vox, res, d_sdf, d_nvert, d_ntri);
     k_mc_scan<<<1, 1024, 0, stream>>>(n_vox, d_nvert, d_ntri, d_voff, d_toff, d_totals);
@@ -381,8 +384,10 @@ extern "C" int nl_mc_emit(int32_t n_vox, int32_t res, float voxel_size, const fl
                           int32_t *d_faces, void *stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (n_vox < 0 || res < 2 || res > MC_MAX_RES) return nl_set_error("nl_mc_emit: need n_vox >= 0 and 2 <= res <= 16");
-    if (!d_sdf || !d_centres || !d_voff || !d_toff || (vert_capacity > 0 && !d_verts) || (tri_capacity > 0 && !d_faces))
+    if ((n_vox > 0 && (!d_sdf || !d_centres || !d_voff || !d_toff)) || (vert_capacity > 0 && !d_verts) || (tri_capacity > 0 && !d_faces))
         return nl_set_error("nl_mc_emit: null pointer");
+    // offsets and face entries are int32 vertex / triangle ids: a mesh with more than INT32_MAX of either cannot be written
+    if (vert_capacity > INT32_MAX || tri_capacity > INT32_MAX) return nl_set_error("nl_mc_emit: capacities above INT32_MAX");
     if (int rc = upload_tables()) return rc;
     if (n_vox > 0)
         k_mc_emit<<<n_vox, MC_THREADS, 0, stream>>>(n_vox, res, voxel_size, d_sdf, d_centres, d_vox_ids, d_voff, d_toff, vert_capacity, tri_capacity,

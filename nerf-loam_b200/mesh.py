@@ -12,11 +12,14 @@ import torch
 from . import _capi
 from .engine import MapState
 
+INT32_MAX = 2 ** 31 - 1
+
 
 @torch.no_grad()
 def marching_cubes_device(sdf, centres, voxel_size, vox_ids=None):
     """sdf f32[n,res,res,res] (CUDA, lattice layout of get_scores), centres f32[N,3] (CUDA), vox_ids i32[n] rows of `centres`
-    (None: row v) -> (verts f32[V,3], faces i32[T,3]) on the device.  One 16-byte read-back (the totals) to size the outputs."""
+    (None: row v) -> (verts f32[V,3], faces i32[T,3]) on the device.  One 16-byte read-back (the totals) to size the outputs.
+    Raises ValueError, before allocating them, when either total is above INT32_MAX (vertex ids and offsets are int32)."""
     if not sdf.is_cuda:
         raise RuntimeError("marching cubes runs on the GPU only (no CPU fallback)")
     sdf = sdf.float().contiguous()
@@ -32,6 +35,9 @@ def marching_cubes_device(sdf, centres, voxel_size, vox_ids=None):
     _capi.check(lib.nl_mc_count(n, res, _capi.ptr(sdf), _capi.ptr(counts[0]), _capi.ptr(counts[1]), _capi.ptr(counts[2]), _capi.ptr(counts[3]),
                                 _capi.ptr(totals), st), "nl_mc_count")
     nv, nt = (int(x) for x in totals.tolist())
+    if max(nv, nt) > INT32_MAX:
+        raise ValueError(f"marching cubes: {nv} vertices and {nt} triangles; vertex ids and offsets are int32, so neither may "
+                         f"exceed INT32_MAX = {INT32_MAX} (extract fewer voxels per call, or at a lower res)")
     verts = torch.empty((nv, 3), dtype=torch.float32, device=dev)
     faces = torch.empty((nt, 3), dtype=torch.int32, device=dev)
     _capi.check(lib.nl_mc_emit(n, res, float(voxel_size), _capi.ptr(sdf), _capi.ptr(centres), _capi.ptr(vox_ids), _capi.ptr(counts[2]),

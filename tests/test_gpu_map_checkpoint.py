@@ -139,10 +139,17 @@ def test_restored_map_renders_identically_and_runs_the_captured_graphs(nl, octre
 
 
 def _trace(fn):
+    """(fn(), its host-to-device and device-to-host copies) from a profiler trace of one call.  The profiler runs a warm-up call
+    of fn first and records the second: in a process that has already been profiled, the first GPU activity records of a new
+    session can be missing (on an H100 80GB HBM3 after the preceding GPU test files, the trace lacked the first two host-to-device
+    copies although the runtime trace showed every cudaMemcpyAsync), and a missing copy must not be mistaken for one not made."""
     torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]) as prof:
-        out = fn()
-        torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA],
+                                schedule=torch.profiler.schedule(wait=0, warmup=1, active=1, repeat=1)) as prof:
+        for _ in range(2):
+            out = fn()
+            torch.cuda.synchronize()
+            prof.step()
     with tempfile.TemporaryDirectory() as d:
         f = os.path.join(d, "trace.json")
         prof.export_chrome_trace(f)

@@ -44,32 +44,37 @@ def _boundary(tris):
 
 
 def test_marching_cubes_vs_python_restatement(nl):
+    """Around 2000 m (one fp32 ulp is 1.2e-4 m) and around 0.15 m, where an FMA-contracted vertex formula would differ from the
+    separately rounded one in the last bit of a fifth or more of the vertices."""
     import itertools as it
     from oracle import mc as OM
-    sdf, centres, c, r = _sphere_block(res=6, nvox=2)
     res = 6
-    verts, faces = nl.mesh.marching_cubes_device(sdf.cuda(), centres.cuda(), 0.3)
-    verts, faces = verts.cpu().numpy(), faces.cpu().numpy()
-    vo, to = 0, 0
-    for v in range(sdf.shape[0]):
-        want_v, _ = OM.marching_cubes_voxel(sdf[v].numpy(), centres[v].numpy(), 0.3)
-        nv = len(want_v)
-        got_v = verts[vo:vo + nv]
-        # vertex set: bit-exact (same fp32 formula), as a set -- the kernel orders a voxel's vertices by lattice-edge id
-        assert sorted(map(tuple, got_v.tolist())) == sorted(tuple(np.asarray(p, np.float32).tolist()) for p in want_v.values())
-        pos = {k: tuple(np.asarray(p, np.float32).tolist()) for k, p in want_v.items()}
-        neg = sdf[v].numpy() < 0
-        # cell by cell (the kernel emits a voxel's triangles in cell order): the same oriented polygons
-        for ci, cj, ck in it.product(range(res - 1), repeat=3):
-            neg8 = {(x, y, z): bool(neg[ci + x, cj + y, ck + z]) for x, y, z in it.product((0, 1), repeat=3)}
-            want = [tuple(pos[(a, ci + x, cj + y, ck + z)] for (a, x, y, z) in t) for t in OM.cell_polygons(neg8)]
-            f = faces[to:to + len(want)]
-            assert len(want) == 0 or (f.min() >= vo and f.max() < vo + nv)               # a voxel's faces index its own welded vertices
-            got = [tuple(tuple(verts[i].tolist()) for i in t) for t in f]
-            assert _boundary(got) == _boundary(want), (v, ci, cj, ck)
-            to += len(want)
-        vo += nv
-    assert vo == verts.shape[0] and to == faces.shape[0]
+    for centre in ((2000.41, 2000.38, 2000.47), (0.15, 0.11, 0.17)):
+        sdf, centres, c, r = _sphere_block(res=res, nvox=2, centre=centre)
+        verts, faces = nl.mesh.marching_cubes_device(sdf.cuda(), centres.cuda(), 0.3)
+        verts, faces = verts.cpu().numpy(), faces.cpu().numpy()
+        vo, to = 0, 0
+        for v in range(sdf.shape[0]):
+            want_v, _ = OM.marching_cubes_voxel(sdf[v].numpy(), centres[v].numpy(), 0.3)
+            nv = len(want_v)
+            got_v = verts[vo:vo + nv]
+            # vertices bit-exact (same fp32 formula) and in the same order: the kernel's lattice-edge ids, the oracle's edge loop
+            want_arr = np.array([np.asarray(p, np.float32) for p in want_v.values()], np.float32).reshape(-1, 3)
+            assert np.array_equal(got_v.view(np.uint32), want_arr.view(np.uint32)), \
+                (centre, v, int((got_v != want_arr).any(1).sum()), nv)
+            pos = {k: tuple(np.asarray(p, np.float32).tolist()) for k, p in want_v.items()}
+            neg = sdf[v].numpy() < 0
+            # cell by cell (the kernel emits a voxel's triangles in cell order): the same oriented polygons
+            for ci, cj, ck in it.product(range(res - 1), repeat=3):
+                neg8 = {(x, y, z): bool(neg[ci + x, cj + y, ck + z]) for x, y, z in it.product((0, 1), repeat=3)}
+                want = [tuple(pos[(a, ci + x, cj + y, ck + z)] for (a, x, y, z) in t) for t in OM.cell_polygons(neg8)]
+                f = faces[to:to + len(want)]
+                assert len(want) == 0 or (f.min() >= vo and f.max() < vo + nv)           # a voxel's faces index its own welded vertices
+                got = [tuple(tuple(verts[i].tolist()) for i in t) for t in f]
+                assert _boundary(got) == _boundary(want), (centre, v, ci, cj, ck)
+                to += len(want)
+            vo += nv
+        assert vo == verts.shape[0] and to == faces.shape[0]
 
 
 def test_sphere_mesh_properties(nl):
