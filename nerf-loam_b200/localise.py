@@ -16,11 +16,17 @@
     reference doubles the rate for scan indices below 2) and replayed for every scan.
   * Per scan, the loss and the fraction of rays that hit the map come from one score_poses(..., deterministic=True) call at the final
     pose, on rays spread evenly over the scan: track_frame only reports a loss through loss_log, which turns its captured graph off.
+  * Recovery (opt-in, config key "recovery_specs"; DESIGN.md §11.5): a tracked scan whose hit fraction or loss fails the lost rule
+    (is_lost) is re-placed by score.relocalise around the constant-velocity guess, then, at most once every global_interval scans
+    while scans stay lost, by the first scan's search over the whole saved trajectory.  A re-placement counts only if its own score
+    passes the rule; otherwise the scan keeps its tracked pose and is reported lost.  After either, the motion model restarts from
+    the last accepted scan.  The map is frozen, so a wrong decision changes one reported pose and nothing else.
 
-Not covered: recovering a scan that is lost partway through, updating the map, loop closure.
+Not covered: updating the map, loop closure.
 """
 import contextlib
 import copy
+import math
 import os
 import time
 from collections import namedtuple
@@ -33,14 +39,53 @@ from . import _capi
 from . import render_helpers as rh
 from .frame import POSE_OFFSET, LidarFrame
 from .globalloc import relocalise_global
-from .score import score_poses
+from .score import relocalise, score_poses
 from .se3pose import OptimizablePose
-from .slam import SavedMap, Tracking, _merge, load_map, write_poses
+from .slam import SavedMap, Tracking, _merge, constant_velocity_guess, load_map, write_poses
 
 # relocalise_global's settings for the first scan (config key "global_specs" overrides them): the search of DESIGN.md §3.4 around
 # every saved pose, and its refinement with 1024 rays, 150 iterations at rate 0.01 (the rate Adam steps at, whatever the scan's index)
 GLOBAL_SPECS = dict(radius=5.0, xy_step=1.0, yaw_steps=72, n_points=512, n_candidates=4096, n_seeds=4, N_rays=1024, refine_iterations=150,
                     learning_rate=0.01)
+
+# the lost rule's settings (config key "recovery_specs" turns recovery on and overrides them; DESIGN.md §11.5 says what they rest on):
+# a scan is lost when its hit fraction is below lost_hit_fraction or its loss exceeds lost_loss_ratio x the median loss of the last
+# HISTORY accepted scans; while scans stay lost, the global search runs at most once every global_interval scans
+RECOVERY_SPECS = dict(lost_hit_fraction=0.5, lost_loss_ratio=3.0, global_interval=5)
+HISTORY = 10
+STATUSES = ("tracked", "local", "global", "lost")
+_NOT_PER_SCAN = ("place", "polish", "recover_local", "recover_global")          # Localiser.times entries summary() reports apart
+
+
+def recovery_specs(specs):
+    """RECOVERY_SPECS with `specs` merged over them, checked: ValueError naming an unknown key or a value out of range."""
+    if not isinstance(specs, dict):
+        raise ValueError(f"recovery_specs must be a dict, got {specs!r}")
+    out = dict(RECOVERY_SPECS)
+    for k, v in specs.items():
+        if k not in RECOVERY_SPECS:
+            raise ValueError(f"recovery_specs: unknown key {k!r} (known: {', '.join(RECOVERY_SPECS)})")
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)) or not math.isfinite(float(v)):
+            raise ValueError(f"recovery_specs: {k} must be a finite number, got {v!r}")
+        out[k] = v
+    if not 0.0 <= float(out["lost_hit_fraction"]) <= 1.0:
+        raise ValueError(f"recovery_specs: lost_hit_fraction must lie in [0, 1], got {out['lost_hit_fraction']}")
+    if not float(out["lost_loss_ratio"]) >= 1.0:
+        raise ValueError(f"recovery_specs: lost_loss_ratio must be >= 1 (below 1 it flags healthy scans), got {out['lost_loss_ratio']}")
+    if int(out["global_interval"]) != out["global_interval"] or int(out["global_interval"]) < 1:
+        raise ValueError(f"recovery_specs: global_interval must be an integer >= 1, got {out['global_interval']}")
+    return {"lost_hit_fraction": float(out["lost_hit_fraction"]), "lost_loss_ratio": float(out["lost_loss_ratio"]),
+            "global_interval": int(out["global_interval"])}
+
+
+def is_lost(loss, hit_fraction, accepted_losses, specs):
+    """The lost rule: True when the loss is not finite, the hit fraction is below specs["lost_hit_fraction"], or the loss exceeds
+    specs["lost_loss_ratio"] x the median of the last HISTORY entries of accepted_losses (the losses of the accepted scans so far, in
+    order; with none, only the first two tests apply)."""
+    if not math.isfinite(loss) or hit_fraction < specs["lost_hit_fraction"]:
+        return True
+    window = list(accepted_losses)[-HISTORY:]
+    return bool(window) and loss > specs["lost_loss_ratio"] * float(np.median(window))
 
 
 def _rate_argument(rate, index):
@@ -50,10 +95,18 @@ def _rate_argument(rate, index):
     return rate / 2 if index < 2 else rate * 3
 
 
-Localisation = namedtuple("Localisation", ["scan_ids", "poses", "loss", "hit_fraction", "placement"])
+def _cpu_pose(pose):
+    p = OptimizablePose(pose.data.detach().cpu().float().clone())
+    p.requires_grad_(False)
+    return p
+
+
+Localisation = namedtuple("Localisation", ["scan_ids", "poses", "loss", "hit_fraction", "placement", "status"])
 Localisation.__doc__ = """Localiser.run's result, per scan in order: scan_ids i64[S], poses f64[S,4,4] in the map frame without POSE_OFFSET
-(what frame_poses.txt holds), loss f64[S] and hit_fraction f64[S] (score_poses at the final pose), and placement: the first scan's
-globalloc.GlobalResult (None when an init_pose was given)."""
+(what frame_poses.txt holds), loss f64[S] and hit_fraction f64[S] (score_poses at the final pose), placement: the first scan's
+globalloc.GlobalResult (None when an init_pose was given), and status: with recovery on, a list of S codes from STATUSES ("tracked":
+the tracker's pose passed the lost rule, "local" / "global": re-placed by that step, "lost": nothing passed, the tracked pose is
+kept; the first scan is "tracked"), None with recovery off."""
 
 
 class FrozenMap:
@@ -77,10 +130,11 @@ class Localiser:
     data_stream: a loader with __len__ and __getitem__ -> (index, points, pointsCos, pose or None) like dataset.<name>.DataLoader;
     a scan that comes with a pose is passed through untracked, as the run's tracker does (build the loader with use_gt=False).
     config: overrides merged over the file's config, e.g. {"tracker_specs": {"num_iterations": 50}} or {"global_specs": {...}}
-    (relocalise_global's settings, GLOBAL_SPECS); voxel_size is the map's and cannot change.
-    generator: a CPU torch.Generator every draw comes from (tracking's, and a seed for the first scan's search, which runs under a
-    forked torch RNG); None draws from torch's global generators.  octree: where a map file is restored ("host" or "device").
-    out_dir: where run() writes frame_poses.txt (None: nowhere)."""
+    (relocalise_global's settings, GLOBAL_SPECS); voxel_size is the map's and cannot change.  {"recovery_specs": {...}} turns
+    recovery of lost scans on (RECOVERY_SPECS; {} for the defaults); without the key run() does what it did before recovery existed.
+    generator: a CPU torch.Generator every draw comes from (tracking's, and a seed for each search -- the first scan's and every
+    recovery's -- which runs under a forked torch RNG); None draws from torch's global generators.  octree: where a map file is restored
+    ("host" or "device").  out_dir: where run() writes frame_poses.txt, and frame_status.txt with recovery on (None: nowhere)."""
 
     def __init__(self, saved, data_stream, config=None, generator=None, octree="host", out_dir=None):
         if not isinstance(saved, SavedMap):
@@ -98,6 +152,7 @@ class Localiser:
                                     tracker_specs={"start_frame": 0, "end_frame": -1, "read_offset": 1, **cfg["tracker_specs"]},
                                     mapper_specs={"voxel_size": float(cfg["voxel_size"])})
         self.global_specs = {**GLOBAL_SPECS, **cfg.get("global_specs", {})}
+        self.recovery = recovery_specs(cfg["recovery_specs"]) if "recovery_specs" in cfg else None
         self.map_state = saved.map.map_states["_mapstate"]
         self.frozen = FrozenMap(self.map_state, saved.decoder)
         self.tracker = Tracking(self.args, data_stream, self.frozen, generator)
@@ -128,6 +183,23 @@ class Localiser:
             frame.pose = OptimizablePose.from_matrix(T.float())
             frame.pose.requires_grad_(False)
             return None
+        res, pose, search_ms, polish_ms = self._search(frame)
+        self.times["place"] = [search_ms]
+        if pose is None:
+            raise _capi.NerfLoamError(f"Localiser: scan {frame.index} could not be placed: no placement within "
+                                      f"{self.global_specs['radius']} m of the saved trajectory hits the map")
+        self.times["polish"] = [polish_ms]
+        frame.pose = pose
+        return res
+
+    def _tracking_kw(self):
+        tr = self.tracker
+        return dict(step_size=tr.step_size, truncation=tr.sdf_truncation, max_voxel_hit=tr.max_voxel_hit, max_distance=tr.max_distance)
+
+    def _search(self, frame):
+        """The search with no pose guess: relocalise_global anchored on every saved pose (global_specs), then track_frame from its
+        placement.  Returns (GlobalResult, the pose as a CPU OptimizablePose or None when no placement hits the map, search ms,
+        tracking ms or None); frame.pose is not touched."""
         tr = self.tracker
         g = dict(self.global_specs)
         search = {k: g.pop(k) for k in ("radius", "xy_step", "yaw_steps", "n_points", "n_candidates", "n_seeds") if k in g}
@@ -135,12 +207,10 @@ class Localiser:
         t0 = time.perf_counter()
         with self._rng():
             res = relocalise_global(frame, self.map_state, self.saved.decoder, tr.loss_criteria, tr.voxel_size, anchors=self.anchors, **search,
-                                    step_size=tr.step_size, truncation=tr.sdf_truncation, max_voxel_hit=tr.max_voxel_hit,
-                                    max_distance=tr.max_distance, **g)
-        self.times["place"] = [(time.perf_counter() - t0) * 1e3]
+                                    **self._tracking_kw(), **g)
+        search_ms = (time.perf_counter() - t0) * 1e3
         if res.hit_mask is None:
-            raise _capi.NerfLoamError(f"Localiser: scan {frame.index} could not be placed: no placement within {search.get('radius', 5.0)} m "
-                                      f"of the saved trajectory hits the map")
+            return res, None, search_ms, None
         # the search's refinement ends at its own rate; the scan is then tracked from the placement like a scan without a motion prior
         # (num_iterations x 5) at the rate of every later scan, so its pose is as settled as theirs
         t0 = time.perf_counter()
@@ -148,10 +218,41 @@ class Localiser:
                                    tr.loss_criteria, tr.voxel_size, tr.N_rays, tr.step_size, tr.num_iterations * 5, tr.sdf_truncation,
                                    _rate_argument(tr.learning_rate / 3, frame.index), tr.max_voxel_hit, tr.max_distance,
                                    generator=self.generator)
-        self.times["polish"] = [(time.perf_counter() - t0) * 1e3]
-        frame.pose = OptimizablePose((pose if hit is not None else res.pose).data.detach().cpu().float().clone())
-        frame.pose.requires_grad_(False)
-        return res
+        polish_ms = (time.perf_counter() - t0) * 1e3
+        return res, _cpu_pose(pose if hit is not None else res.pose), search_ms, polish_ms
+
+    # -- recovery -------------------------------------------------------------------------------------------------------
+    def _local(self, frame, guess):
+        """score.relocalise around the 4x4 guess with its default lattice (N_rays, refine_iterations and the rate from global_specs):
+        the re-placed pose as a CPU OptimizablePose, or None when no hypothesis hits the map."""
+        g = self.global_specs
+        with self._rng():
+            pose, hit, _ = relocalise(frame, OptimizablePose.from_matrix(guess), self.map_state, self.saved.decoder,
+                                      self.tracker.loss_criteria, self.tracker.voxel_size, N_rays=g["N_rays"],
+                                      refine_iterations=g["refine_iterations"],
+                                      learning_rate=_rate_argument(g["learning_rate"], frame.index), **self._tracking_kw())
+        return None if hit is None else _cpu_pose(pose)
+
+    def _recover(self, frame, guess, accepted_losses, global_allowed):
+        """The fallback order for a lost scan: the local search around the guess, then, if global_allowed, the search with no guess.
+        Each re-placement is scored and kept only if it passes the lost rule.  Returns (status, (loss, hit fraction) of the kept pose),
+        or ("lost", None) with frame.pose left as it was."""
+        steps = [("local", lambda: self._local(frame, guess))]
+        if global_allowed:
+            steps.append(("global", lambda: self._search(frame)[1]))
+        tracked = frame.pose
+        for name, step in steps:
+            t0 = time.perf_counter()
+            pose, ok = step(), False
+            if pose is not None:
+                frame.pose = pose
+                sc = self.score(frame)
+                ok = not is_lost(*sc, accepted_losses, self.recovery)
+            self.times.setdefault(f"recover_{name}", []).append((time.perf_counter() - t0) * 1e3)
+            if ok:
+                return name, sc
+        frame.pose = tracked
+        return "lost", None
 
     # -- scoring --------------------------------------------------------------------------------------------------------
     def score(self, frame):
@@ -171,7 +272,10 @@ class Localiser:
     # -- the sequence ---------------------------------------------------------------------------------------------------
     def run(self, start_frame=0, end_frame=-1, read_offset=1, init_pose=None):
         """Localises scans start_frame .. end_frame (clamped to the last; -1: the last) whose index is divisible by read_offset, the
-        first scan always.  Returns a Localisation and, with out_dir, writes out_dir/frame_poses.txt (slam.write_poses)."""
+        first scan always.  Returns a Localisation and, with out_dir, writes out_dir/frame_poses.txt (slam.write_poses) and, with
+        recovery on, out_dir/frame_status.txt ("<scan id> <status>" per line).  With recovery on, each tracked scan is judged by
+        is_lost against the losses of the accepted scans (the first scan counts as accepted); a lost one goes through _recover, and a
+        global step runs only if none ran in the current run of lost scans within the last global_interval scans."""
         tr, n = self.tracker, len(self.data_stream)
         if not 0 <= int(start_frame) < n:
             raise ValueError(f"Localiser.run: start_frame {start_frame} outside the stream's {n} scans")
@@ -188,29 +292,66 @@ class Localiser:
         placement = self.place(first, init_pose)
         tr.last_frame, tr.start_frame = first, int(start_frame) + 1
         frames, scores = [first], [self.score(first)]
+        status = None if self.recovery is None else ["tracked"]
+        accepted, last_global = [scores[0][0]], None            # losses of the accepted scans; where the current lost run last searched
         for fid in tr.frame_ids():
+            ref, rel = tr.last_frame, tr.rel_pose
             f = tr.track(fid, 0)
             frames.append(f)
             scores.append(self.score(f))
+            if status is None:
+                continue
+            # a scan that came with a pose was passed through untracked (it has no relative pose): there is no track to judge
+            if f.rel_pose is None or not is_lost(*scores[-1], accepted, self.recovery):
+                status.append("tracked")
+                accepted.append(scores[-1][0])
+                last_global = None
+                continue
+            pos = len(frames) - 1
+            global_allowed = last_global is None or pos - last_global >= self.recovery["global_interval"]
+            code, sc = self._recover(f, constant_velocity_guess(ref.get_pose(), rel), accepted, global_allowed)
+            status.append(code)
+            if global_allowed and code != "local":
+                last_global = pos
+            if code == "lost":                                  # the scan keeps its tracked pose and score; tracking restarts from ref
+                tr.last_frame = ref
+            else:
+                scores[-1] = sc
+                accepted.append(sc[0])
+                last_global = None
+                tr.last_frame = f
+            tr.rel_pose = None                                  # the next scan is tracked like one without a motion prior
         poses = torch.stack([f.get_pose().detach().double() for f in frames])
         poses[:, :3, 3] -= POSE_OFFSET
+        scan_ids = [int(f.index) for f in frames]
         if self.out_dir is not None:
             os.makedirs(self.out_dir, exist_ok=True)
             write_poses(os.path.join(self.out_dir, "frame_poses.txt"), poses.numpy())
+            if status is not None:
+                with open(os.path.join(self.out_dir, "frame_status.txt"), "w") as fh:
+                    fh.writelines(f"{i} {s}\n" for i, s in zip(scan_ids, status))
         self.times.update(tr.times)
-        return Localisation(torch.tensor([int(f.index) for f in frames], dtype=torch.int64), poses,
+        return Localisation(torch.tensor(scan_ids, dtype=torch.int64), poses,
                             torch.tensor([s[0] for s in scores], dtype=torch.float64), torch.tensor([s[1] for s in scores], dtype=torch.float64),
-                            placement)
+                            placement, status)
 
     def summary(self, result):
         """A JSON-ready summary of run()'s result: scans, the map file's load time, median host ms per scan per stage (load, track,
         score; tracking's stages end in a read-back), the first scan's placement (ms, stage times, placements searched), the median
-        loss and the smallest hit fraction.  The placement's ms is the relocalise_global call; its track_ms the tracking from it."""
+        loss and the smallest hit fraction.  The placement's ms is the relocalise_global call; its track_ms the tracking from it.  With
+        recovery on, "recovery": the scans per status and the median ms of a local and of a global step (each with the score of its
+        pose; None where the step never ran)."""
         p = result.placement
         place = None
         if p is not None:
             place = {"ms": self.times["place"][0], "stages_ms": {k: v * 1e3 for k, v in p.diagnostics.times.items()},
                      "placements": int(p.diagnostics.n_placements), "loss": float(p.loss), "track_ms": self.times["polish"][0]}
-        return {"scans": int(result.scan_ids.numel()), "map_load_ms": self.load_ms,
-                "ms_per_scan": {k: float(np.median(v)) for k, v in self.times.items() if k not in ("place", "polish")}, "placement": place,
-                "median_loss": float(result.loss.median()), "min_hit_fraction": float(result.hit_fraction.min()), "out_dir": self.out_dir}
+        out = {"scans": int(result.scan_ids.numel()), "map_load_ms": self.load_ms,
+               "ms_per_scan": {k: float(np.median(v)) for k, v in self.times.items() if k not in _NOT_PER_SCAN},
+               "placement": place, "median_loss": float(result.loss.median()), "min_hit_fraction": float(result.hit_fraction.min()),
+               "out_dir": self.out_dir}
+        if result.status is not None:
+            out["recovery"] = {"counts": {s: result.status.count(s) for s in STATUSES},
+                               "ms": {s: float(np.median(self.times[f"recover_{s}"])) if f"recover_{s}" in self.times else None
+                                      for s in ("local", "global")}}
+        return out
