@@ -711,6 +711,11 @@ NL_API int nl_refine_pass_begin(int n_frames, int64_t cap, int n_keyframes, int 
  * (u32[ceil(n_rows / 32)]) was clear is set and appended to d_rows at d_state[NL_REFINE_LISTED] (each row once; order unspecified). */
 NL_API int nl_mark_rows(int64_t M, const int32_t *d_M, const int32_t *d_vox, const int32_t *d_vox2row, int64_t n_rows, uint32_t *d_row_bits,
                         int32_t *d_rows, int32_t *d_state, void *stream);
+/* nl_mark_rows with a floor: only rows >= row_floor are flagged and listed, so nl_adam_bf16_rows_ctl never steps rows [0, row_floor)
+ * (the saved rows of a map extended with a later drive, which stay fixed).  0 <= row_floor <= n_rows; row_floor = 0 is nl_mark_rows,
+ * with the same bits, list and count. */
+NL_API int nl_mark_rows_floor(int64_t M, const int32_t *d_M, const int32_t *d_vox, const int32_t *d_vox2row, int64_t n_rows,
+                              int64_t row_floor, uint32_t *d_row_bits, int32_t *d_rows, int32_t *d_state, void *stream);
 /* nl_adam_bf16_ctl (optim.step() on the embedding table, render_helpers.py:421-423) over the first min(*d_n_listed, n_rows) rows of d_rows
  * only, 16 elements per row, with the same arithmetic; step count and skip flag from d_ctl.  Every listed row's gradient is cleared
  * after it is read, on a skipped iteration too (its scatter may have run). */

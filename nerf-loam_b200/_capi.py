@@ -187,6 +187,7 @@ _SIGNATURES = {
     # key-scan map refinement (include/nerfloam_b200.h section 14)
     "nl_refine_pass_begin": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int] + [vp] * 15 + [C.c_int64] + [vp] * 5),
     "nl_mark_rows": (C.c_int, [C.c_int64, vp, vp, vp, C.c_int64, vp, vp, vp, vp]),
+    "nl_mark_rows_floor": (C.c_int, [C.c_int64, vp, vp, vp, C.c_int64, C.c_int64, vp, vp, vp, vp]),
     "nl_adam_bf16_rows_ctl": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp]),
     "nl_refine_iter_end": (C.c_int, [C.c_int, vp, vp, C.c_int32, vp, C.c_int32, vp]),
     # global localisation, coarse stage (include/nerfloam_b200.h section 15)

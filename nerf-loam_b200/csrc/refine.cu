@@ -5,7 +5,8 @@
 //   pass boundary : on the first iteration of a pass, the pass's window and poses go into the selection buffers, its seeds are set,
 //                   Adam's step count restarts, and the previous pass's rows get fresh moments and clear flags.
 //   row list      : a bit per embedding row; nl_mark_rows sets the bits of the rows the gradient scatter writes and appends each
-//                   newly set row to the list (warp-aggregated counter).  A plain load filters rows already flagged: bits only go
+//                   newly set row to the list (warp-aggregated counter).  nl_mark_rows_floor skips the rows below a floor, so Adam
+//                   never steps them (the saved rows of a map being extended).  A plain load filters rows already flagged: bits only go
 //                   from 0 to 1 inside the kernel, so a stale 0 costs an atomic and never loses a row.
 //   row Adam      : nl_adam_bf16_elem (adam.cuh, shared with nl_adam_bf16_ctl) on the listed rows, two threads per row (8 elements:
 //                   one 16-byte load each of p, m, v, two of the gradient); the gradient row is cleared after it is read, which
@@ -68,7 +69,7 @@ __global__ void __launch_bounds__(kThreads)
 // One thread per (sample, corner): the eight row ids of a sample are contiguous in vox2row, so a warp reads 4 samples' rows at once.
 __global__ void __launch_bounds__(kThreads)
     k_mark_rows(long long M_host, const int32_t *__restrict__ M_dev, const int32_t *__restrict__ vox, const int32_t *__restrict__ vox2row,
-                uint32_t *row_bits, int32_t *__restrict__ rows, int32_t *__restrict__ n_listed) {
+                int32_t row_floor, uint32_t *row_bits, int32_t *__restrict__ rows, int32_t *__restrict__ n_listed) {
     const long long M = M_dev ? min((long long)*M_dev, M_host) : M_host;
     const long long total = 8 * M;
     const int lane = threadIdx.x & 31;
@@ -78,7 +79,7 @@ __global__ void __launch_bounds__(kThreads)
         int row = -1;
         if (i < total) {
             row = vox2row[(size_t)vox[i >> 3] * 8 + (i & 7)];
-            if (row >= 0) {
+            if (row >= row_floor) {             // row_floor >= 0: also drops the -1 of an unset corner
                 const uint32_t bit = 1u << (row & 31);
                 if (!(row_bits[row >> 5] & bit)) fresh = !(atomicOr(&row_bits[row >> 5], bit) & bit);
             }
@@ -155,15 +156,21 @@ extern "C" int nl_refine_pass_begin(int n_frames, int64_t cap, int n_keyframes, 
     return NL_OK;
 }
 
-extern "C" int nl_mark_rows(int64_t M, const int32_t *d_M, const int32_t *d_vox, const int32_t *d_vox2row, int64_t n_rows, uint32_t *d_row_bits,
-                            int32_t *d_rows, int32_t *d_state, void *stream) {
+extern "C" int nl_mark_rows_floor(int64_t M, const int32_t *d_M, const int32_t *d_vox, const int32_t *d_vox2row, int64_t n_rows,
+                                  int64_t row_floor, uint32_t *d_row_bits, int32_t *d_rows, int32_t *d_state, void *stream) {
     if (M < 0 || n_rows <= 0 || n_rows > INT32_MAX) return nl_set_error("nl_mark_rows: bad sizes (M >= 0, 0 < n_rows < 2^31)");
+    if (row_floor < 0 || row_floor > n_rows) return nl_set_error("nl_mark_rows_floor: row_floor must lie in [0, n_rows]");
     if (!d_vox || !d_vox2row || !d_row_bits || !d_rows || !d_state) return nl_set_error("nl_mark_rows: null pointer");
     if (M == 0) return NL_OK;
-    k_mark_rows<<<grid_for(8 * M, 8), kThreads, 0, (cudaStream_t)stream>>>(M, d_M, d_vox, d_vox2row, d_row_bits, d_rows,
-                                                                             d_state + NL_REFINE_LISTED);
+    k_mark_rows<<<grid_for(8 * M, 8), kThreads, 0, (cudaStream_t)stream>>>(M, d_M, d_vox, d_vox2row, (int32_t)row_floor, d_row_bits,
+                                                                             d_rows, d_state + NL_REFINE_LISTED);
     NL_CHECK_LAUNCH("nl_mark_rows");
     return NL_OK;
+}
+
+extern "C" int nl_mark_rows(int64_t M, const int32_t *d_M, const int32_t *d_vox, const int32_t *d_vox2row, int64_t n_rows, uint32_t *d_row_bits,
+                            int32_t *d_rows, int32_t *d_state, void *stream) {
+    return nl_mark_rows_floor(M, d_M, d_vox, d_vox2row, n_rows, 0, d_row_bits, d_rows, d_state, stream);
 }
 
 extern "C" int nl_adam_bf16_rows_ctl(int64_t n_rows, const int32_t *d_rows, const int32_t *d_n_listed, uint16_t *d_param, float *d_grad_f32,

@@ -22,7 +22,8 @@
     passes the rule; otherwise the scan keeps its tracked pose and is reported lost.  After either, the motion model restarts from
     the last accepted scan.  The map is frozen, so a wrong decision changes one reported pose and nothing else.
 
-Not covered: updating the map, loop closure.
+Not covered here: updating the map (slam.NeRFLOAM's base_map grows a saved map with a later drive, placing its first scan with
+place_scan; DESIGN.md §11.6), loop closure.
 """
 import contextlib
 import copy
@@ -101,6 +102,70 @@ def _cpu_pose(pose):
     return p
 
 
+def forked_rng(generator):
+    """With a generator, a context under which torch's global generators are seeded from one draw of it and restored afterwards
+    (torch.random.fork_rng); with None, nothing: the caller draws from torch's global generators."""
+    if generator is None:
+        return contextlib.nullcontext()
+    seed = int(torch.randint(0, 2 ** 62, (1,), generator=generator))
+    stack = contextlib.ExitStack()
+    stack.enter_context(torch.random.fork_rng(devices=[torch.cuda.current_device()]))
+    torch.manual_seed(seed)
+    return stack
+
+
+def _tracking_kw(tr):
+    return dict(step_size=tr.step_size, truncation=tr.sdf_truncation, max_voxel_hit=tr.max_voxel_hit, max_distance=tr.max_distance)
+
+
+def place_scan(frame, map_state, decoder, tracker, anchors, global_specs, generator=None):
+    """The search with no pose guess: relocalise_global anchored on every pose of `anchors` (f64[S,4,4] in the map frame, POSE_OFFSET
+    included) with global_specs (GLOBAL_SPECS' keys), under forked_rng(generator), then track_frame from its placement with
+    `tracker`'s settings (a slam.Tracking).  Localiser's first scan and its global recovery use it, and so does slam.NeRFLOAM's first
+    scan when it extends a saved map.  Returns (GlobalResult, the pose as a CPU OptimizablePose or None when no placement hits the
+    map, search ms, tracking ms or None); frame.pose is not touched."""
+    tr = tracker
+    g = dict(global_specs)
+    search = {k: g.pop(k) for k in ("radius", "xy_step", "yaw_steps", "n_points", "n_candidates", "n_seeds") if k in g}
+    g["learning_rate"] = _rate_argument(g["learning_rate"], frame.index)
+    t0 = time.perf_counter()
+    with forked_rng(generator):
+        res = relocalise_global(frame, map_state, decoder, tr.loss_criteria, tr.voxel_size, anchors=anchors, **search, **_tracking_kw(tr), **g)
+    search_ms = (time.perf_counter() - t0) * 1e3
+    if res.hit_mask is None:
+        return res, None, search_ms, None
+    # the search's refinement ends at its own rate; the scan is then tracked from the placement like a scan without a motion prior
+    # (num_iterations x 5) at the rate of every later scan, so its pose is as settled as theirs
+    t0 = time.perf_counter()
+    pose, hit = rh.track_frame(OptimizablePose(res.pose.data.detach().cpu().float().clone()), frame, map_state, decoder,
+                               tr.loss_criteria, tr.voxel_size, tr.N_rays, tr.step_size, tr.num_iterations * 5, tr.sdf_truncation,
+                               _rate_argument(tr.learning_rate / 3, frame.index), tr.max_voxel_hit, tr.max_distance, generator=generator)
+    polish_ms = (time.perf_counter() - t0) * 1e3
+    return res, _cpu_pose(pose if hit is not None else res.pose), search_ms, polish_ms
+
+
+def trajectory_anchors(trajectory):
+    """A saved trajectory (f64[S,4,4] without POSE_OFFSET) as place_scan's anchors: a copy with POSE_OFFSET added, since the map
+    carries it."""
+    anchors = torch.as_tensor(np.asarray(trajectory, dtype=np.float64)).clone()
+    anchors[:, :3, 3] += POSE_OFFSET
+    return anchors
+
+
+def place_first(frame, map_state, decoder, tracker, anchors, global_specs, generator, times, who):
+    """A sequence's first scan placed in a saved map with no pose guess: place_scan, then frame.pose = its pose.  times["place"] gets
+    the search's ms and, when it succeeded, times["polish"] the tracking's.  Raises NerfLoamError naming `who` when no placement
+    hits the map.  Returns the GlobalResult.  Localiser.place and slam.NeRFLOAM's base_map both use it."""
+    res, pose, search_ms, polish_ms = place_scan(frame, map_state, decoder, tracker, anchors, global_specs, generator)
+    times["place"] = [search_ms]
+    if pose is None:
+        raise _capi.NerfLoamError(f"{who}: scan {frame.index} could not be placed: no placement within "
+                                  f"{global_specs['radius']} m of the saved trajectory hits the map")
+    times["polish"] = [polish_ms]
+    frame.pose = pose
+    return res
+
+
 Localisation = namedtuple("Localisation", ["scan_ids", "poses", "loss", "hit_fraction", "placement", "status"])
 Localisation.__doc__ = """Localiser.run's result, per scan in order: scan_ids i64[S], poses f64[S,4,4] in the map frame without POSE_OFFSET
 (what frame_poses.txt holds), loss f64[S] and hit_fraction f64[S] (score_poses at the final pose), placement: the first scan's
@@ -156,20 +221,12 @@ class Localiser:
         self.map_state = saved.map.map_states["_mapstate"]
         self.frozen = FrozenMap(self.map_state, saved.decoder)
         self.tracker = Tracking(self.args, data_stream, self.frozen, generator)
-        self.anchors = torch.as_tensor(np.asarray(saved.trajectory, dtype=np.float64)).clone()
-        self.anchors[:, :3, 3] += POSE_OFFSET
+        self.anchors = trajectory_anchors(saved.trajectory)
         self.times = {}
 
     # -- the first scan -------------------------------------------------------------------------------------------------
     def _rng(self):
-        """With a generator, the search draws from torch's global generators seeded from it, restored afterwards."""
-        if self.generator is None:
-            return contextlib.nullcontext()
-        seed = int(torch.randint(0, 2 ** 62, (1,), generator=self.generator))
-        stack = contextlib.ExitStack()
-        stack.enter_context(torch.random.fork_rng(devices=[torch.cuda.current_device()]))
-        torch.manual_seed(seed)
-        return stack
+        return forked_rng(self.generator)
 
     def place(self, frame, init_pose=None):
         """Sets frame.pose for the first scan: init_pose (4x4 in the map frame, without POSE_OFFSET) or relocalise_global over the
@@ -183,43 +240,15 @@ class Localiser:
             frame.pose = OptimizablePose.from_matrix(T.float())
             frame.pose.requires_grad_(False)
             return None
-        res, pose, search_ms, polish_ms = self._search(frame)
-        self.times["place"] = [search_ms]
-        if pose is None:
-            raise _capi.NerfLoamError(f"Localiser: scan {frame.index} could not be placed: no placement within "
-                                      f"{self.global_specs['radius']} m of the saved trajectory hits the map")
-        self.times["polish"] = [polish_ms]
-        frame.pose = pose
-        return res
+        return place_first(frame, self.map_state, self.saved.decoder, self.tracker, self.anchors, self.global_specs, self.generator,
+                           self.times, "Localiser")
 
     def _tracking_kw(self):
-        tr = self.tracker
-        return dict(step_size=tr.step_size, truncation=tr.sdf_truncation, max_voxel_hit=tr.max_voxel_hit, max_distance=tr.max_distance)
+        return _tracking_kw(self.tracker)
 
     def _search(self, frame):
-        """The search with no pose guess: relocalise_global anchored on every saved pose (global_specs), then track_frame from its
-        placement.  Returns (GlobalResult, the pose as a CPU OptimizablePose or None when no placement hits the map, search ms,
-        tracking ms or None); frame.pose is not touched."""
-        tr = self.tracker
-        g = dict(self.global_specs)
-        search = {k: g.pop(k) for k in ("radius", "xy_step", "yaw_steps", "n_points", "n_candidates", "n_seeds") if k in g}
-        g["learning_rate"] = _rate_argument(g["learning_rate"], frame.index)
-        t0 = time.perf_counter()
-        with self._rng():
-            res = relocalise_global(frame, self.map_state, self.saved.decoder, tr.loss_criteria, tr.voxel_size, anchors=self.anchors, **search,
-                                    **self._tracking_kw(), **g)
-        search_ms = (time.perf_counter() - t0) * 1e3
-        if res.hit_mask is None:
-            return res, None, search_ms, None
-        # the search's refinement ends at its own rate; the scan is then tracked from the placement like a scan without a motion prior
-        # (num_iterations x 5) at the rate of every later scan, so its pose is as settled as theirs
-        t0 = time.perf_counter()
-        pose, hit = rh.track_frame(OptimizablePose(res.pose.data.detach().cpu().float().clone()), frame, self.map_state, self.saved.decoder,
-                                   tr.loss_criteria, tr.voxel_size, tr.N_rays, tr.step_size, tr.num_iterations * 5, tr.sdf_truncation,
-                                   _rate_argument(tr.learning_rate / 3, frame.index), tr.max_voxel_hit, tr.max_distance,
-                                   generator=self.generator)
-        polish_ms = (time.perf_counter() - t0) * 1e3
-        return res, _cpu_pose(pose if hit is not None else res.pose), search_ms, polish_ms
+        """place_scan over this map, its saved trajectory and global_specs, drawing from the Localiser's generator."""
+        return place_scan(frame, self.map_state, self.saved.decoder, self.tracker, self.anchors, self.global_specs, self.generator)
 
     # -- recovery -------------------------------------------------------------------------------------------------------
     def _local(self, frame, guess):

@@ -255,6 +255,20 @@ class MapUpdater:
             self._emb_buf[self.n_rows:new_rows] = add.to(torch.bfloat16).to(self.device)
         self.n_rows = new_rows
 
+    def reserve(self, nodes=0, rows=0):
+        """Room for at least `nodes` nodes and `rows` embedding rows: one move of the buffers now instead of capacity doublings later
+        (each of which invalidates the captured graphs).  The map's contents are unchanged; map_states is re-published over the
+        moved buffers."""
+        moved = False
+        if self.incremental and int(nodes) > self._centres.shape[0]:
+            self._grow_nodes(int(nodes))
+            moved = True
+        if int(rows) > self._emb_buf.shape[0]:
+            self._emb_buf = grown(self._emb_buf, int(rows), self.n_rows, 0)
+            moved = True
+        if moved and self.incremental and self.map_states is not None:
+            self._publish()
+
     def _grow_nodes(self, n):
         k = self.n_nodes
         self._centres, self._structure, self._vox2row, self._vertex, self._v2r = (

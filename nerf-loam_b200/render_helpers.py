@@ -12,6 +12,7 @@ Behavioural notes (also in DESIGN.md):
     (voxel_helpers.py:531-533; render_helpers.py:190-318);
   * the unused autograd.grad(sdf, xyz) of render_helpers.py:293-297 is not computed.
 """
+import numbers
 import os
 import threading
 import weakref
@@ -392,6 +393,14 @@ def _check_ctl(ctl, what):
         raise _capi.NerfLoamError(f"{what}: octree traversal stack overflow (octree deeper than the 18 levels of octree.cpp:39?)")
 
 
+def _frozen_rows(frozen_rows, embeddings, what):
+    """frozen_rows as an int in [0, the table's row count]; ValueError otherwise."""
+    n = int(embeddings.shape[0])
+    if isinstance(frozen_rows, bool) or not isinstance(frozen_rows, numbers.Integral) or not 0 <= int(frozen_rows) <= n:
+        raise ValueError(f"{what}: frozen_rows must be an int in [0, {n}] (the table's rows), got {frozen_rows!r}")
+    return int(frozen_rows)
+
+
 def _grown_capacity(cap, ctl, what):
     _check_sample_total(ctl[_capi.CTL_MAX_SAMPLES], what)
     return max(2 * cap, int(ctl[_capi.CTL_MAX_SAMPLES] * 1.25) + 1024)
@@ -406,7 +415,7 @@ class _MapGraph:
 
     _cache = {}
 
-    def __init__(self, key, m, emb, sdf_network, cfg, F, N_rays, lrs, update_decoder, pose_rows, deterministic, cap, spr):
+    def __init__(self, key, m, emb, sdf_network, cfg, F, N_rays, lrs, update_decoder, pose_rows, deterministic, cap, spr, frozen_rows=0):
         dev = emb.device
         R = F * N_rays
         eng = SDFEngine(R, R * spr, dev)            # private: captured pointers must stay valid
@@ -425,7 +434,7 @@ class _MapGraph:
         self.pose_m, self.pose_v = torch.zeros((F, 6), device=dev), torch.zeros((F, 6), device=dev)     # Adam moments of the poses (nl_pose_step)
         self.seed_dev = torch.zeros(1, dtype=torch.int32, device=dev)
         any_pose = len(pose_rows) > 0
-        groups = [dict(param=emb, grad=None, lr=lrs[0])]
+        groups = [dict(param=emb[frozen_rows:], grad=None, lr=lrs[0])]        # rows below frozen_rows are never stepped
         if update_decoder:
             groups += [dict(param=p.data, grad=g, lr=lrs[1]) for p, g in zip(bufs.params, bufs.grads)]
         state = {"opt": None}
@@ -441,7 +450,7 @@ class _MapGraph:
                                  pose_step=dict(mask=sum(1 << i for i in pose_rows), m=self.pose_m, v=self.pose_v, lr=lrs[2],
                                                 seeds=[(self.sel_seed, 0x632BE5), (self.seed_dev, 0x3779B1)]) if fused_tail else None)
             if state["opt"] is None:
-                groups[0]["grad"] = eng.grad_emb
+                groups[0]["grad"] = eng.grad_emb[frozen_rows:]
                 pg = [] if fused_tail else [dict(param=self.pose6[i], grad=eng.pose_grad[i], lr=lrs[2]) for i in pose_rows]
                 state["opt"] = FusedAdam(groups + pg, ctl=eng.ctl)     # one fixed control block: forward_backward folds in place
             state["opt"].step()
@@ -470,7 +479,7 @@ class _MapGraph:
                 p.data.copy_(q)
 
     @classmethod
-    def get(cls, m, emb, sdf_network, cfg, F, N_rays, lrs, update_decoder, pose_rows, deterministic, n_points, spr):
+    def get(cls, m, emb, sdf_network, cfg, F, N_rays, lrs, update_decoder, pose_rows, deterministic, n_points, spr, frozen_rows=0):
         cap = max(1 << 17, 1 << (int(n_points) - 1).bit_length())
         stable = m.stable
         if stable and m.emb_full is not None and emb.data_ptr() == m.emb_full.data_ptr():
@@ -481,11 +490,11 @@ class _MapGraph:
         key = (F, N_rays, tuple(float(x) for x in lrs), bool(update_decoder), tuple(pose_rows), bool(deterministic), cap, int(spr),
                m.centres.data_ptr(), m.structure.data_ptr(), m.vox2row.data_ptr(), m.packed_children().data_ptr(), emb.data_ptr(),
                -1 if stable else m.n_nodes, int(emb.shape[0]), tuple(p.data_ptr() for p in _decoder_params(sdf_network)),
-               tuple(sorted(cfg.items())))
+               tuple(sorted(cfg.items())), int(frozen_rows))
         g = cls._cache.get("g")
         if g is None or g.key != key:
             cls._cache = {}
-            g = cls(key, m, emb, sdf_network, cfg, F, N_rays, lrs, update_decoder, pose_rows, deterministic, cap, spr)
+            g = cls(key, m, emb, sdf_network, cfg, F, N_rays, lrs, update_decoder, pose_rows, deterministic, cap, spr, frozen_rows)
             cls._cache = {"g": g}
         return g
 
@@ -519,7 +528,7 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
                          N_rays=512, num_iterations=10, truncation=0.1, max_voxel_hit=10, max_distance=10,
                          learning_rate=[1e-2, 1e-2, 5e-3], update_pose=True, update_decoder=True, profiler=None,
                          deterministic=False, noise_per_iter=None, loss_log=None, ray_selection="device", cuda_graph=None,
-                         generator=None):
+                         generator=None, frozen_rows=0):
     """render_helpers.py:321-425.  Mutates `embeddings` (bf16 CUDA table), the decoder parameters and the
     frame poses in place, like the reference.  Returns None.  ray_selection: see _FrameBatch.select ("device" by default;
     "host" reproduces the reference's CPU RNG stream ray for ray).  cuda_graph (default: on whenever ray_selection="device" and no
@@ -531,7 +540,11 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
     restored and the whole call is redone with a larger engine, so a truncated sample set never reaches the parameters.
 
     generator: a CPU torch.Generator that every random draw of the call (ray selection, sampler seeds) comes from instead of torch's
-    global generators, which it then leaves untouched -- two threads each with their own generator draw reproducibly."""
+    global generators, which it then leaves untouched -- two threads each with their own generator draw reproducibly.
+
+    frozen_rows: embedding rows [0, frozen_rows) are held fixed: Adam steps only the table's tail (the saved rows of a map being
+    extended, slam.NeRFLOAM's base_map).  Their gradients are still scattered; nothing reads them.  0 steps the whole table."""
+    frozen_rows = _frozen_rows(frozen_rows, embeddings, "bundle_adjust_frames")
     if ray_selection not in ("host", "device"):
         raise ValueError("ray_selection must be 'host' or 'device'")
     dev = embeddings.device
@@ -561,7 +574,7 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
 
     def run(eng):
         eng.begin_call()
-        groups = [dict(param=emb, grad=None, lr=learning_rate[0])]
+        groups = [dict(param=emb[frozen_rows:], grad=None, lr=learning_rate[0])]
         if update_decoder:
             groups += [dict(param=p.data, grad=g, lr=learning_rate[1], side=True) for p, g in zip(bufs.params, bufs.grads)]
         opt = None
@@ -574,7 +587,7 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
                                  rng_seed=seed, update_decoder=update_decoder, update_emb=True, update_pose=any(pose_opt), pose6=pose6,
                                  defer_wgrad=pipeline)
             if opt is None:
-                groups[0]["grad"] = eng.grad_emb
+                groups[0]["grad"] = eng.grad_emb[frozen_rows:]
                 pg = [dict(param=pose_params[k], grad=eng.pose_grad[i], lr=learning_rate[2]) for k, i in enumerate(pose_rows)]
                 opt = FusedAdam(groups + pg, ctl=lambda: eng.ctl)
             if loss_log is not None:                    # diagnostic path: one read-back per iteration
@@ -600,7 +613,7 @@ def bundle_adjust_frames(keyframe_graph, embeddings, map_states, sdf_network, lo
         n_log = len(loss_log) if loss_log is not None else 0
         if cuda_graph:
             g = _MapGraph.get(m, emb, sdf_network, cfg, F, N_rays, learning_rate, update_decoder, pose_rows, deterministic,
-                              max(f.points.shape[0] for f in frames), -(-cap // R))
+                              max(f.points.shape[0] for f in frames), -(-cap // R), frozen_rows)
             ctl = g.run(frames, pose6, num_iterations, 0 if deterministic else _seed_from_torch(generator), generator)
             pose6.copy_(g.pose6)
         else:
@@ -653,7 +666,7 @@ class _RefineGraph:
 
     _cache = {}
 
-    def __init__(self, key, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, cap, spr, K, P, iters):
+    def __init__(self, key, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, cap, spr, K, P, iters, frozen_rows=0):
         dev = emb.device
         R = F * N_rays
         V = emb.shape[0]
@@ -701,8 +714,8 @@ class _RefineGraph:
             eng.forward_backward(m, bufs, R, cfg, gt, cos, dir_local=dirs, ray_frame=self.fid, n_frames=F, update_decoder=False,
                                  update_emb=True, update_pose=False, pose6=self.pose6, refresh_weights=False, rng_seed_dev=self.seed_dev,
                                  zero_grads=False)
-            _capi.check(lib.nl_mark_rows(eng.max_samples, eng.n_samples_dev, _capi.ptr(eng.s_vox), _capi.ptr(m.vox2row), V,
-                                         _capi.ptr(self.row_bits), _capi.ptr(self.rows), _capi.ptr(self.state), st), "nl_mark_rows")
+            _capi.check(lib.nl_mark_rows_floor(eng.max_samples, eng.n_samples_dev, _capi.ptr(eng.s_vox), _capi.ptr(m.vox2row), V, frozen_rows,
+                                               _capi.ptr(self.row_bits), _capi.ptr(self.rows), _capi.ptr(self.state), st), "nl_mark_rows_floor")
             _capi.check(lib.nl_adam_bf16_rows_ctl(V, _capi.ptr(self.rows), _capi.ptr(self.state[_capi.REFINE_LISTED:]), _capi.ptr(emb),
                                                   _capi.ptr(eng.grad_emb), _capi.ptr(self.adam_m), _capi.ptr(self.adam_v), self.lr, 0.9, 0.999,
                                                   1e-8, _capi.ptr(eng.ctl), st), "nl_adam_bf16_rows_ctl")
@@ -733,15 +746,15 @@ class _RefineGraph:
             t.zero_()
 
     @classmethod
-    def get(cls, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, n_points, spr, K, P, iters):
+    def get(cls, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, n_points, spr, K, P, iters, frozen_rows=0):
         cap = max(1 << 17, 1 << (int(n_points) - 1).bit_length())
         key = (F, N_rays, float(lr), bool(deterministic), cap, int(spr), K, P, iters, m.centres.data_ptr(), m.structure.data_ptr(),
                m.vox2row.data_ptr(), m.packed_children().data_ptr(), emb.data_ptr(), -1 if m.stable else m.n_nodes, int(emb.shape[0]),
-               tuple(p.data_ptr() for p in _decoder_params(sdf_network)), tuple(sorted(cfg.items())))
+               tuple(p.data_ptr() for p in _decoder_params(sdf_network)), tuple(sorted(cfg.items())), int(frozen_rows))
         g = cls._cache.get("g")
         if g is None or g.key != key:
             cls._cache = {}
-            g = cls(key, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, cap, spr, K, P, iters)
+            g = cls(key, m, emb, sdf_network, cfg, F, N_rays, lr, deterministic, cap, spr, K, P, iters, frozen_rows)
             cls._cache = {"g": g}
         return g
 
@@ -768,7 +781,8 @@ class _RefineGraph:
 
 
 def refine_map(keyframe_graph, embeddings, map_states, sdf_network, loss_criteria, voxel_size, step_size, N_rays=512, num_iterations=10,
-               truncation=0.1, max_voxel_hit=10, max_distance=10, learning_rate=1e-2, passes=None, deterministic=False, generator=None):
+               truncation=0.1, max_voxel_hit=10, max_distance=10, learning_rate=1e-2, passes=None, deterministic=False, generator=None,
+               frozen_rows=0):
     """The mapper's key-scan refinement (`mapper_specs.final_iter`, mapping.py:154-164): `passes` (default len(keyframe_graph) + 1)
     bundle adjustments of a random window of keyframes with poses and decoder frozen, each with a fresh Adam on the embedding table,
     i.e. under the same random.seed / torch.manual_seed what
@@ -784,7 +798,10 @@ def refine_map(keyframe_graph, embeddings, map_states, sdf_network, loss_criteri
     Everything the loop draws is drawn up front (refine_schedule) and uploaded once; one captured iteration (_RefineGraph) is replayed
     passes x num_iterations times, and Adam steps only the rows the pass has reached, which is exact because the optimiser is fresh in
     every pass (include/nerfloam_b200.h section 14).  The control block is read once at the end; a call that exceeded the sample
-    capacity is undone and redone with room for its largest iteration.  generator: a CPU torch.Generator for every draw (refine_schedule)."""
+    capacity is undone and redone with room for its largest iteration.  generator: a CPU torch.Generator for every draw (refine_schedule).
+    frozen_rows: rows [0, frozen_rows) never enter the row list (nl_mark_rows_floor), so Adam leaves them bitwise unchanged; 0 lists
+    every row the scatter reaches."""
+    frozen_rows = _frozen_rows(frozen_rows, embeddings, "refine_map")
     frames = list(keyframe_graph.keyframe_graph)
     K = len(frames)
     if K == 0:
@@ -821,7 +838,7 @@ def refine_map(keyframe_graph, embeddings, map_states, sdf_network, loss_criteri
         if snap is None:
             snap = emb.clone()
         g = _RefineGraph.get(m, emb, sdf_network, cfg, F, N_rays, learning_rate, deterministic, max(counts), -(-cap // R), K, P,
-                             int(num_iterations))
+                             int(num_iterations), frozen_rows)
         ctl = g.run(arrays, counts, pose6, windows, noise, sel_seeds)
         _check_ctl(ctl, "refine_map")
         if not (ctl[_capi.CTL_ERROR] & 2):

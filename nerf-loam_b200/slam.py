@@ -40,6 +40,7 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
+from . import _capi
 from . import render_helpers as rh
 from .criterion import Criterion
 from .frame import POSE_OFFSET, LidarFrame
@@ -207,8 +208,9 @@ class Tracking(_Timed):
     mapper's copy of it: a new LidarFrame over the same points with its OWN OptimizablePose (the reference's copy crosses a process
     boundary, so the mapper's bundle adjustment never moves the tracker's last_frame)."""
 
-    def __init__(self, args, data_stream, shared, generator=None):
+    def __init__(self, args, data_stream, shared, generator=None, place=None):
         self.args, self.data_stream, self.shared, self.generator = args, data_stream, shared, generator
+        self.place = place                  # None: the first scan at get_init_pose; else place(frame) sets its pose (NeRFLOAM's base_map)
         ts, ms = args.tracker_specs, args.mapper_specs
         self.loss_criteria = Criterion(args)
         self.voxel_size = ms["voxel_size"]
@@ -228,9 +230,13 @@ class Tracking(_Timed):
         self.times, self.streams = {}, set()
 
     def first_frame(self):
-        """process_first_frame (tracking.py:51-61): the first scan at get_init_pose(start_frame)."""
+        """process_first_frame (tracking.py:51-61): the first scan at get_init_pose(start_frame), or where place(frame) puts it."""
         index, points, pointcos, _ = self.data_stream[self.start_frame]
-        first = LidarFrame(index, points, pointcos, np.array(self.data_stream.get_init_pose(self.start_frame), dtype=np.float64))
+        if self.place is None:
+            first = LidarFrame(index, points, pointcos, np.array(self.data_stream.get_init_pose(self.start_frame), dtype=np.float64))
+        else:
+            first = LidarFrame(index, points, pointcos, OptimizablePose(torch.zeros(6)), new_keyframe=True)
+            self.place(first)
         first.pose.requires_grad_(False)
         self.last_frame = first
         self.start_frame += 1
@@ -289,10 +295,13 @@ class Tracking(_Timed):
 class Mapping(_Timed):
     """mapping.py:30-351 on a MapUpdater, a KeyframeGraph and a SharedMap.  init(frame) maps the first scan; optimise(frame) is the
     bundle adjustment of a tracked scan, update(frame) the rest of its mapping step (create_voxels, keyframe, trajectory entry,
-    periodic mesh); both of those end with a publication whose version they return.  finish() writes the final outputs."""
+    periodic mesh); both of those end with a publication whose version they return.  finish() writes the final outputs.
+
+    map_updater: a MapUpdater to grow (a saved map's) instead of a new one; its rows [0, n_rows) at construction are then held fixed
+    (frozen_rows in every bundle_adjust_frames and refine_map call) and the decoder is never stepped."""
 
     def __init__(self, args, out_dir, shared, decoder, generator=None, selection="current", init_calls=12, reserve_nodes=1 << 20,
-                 reserve_rows=1 << 20):
+                 reserve_rows=1 << 20, map_updater=None):
         if selection not in SELECTIONS:
             raise ValueError(f"selection must be one of {SELECTIONS}, not {selection!r}")
         ms = args.mapper_specs
@@ -310,7 +319,12 @@ class Mapping(_Timed):
         self.remove_back, self.key_distance = ms["remove_back"], ms["key_distance"]
         self.final_iter, self.mesh_res = ms["final_iter"], ms["mesh_res"]
         self.mesh_freq = args.debug_args["mesh_freq"]
-        self.map = MapUpdater(self.voxel_size, reserve_nodes=reserve_nodes, reserve_rows=reserve_rows)
+        if map_updater is None:
+            self.map = MapUpdater(self.voxel_size, reserve_nodes=reserve_nodes, reserve_rows=reserve_rows)
+            self.frozen_rows, self.train_decoder = 0, True
+        else:
+            self.map = map_updater                              # new vertices get rows >= n_rows: rows are appended in creation order
+            self.frozen_rows, self.train_decoder = int(map_updater.n_rows), False
         self.map.readers = shared
         self.map_state = None
         self.kg = KeyframeGraph(self.window_size, self.keyframe_gap, self.key_distance, self.n_rays, self.voxel_size)
@@ -367,7 +381,7 @@ class Mapping(_Timed):
         rh.refine_map(self.kg, self.map.embeddings, self.map_state, self.decoder, self.loss_criteria, self.voxel_size, self.step_size,
                       N_rays=2 * self.n_rays, num_iterations=self.num_iterations, truncation=self.sdf_truncation,
                       max_voxel_hit=self.max_voxel_hit, max_distance=self.max_distance, learning_rate=self.learning_rate[0],
-                      generator=self.generator)
+                      generator=self.generator, frozen_rows=self.frozen_rows)
         torch.cuda.current_stream().synchronize()
         self._tick("refine", t0)
 
@@ -389,12 +403,13 @@ class Mapping(_Timed):
         return version
 
     def _do_mapping(self, frame, selection):
-        """mapping.py:172-202 (update_decoder only while index - first < freeze_frame)."""
+        """mapping.py:172-202 (update_decoder only while index - first < freeze_frame, and never when growing a saved map)."""
         targets = self.kg.select_optimize_targets(frame, selection, generator=self.generator)
         rh.bundle_adjust_frames(targets, self.map.embeddings, self.map_state, self.decoder, self.loss_criteria, self.voxel_size,
                                 self.step_size, self.n_rays, self.num_iterations, self.sdf_truncation, self.max_voxel_hit,
                                 self.max_distance, learning_rate=self.learning_rate, update_pose=True,
-                                update_decoder=(frame.index - self.first_frame_id) < self.freeze_frame, generator=self.generator)
+                                update_decoder=self.train_decoder and (frame.index - self.first_frame_id) < self.freeze_frame,
+                                generator=self.generator, frozen_rows=self.frozen_rows)
 
     def _create_voxels(self, frame):
         self.map_state = self.map.create_voxels(frame.points, frame.get_pose().detach())
@@ -630,6 +645,29 @@ def _decoder_size(specs):
         return sum(p.numel() for p in Decoder(**specs).state_dict().values())
 
 
+def grown_trajectory(saved, poses, scan_ids):
+    """The trajectory and scan ids of a saved map grown by a later drive: the saved ones (SavedMap) followed by the drive's poses
+    f64[S,4,4] (without POSE_OFFSET) and ids, in that order.  Ids may repeat across drives: the map file only keeps them beside the
+    poses.  Returns (f64[S0 + S,4,4], i64[S0 + S])."""
+    traj = np.concatenate([np.asarray(saved.trajectory, dtype=np.float64).reshape(-1, 4, 4), np.asarray(poses, dtype=np.float64).reshape(-1, 4, 4)])
+    ids = np.concatenate([np.asarray(saved.scan_ids, dtype=np.int64).reshape(-1), np.asarray(scan_ids, dtype=np.int64).reshape(-1)])
+    return traj, ids
+
+
+BASE_KEYS = ("voxel_size", "decoder_specs", "criteria")
+
+
+def check_base_config(args, saved):
+    """A run that grows `saved` (SavedMap) must agree with it on what its decoder was trained for: voxel_size (the run's
+    mapper_specs.voxel_size), decoder_specs and criteria (the truncation and loss weights).  ValueError naming the first key that
+    differs."""
+    ours = {"voxel_size": args.mapper_specs["voxel_size"], "decoder_specs": args.decoder_specs, "criteria": args.criteria}
+    theirs = {"voxel_size": saved.config["voxel_size"], "decoder_specs": saved.decoder_specs, "criteria": saved.config["criteria"]}
+    for k in BASE_KEYS:
+        if _plain(ours[k], k) != _plain(theirs[k], k):
+            raise ValueError(f"base_map: the config's {k} {ours[k]!r} differs from the map's {theirs[k]!r}")
+
+
 def _check_map_file(obj):
     """The checks of a map file above the map itself (from_state_dict checks that); the names of the failed ones."""
     if not isinstance(obj, dict):
@@ -728,24 +766,54 @@ class NeRFLOAM:
     __len__, __getitem__ -> (index, points, pointsCos, pose or None) and get_init_pose (default: dataset.<dataset>.DataLoader over
     data_specs).  selection: the mapping window, 'current' (the reference's), 'previous' or 'overlap' (KeyframeGraph).  init_calls:
     'current' mapping calls on the first scan.  The constructor seeds torch, numpy and random with `seeding` like run.py:13-23 (the
-    decoder's initial weights come from torch's generator); the tracker and the mapper then draw from generators of their own."""
+    decoder's initial weights come from torch's generator); the tracker and the mapper then draw from generators of their own.
 
-    def __init__(self, config, out_dir, data_stream=None, selection="current", init_calls=12, reserve_nodes=1 << 20, reserve_rows=1 << 20):
+    base_map: a map file (write_map) or a SavedMap (on the host octree) to grow with this sequence instead of starting an empty map
+    (DESIGN.md section 11.6).  The config must agree with it on BASE_KEYS (check_base_config); its "global_specs" key overrides
+    localise.GLOBAL_SPECS.  The first scan is placed as localise.Localiser places it (localise.place_first over the saved trajectory,
+    drawing from the tracker's generator), and run() raises NerfLoamError, writing nothing, when no placement hits the map.  The saved
+    MapUpdater is grown in place, with reserve_nodes / reserve_rows of room like a new map (MapUpdater.reserve); its decoder is never
+    stepped and its rows stay fixed (Mapping's map_updater); frame_poses.txt holds
+    this sequence's poses, and save_map writes the saved trajectory followed by them.  None: an empty map, as before."""
+
+    def __init__(self, config, out_dir, data_stream=None, selection="current", init_calls=12, reserve_nodes=1 << 20, reserve_rows=1 << 20,
+                 base_map=None):
         args = load_config(config)
         self.args, self.out_dir = args, out_dir
+        self.base = None
+        if base_map is not None:
+            self.base = base_map if isinstance(base_map, SavedMap) else load_map(base_map, octree="host")
+            if self.base.map.on_device:
+                raise ValueError("base_map: the map must be on the host octree (load_map(..., octree='host'))")
+            check_base_config(args, self.base)
+            self.base.map.reserve(reserve_nodes, reserve_rows)     # the room a new map would have had
         torch.manual_seed(args.seeding)
         torch.cuda.manual_seed_all(args.seeding)
         np.random.seed(args.seeding)
         random.seed(args.seeding)
         self.data_stream = data_stream if data_stream is not None else load_dataset(args)
         dspec = dict(args.decoder_specs)
-        decoder = Decoder(**dspec).cuda()
+        decoder = Decoder(**dspec).cuda() if self.base is None else self.base.decoder
         self.shared = SharedMap(lambda: Decoder(**dspec).cuda())
-        self.tracker = Tracking(args, self.data_stream, self.shared, torch.Generator().manual_seed(args.seeding))
+        self.tracker = Tracking(args, self.data_stream, self.shared, torch.Generator().manual_seed(args.seeding),
+                                place=None if self.base is None else self._place_first)
         self.mapper = Mapping(args, out_dir, self.shared, decoder, torch.Generator().manual_seed(args.seeding + 1), selection, init_calls,
-                              reserve_nodes, reserve_rows)
+                              reserve_nodes, reserve_rows, map_updater=None if self.base is None else self.base.map)
         self.streams = (torch.cuda.Stream(), torch.cuda.Stream())
         self.schedule = None
+        self.placement, self.place_ms = None, None
+
+    def _place_first(self, frame):
+        """The first scan's pose in the base map, as Localiser places it (localise.place_first over the saved trajectory, with
+        localise.GLOBAL_SPECS under the config's global_specs), drawing from the tracker's generator."""
+        from .localise import GLOBAL_SPECS, place_first, trajectory_anchors          # localise imports this module
+        specs = {**GLOBAL_SPECS, **(getattr(self.args, "global_specs", None) or {})}
+        times = {}
+        try:
+            self.placement = place_first(frame, self.base.map.map_states["_mapstate"], self.base.decoder, self.tracker,
+                                         trajectory_anchors(self.base.trajectory), specs, self.tracker.generator, times, "NeRFLOAM")
+        finally:
+            self.place_ms = {"search": times["place"][0] if "place" in times else None, "track": times.get("polish", [None])[0]}
 
     def run(self):
         """Runs the sequence and returns a summary: scans, keyframes, the wall time, and per stage the median host milliseconds per
@@ -761,8 +829,10 @@ class NeRFLOAM:
         m = self.mapper
         if m.map_state is None or m.trajectory.frame_poses or not m.trajectory.final_poses:
             raise RuntimeError("save_map: the run has not finished (call run() first)")
-        return SavedMap(m.map, m.decoder, dict(self.args.decoder_specs), np.stack(m.trajectory.final_poses).astype(np.float64),
-                        np.asarray(m.scan_ids, dtype=np.int64), map_config(self.args))
+        traj, ids = np.stack(m.trajectory.final_poses).astype(np.float64), np.asarray(m.scan_ids, dtype=np.int64)
+        if self.base is not None:
+            traj, ids = grown_trajectory(self.base, traj, ids)
+        return SavedMap(m.map, m.decoder, dict(self.args.decoder_specs), traj, ids, map_config(self.args))
 
     def save_map(self, path):
         """Writes the finished run's map to one file (write_map); localise.Localiser and load_map read it."""
@@ -771,6 +841,10 @@ class NeRFLOAM:
     def summary(self, wall_ms):
         times = {**self.tracker.times, **self.mapper.times}
         n = len(self.mapper.trajectory.final_poses)
-        return {"scans": n, "keyframes": len(self.mapper.keyframe_indices), "wall_ms": wall_ms, "ms_per_scan_wall": wall_ms / max(n, 1),
-                "ms_per_scan": {k: float(np.median(v)) for k, v in times.items() if k not in ("init", "refine")},
-                "init_ms": times.get("init", [0.0])[0], "refine_ms": times.get("refine", []), "out_dir": self.out_dir}
+        out = {"scans": n, "keyframes": len(self.mapper.keyframe_indices), "wall_ms": wall_ms, "ms_per_scan_wall": wall_ms / max(n, 1),
+               "ms_per_scan": {k: float(np.median(v)) for k, v in times.items() if k not in ("init", "refine")},
+               "init_ms": times.get("init", [0.0])[0], "refine_ms": times.get("refine", []), "out_dir": self.out_dir}
+        if self.base is not None:           # the first scan's placement and the saved map's size, rows held fixed
+            out["base"] = {"place_ms": self.place_ms, "frozen_rows": self.mapper.frozen_rows, "rows": int(self.mapper.map.n_rows),
+                           "nodes": int(self.mapper.map.n_nodes)}
+        return out
