@@ -779,6 +779,46 @@ NL_API int64_t nl_globalloc_select_workspace_bytes(int64_t n_placements, int32_t
 NL_API int nl_globalloc_select(int64_t n_placements, const int32_t *d_counts, int32_t n_points, int64_t n_select, void *d_ws, int64_t ws_bytes,
                                int32_t *d_ids, int32_t *d_sel_counts, void *stream);
 
+/* ============================================================================================
+ * 16. Change detection against a saved map (DESIGN.md section 11.7; csrc/changes.cu): for every saved voxel, how many rays of a
+ *     later drive pass through its surface in space the drive says is empty ("through") and how many end on it ("surface"); and
+ *     the voxels where the drive's returns land outside the map's leaves ("added").  Counts are u32 summed with integer atomics,
+ *     independent of launch order; the outputs of nl_change_finish are in node order and key order.  No reference counterpart:
+ *     the reference treats a map as true once it is built.
+ * ============================================================================================ */
+/* Votes from the sample list of one nl_render_samples call (rays r in [0, R)) after the decoder forward: d_s_ray, d_s_vox, d_s_depth,
+ * d_sdf f32[cap] and d_ray_offset i32[R] as that call and the forward left them, the measured depth d_gt f32[R] of each ray (the
+ * point's range).  The sample count is read from d_stats->n_samples, so nothing is read back.  A run is the samples of one ray in one
+ * voxel; over the union of a voxel's samples on a ray, with d = gt - depth (fp32): "through" when every d > through_depth
+ * (truncation + margin) and the smallest sdf <= 0, adding 1 to d_votes[v][0]; otherwise "surface" when some |d| <= truncation, adding
+ * 1 to d_votes[v][1].  d_votes u32[n_nodes][2].  When d_stats->error has bit1 or bit2 set, nothing is added and d_status i32[2] =
+ * (error & 6, n_samples); otherwise d_status is not written. */
+NL_API int nl_change_votes(int64_t cap, const nl_render_stats *d_stats, const int32_t *d_s_ray, const int32_t *d_s_vox, const float *d_s_depth,
+                           const float *d_sdf, const float *d_gt, const int32_t *d_ray_offset, int64_t n_nodes, float truncation,
+                           float through_depth, uint32_t *d_votes, int32_t *d_status, void *stream);
+/* The added table: d_keys u64[slots] (voxel keys of section 15, NL_HASH_EMPTY = ~0 in free slots) and d_vals u32[slots][3] =
+ * (points, distinct scans, last scan id); slots a power of two in [2^10, 2^30].  d_state u32[3] = (keys committed, keys inserted,
+ * overflow).  Clears the table and, with old_slots > 0, moves every key of the old table into it with its values (state counts
+ * kept); old_slots == 0 zeroes the counts.  The overflow word is cleared either way. */
+NL_API int nl_change_rehash(int64_t old_slots, const uint64_t *d_old_keys, const uint32_t *d_old_vals, int64_t slots, uint64_t *d_keys,
+                            uint32_t *d_vals, uint32_t *d_state, void *stream);
+/* One scan into the added table: each of d_points f32[n_points][3] (sensor frame) posed by d_Rt12 f32[12] (nl_pose_matrices' layout)
+ * whose voxel key (section 15's arithmetic) is not in the occupied set d_occ u64[occ_slots] adds 1 to its slot's points, and the
+ * scan count rises when the slot's last scan id is not `scan`.  Only when keys committed + n_points <= slots / 2; otherwise the call
+ * inserts nothing and sets the overflow word, and the caller rehashes into a larger table and calls again.  scan < 2^32 - 1. */
+NL_API int nl_change_added(int64_t n_points, const float *d_points, const float *d_Rt12, double voxel_size, int64_t grid_dim,
+                           const uint64_t *d_occ, int64_t occ_slots, int64_t slots, uint64_t *d_keys, uint32_t *d_vals, uint32_t scan,
+                           uint32_t *d_state, void *stream);
+NL_API int64_t nl_change_finish_workspace_bytes(int64_t n_nodes, int64_t slots);
+/* Classification and compaction.  A leaf (d_structure[i][8] == 1) is removed when through >= min_votes and through >= ratio x
+ * (through + surface) (fp64), confirmed when it has surface votes and is not removed, unobserved when it has no votes.  d_removed
+ * i32[n_nodes]: the removed node ids in ascending order; d_added u64[slots]: the keys with points >= min_points and scans >=
+ * min_scans in ascending order, then NL_HASH_EMPTY; d_added_vals u32[slots][2]: their (points, scans); d_totals i64[4] = (confirmed,
+ * removed, unobserved, added).  0 < ratio <= 1; the counts >= 1. */
+NL_API int nl_change_finish(int64_t n_nodes, const int32_t *d_structure, const uint32_t *d_votes, uint32_t min_votes, double ratio, int64_t slots,
+                            const uint64_t *d_keys, const uint32_t *d_vals, uint32_t min_points, uint32_t min_scans, void *d_ws, int64_t ws_bytes,
+                            int32_t *d_removed, uint64_t *d_added, uint32_t *d_added_vals, int64_t *d_totals, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

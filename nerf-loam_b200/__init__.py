@@ -29,6 +29,8 @@ Public surface (mirrors the reference, see INTEGRATION.md):
                                     NeRFLOAM.save_map / slam.load_map: the finished run's map, decoder and trajectory as one file
     localise.Localiser              a sequence localised in a saved map: the first scan placed by relocalise_global with no guess,
                                     the rest tracked by slam.Tracking against the frozen map
+    changes.ChangeDetector          what changed since a map was saved: the saved voxels a later drive sees through and the new
+                                    ground it hits, counted on the GPU (Localiser's "change_specs")
 Every device computation goes through the C ABI of libnerfloam_b200.so (include/nerfloam_b200.h); there is
 no CPU or eager-PyTorch fallback for the kernels.
 """
@@ -36,7 +38,7 @@ from . import _capi  # noqa: F401
 
 __all__ = ["svo", "grid", "lidar", "criterion", "se3pose", "frame", "render_helpers", "mapping", "engine", "synthetic", "dist", "dropin", "mesh", "share",
            "evaluate", "keyframes", "ground", "dataset", "track_batch", "track_frames", "score", "score_poses", "relocalise", "refine_map", "slam",
-           "globalloc", "relocalise_global", "localise"]
+           "globalloc", "relocalise_global", "localise", "changes"]
 
 
 def __getattr__(name):

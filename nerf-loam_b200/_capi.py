@@ -203,6 +203,12 @@ _SIGNATURES = {
                                      C.c_int64, vp, vp]),
     "nl_globalloc_select_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int64]),
     "nl_globalloc_select": (C.c_int, [C.c_int64, vp, C.c_int32, C.c_int64, vp, C.c_int64, vp, vp, vp]),
+    "nl_change_votes": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, C.c_int64, C.c_float, C.c_float, vp, vp, vp]),
+    "nl_change_rehash": (C.c_int, [C.c_int64, vp, vp, C.c_int64, vp, vp, vp, vp]),
+    "nl_change_added": (C.c_int, [C.c_int64, vp, vp, C.c_double, C.c_int64, vp, C.c_int64, C.c_int64, vp, vp, C.c_uint32, vp, vp]),
+    "nl_change_finish_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
+    "nl_change_finish": (C.c_int, [C.c_int64, vp, vp, C.c_uint32, C.c_double, C.c_int64, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_int64, vp, vp, vp,
+                                   vp, vp]),
 }
 
 # words of the device-side iteration control block (include/nerfloam_b200.h section 8)

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libnerfloam_b200.so")
-SOURCES = ["nl_error.cpp", "octree_host.cpp", "grid_dropin.cu", "render.cu", "gather.cu", "mlp.cu", "mlp_tc.cu", "pose.cu", "optim.cu", "mc.cu", "peer.cu", "select.cu", "octree_dev.cu", "eval.cu", "overlap.cu", "ground.cu", "refine.cu", "globalloc.cu"]
+SOURCES = ["nl_error.cpp", "octree_host.cpp", "grid_dropin.cu", "render.cu", "gather.cu", "mlp.cu", "mlp_tc.cu", "pose.cu", "optim.cu", "mc.cu", "peer.cu", "select.cu", "octree_dev.cu", "eval.cu", "overlap.cu", "ground.cu", "refine.cu", "globalloc.cu", "changes.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--extended-lambda", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 

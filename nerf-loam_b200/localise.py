@@ -21,6 +21,9 @@
     while scans stay lost, by the first scan's search over the whole saved trajectory.  A re-placement counts only if its own score
     passes the rule; otherwise the scan keeps its tracked pose and is reported lost.  After either, the motion model restarts from
     the last accepted scan.  The map is frozen, so a wrong decision changes one reported pose and nothing else.
+  * Changes (opt-in, config key "change_specs"; DESIGN.md §11.7): after the drive, every scan that is not lost goes to a
+    changes.ChangeDetector at its final pose, which reports the saved voxels the drive sees through (removed) and the voxels where its
+    returns land outside the map (added).  It reports and does not edit the map.
 
 Not covered here: updating the map (slam.NeRFLOAM's base_map grows a saved map with a later drive, placing its first scan with
 place_scan; DESIGN.md §11.6), loop closure.
@@ -38,6 +41,7 @@ import torch
 
 from . import _capi
 from . import render_helpers as rh
+from .changes import ChangeDetector, change_specs, write_changes
 from .frame import POSE_OFFSET, LidarFrame
 from .globalloc import relocalise_global
 from .score import relocalise, score_poses
@@ -166,12 +170,13 @@ def place_first(frame, map_state, decoder, tracker, anchors, global_specs, gener
     return res
 
 
-Localisation = namedtuple("Localisation", ["scan_ids", "poses", "loss", "hit_fraction", "placement", "status"])
+Localisation = namedtuple("Localisation", ["scan_ids", "poses", "loss", "hit_fraction", "placement", "status", "changes"])
 Localisation.__doc__ = """Localiser.run's result, per scan in order: scan_ids i64[S], poses f64[S,4,4] in the map frame without POSE_OFFSET
 (what frame_poses.txt holds), loss f64[S] and hit_fraction f64[S] (score_poses at the final pose), placement: the first scan's
 globalloc.GlobalResult (None when an init_pose was given), and status: with recovery on, a list of S codes from STATUSES ("tracked":
 the tracker's pose passed the lost rule, "local" / "global": re-placed by that step, "lost": nothing passed, the tracked pose is
-kept; the first scan is "tracked"), None with recovery off."""
+kept; the first scan is "tracked"), None with recovery off, and changes: with change detection on, the changes.Changes of every scan
+that is not lost, None with it off."""
 
 
 class FrozenMap:
@@ -197,9 +202,11 @@ class Localiser:
     config: overrides merged over the file's config, e.g. {"tracker_specs": {"num_iterations": 50}} or {"global_specs": {...}}
     (relocalise_global's settings, GLOBAL_SPECS); voxel_size is the map's and cannot change.  {"recovery_specs": {...}} turns
     recovery of lost scans on (RECOVERY_SPECS; {} for the defaults); without the key run() does what it did before recovery existed.
+    {"change_specs": {...}} turns change detection on (changes.CHANGE_SPECS; {} for the defaults); without it no detector is built.
     generator: a CPU torch.Generator every draw comes from (tracking's, and a seed for each search -- the first scan's and every
     recovery's -- which runs under a forked torch RNG); None draws from torch's global generators.  octree: where a map file is restored
-    ("host" or "device").  out_dir: where run() writes frame_poses.txt, and frame_status.txt with recovery on (None: nowhere)."""
+    ("host" or "device").  out_dir: where run() writes frame_poses.txt, frame_status.txt with recovery on and changes.write_changes
+    files with change detection on (None: nowhere)."""
 
     def __init__(self, saved, data_stream, config=None, generator=None, octree="host", out_dir=None):
         if not isinstance(saved, SavedMap):
@@ -218,6 +225,8 @@ class Localiser:
                                     mapper_specs={"voxel_size": float(cfg["voxel_size"])})
         self.global_specs = {**GLOBAL_SPECS, **cfg.get("global_specs", {})}
         self.recovery = recovery_specs(cfg["recovery_specs"]) if "recovery_specs" in cfg else None
+        self.change_specs = change_specs(cfg["change_specs"]) if "change_specs" in cfg else None
+        self.change_ms = []
         self.map_state = saved.map.map_states["_mapstate"]
         self.frozen = FrozenMap(self.map_state, saved.decoder)
         self.tracker = Tracking(self.args, data_stream, self.frozen, generator)
@@ -360,16 +369,34 @@ class Localiser:
                 with open(os.path.join(self.out_dir, "frame_status.txt"), "w") as fh:
                     fh.writelines(f"{i} {s}\n" for i, s in zip(scan_ids, status))
         self.times.update(tr.times)
+        changes = None if self.change_specs is None else self.detect_changes(frames, status)
         return Localisation(torch.tensor(scan_ids, dtype=torch.int64), poses,
                             torch.tensor([s[0] for s in scores], dtype=torch.float64), torch.tensor([s[1] for s in scores], dtype=torch.float64),
-                            placement, status)
+                            placement, status, changes)
+
+    def detect_changes(self, frames, status):
+        """Every frame whose status is not "lost" (every frame with recovery off) into a new ChangeDetector at its final pose; returns
+        its Changes and, with out_dir, writes them there.  change_ms gets each add_scan's host ms (ending in its read-back)."""
+        det = ChangeDetector(self.map_state, self.saved.decoder, self.tracker.voxel_size, self.args.criteria, self._tracking_kw(), self.change_specs)
+        self.change_ms = []
+        for i, f in enumerate(frames):
+            if status is not None and status[i] == "lost":
+                continue
+            t0 = time.perf_counter()
+            det.add_scan(f, f.pose)
+            self.change_ms.append((time.perf_counter() - t0) * 1e3)
+        changes = det.result()
+        if self.out_dir is not None:
+            write_changes(self.out_dir, changes)
+        return changes
 
     def summary(self, result):
         """A JSON-ready summary of run()'s result: scans, the map file's load time, median host ms per scan per stage (load, track,
         score; tracking's stages end in a read-back), the first scan's placement (ms, stage times, placements searched), the median
         loss and the smallest hit fraction.  The placement's ms is the relocalise_global call; its track_ms the tracking from it.  With
         recovery on, "recovery": the scans per status and the median ms of a local and of a global step (each with the score of its
-        pose; None where the step never ran)."""
+        pose; None where the step never ran).  With change detection on, "changes": the scans added, the confirmed, removed,
+        unobserved and added voxel totals and the median ms of an add_scan."""
         p = result.placement
         place = None
         if p is not None:
@@ -383,4 +410,8 @@ class Localiser:
             out["recovery"] = {"counts": {s: result.status.count(s) for s in STATUSES},
                                "ms": {s: float(np.median(self.times[f"recover_{s}"])) if f"recover_{s}" in self.times else None
                                       for s in ("local", "global")}}
+        if result.changes is not None:
+            c = result.changes
+            out["changes"] = {"scans": c.n_scans, "confirmed": c.n_confirmed, "removed": c.n_removed, "unobserved": c.n_unobserved,
+                              "added": int(len(c.added_centres)), "ms_per_scan": float(np.median(self.change_ms)) if self.change_ms else None}
         return out
