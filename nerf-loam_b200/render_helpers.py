@@ -12,6 +12,7 @@ Behavioural notes (also in DESIGN.md):
     (voxel_helpers.py:531-533; render_helpers.py:190-318);
   * the unused autograd.grad(sdf, xyz) of render_helpers.py:293-297 is not computed.
 """
+import gc
 import numbers
 import os
 import threading
@@ -56,9 +57,22 @@ def _graph_capture(graph):
     """torch.cuda.graph for the captured loops.  capture_error_mode="thread_local": in the default "global" mode a capture on one host
     thread makes the other thread's stream synchronisations and read-backs fail (slam.NeRFLOAM runs the tracker and the mapper on two
     threads); a single thread behaves the same in either mode.  The lock keeps two captures from running at once: torch.cuda.graph
-    shares one capture stream between threads, and entering a capture synchronises the device and empties the allocator's cache."""
-    with _CAPTURE_LOCK, torch.cuda.graph(graph, capture_error_mode="thread_local"):
-        yield
+    shares one capture stream between threads, and entering a capture synchronises the device and empties the allocator's cache.
+
+    The cyclic garbage collector is run before the capture and kept off during it.  A dropped graph object (_RefineGraph keeps its
+    body, which refers back to it) is freed only by that collector, and with it its engine's pinned read-back buffers; freeing a pinned
+    buffer records an event on the stream that last copied through it, the legacy default stream, which invalidates a capture in
+    progress.  Left to run inside a capture, the collector made the capture fail whenever it happened to collect such a graph."""
+    with _CAPTURE_LOCK:
+        gc.collect()
+        enabled = gc.isenabled()
+        gc.disable()
+        try:
+            with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+                yield
+        finally:
+            if enabled:
+                gc.enable()
 
 
 def _seed_from_torch(generator=None):
