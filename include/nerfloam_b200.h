@@ -127,9 +127,8 @@ NL_API int nl_octree_restore(nl_octree *t, const int32_t *h_child, const uint64_
  *     Workspace for n points with L = log2(grid_dim), P = 8n, T = sum_{d=1..L} min(P, 8^d) (bound on the new nodes):
  *       bytes = max(42 P + 8 + 33 T + sort/scan scratch,  4 (P + 2n) + (T + P + 2n) + 68 n + 4 + sort/select/scan scratch), each array
  *       256-byte aligned; the CUB scratch is queried for the current device, so only this call gives the exact figure.
- *     Unlike nl_octree_insert, which inserts the points before a bad one and then fails, a batch with any coordinate outside
- *     [0, grid_dim-2] is rejected as a whole: d_counts[0] = 1 and nothing is written to the tree by insert_count; the caller
- *     then does not call insert_commit.
+ *     Like nl_octree_insert, a batch with any coordinate outside [0, grid_dim-2] is rejected as a whole: d_counts[0] = 1 and
+ *     nothing is written to the tree by insert_count; the caller then does not call insert_commit.
  * ============================================================================================ */
 NL_API int64_t nl_devoctree_workspace_bytes(int64_t n_points, int64_t grid_dim);
 /* Octree::insert octree.cpp:51-111, step 1 (reads the tree only): validate the batch d_vox i32[n,3] (n <= 2^23), find the nodes

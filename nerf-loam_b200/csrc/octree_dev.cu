@@ -186,7 +186,8 @@ __global__ void k_corners(int n, int L, int size, const int32_t *__restrict__ vo
     const uint64_t none = uint64_t(1) << (3 * L);
     const int px = vox[3 * i], py = vox[3 * i + 1], pz = vox[3 * i + 2];
     vals[p] = (uint32_t)p;
-    if (px < 0 || py < 0 || pz < 0 || px + 1 >= size || py + 1 >= size || pz + 1 >= size) {
+    // (not `px + 1 >= size`: for px = INT32_MAX that overflows, and the point would pass and alias into the grid)
+    if (px < 0 || py < 0 || pz < 0 || px >= size - 1 || py >= size - 1 || pz >= size - 1) {
         counts[0] = 1;                      // the batch is rejected after the read-back; nothing below modifies the tree
         keys[p] = none; dm[p] = (uint8_t)(L + 1); enode[p] = -1; eparent[p] = -1;
         return;

@@ -161,12 +161,14 @@ int nl_octree_insert(nl_octree *t, const int32_t *vox, int64_t n) {
     const unsigned shift = (unsigned)(kMaxBits - t->max_level - 1);  // octree.cpp:79
     std::vector<uint64_t> lvl_mask((size_t)t->max_level + 1);
     for (int d = 1; d <= t->max_level; ++d) lvl_mask[d] = level_mask(d + (int)shift);
+    for (int64_t i = 0; i < n * 3; ++i) {
+        // The reference silently wraps such coordinates through the bit masks; refuse the whole batch, before any point of it
+        // changes the tree, instead of corrupting it.
+        if (vox[i] < 0 || vox[i] >= t->size - 1)
+            return nl_set_error("nl_octree_insert: voxel coordinate outside [0, grid_dim-2]; the batch was rejected and the tree is unchanged");
+    }
     for (int64_t i = 0; i < n; ++i) {
         const int px = vox[i * 3 + 0], py = vox[i * 3 + 1], pz = vox[i * 3 + 2];
-        if (px < 0 || py < 0 || pz < 0 || px + 1 >= t->size || py + 1 >= t->size || pz + 1 >= t->size) {
-            // The reference silently wraps such coordinates through the bit masks; refuse instead of corrupting.
-            return nl_set_error("nl_octree_insert: voxel coordinate outside [0, grid_dim-2]");
-        }
         if (!t->seen_points.insert(morton(px, py, pz))) continue;
         for (int j = 0; j < 8; ++j) {
             const int x = px + kIncX[j], y = py + kIncY[j], z = pz + kIncZ[j];

@@ -276,7 +276,7 @@ class DeviceOctree(_ReferenceMethods):
     exports and counts as the host tree bit for bit, without copying the batch or the tree to the host.
 
     `insert` accepts CPU or CUDA int32 [N,3] and reads back two counters (the rejection flag and the number of new nodes, to grow
-    the capacity-doubling node arrays).  Unlike the host tree, a batch with a coordinate outside [0, grid_dim-2] is rejected as a
+    the capacity-doubling node arrays).  Like the host tree, it rejects a batch with a coordinate outside [0, grid_dim-2] as a
     whole (NerfLoamError) and leaves the tree unchanged.  `export_map` returns CPU tensors like `Octree.export_map`;
     `export_dirty` (numpy, like the host) and `update_map` (straight into a MapUpdater's device buffers) export the rows changed
     since the last dirty export.  `get_centres_and_children`, `get_voxels` and `get_leaf_voxels` return the host tree's CPU
