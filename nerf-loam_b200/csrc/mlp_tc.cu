@@ -21,8 +21,9 @@
 //   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c
 // h1 = relu(x W0^T + b0) is not stored: its input x (K = 16, 64 B per sample) is, and recomputing h1 costs a tenth of G.  One
 // split-K kernel (k_wgrad_tc) recomputes h1 and forms G on wgmma, both transposed so that the sample is wgmma's K: h1^T = W0 x^T
-// with A = W0 from registers and B = x (K-major as stored), then G^T = (dsdf h1)^T m2 with A = the h1^T accumulator from
-// registers and B = the exact 0/1 mask expanded into a K-major tile.  The column sums c and gb2 run beside it.
+// with A = W0 from registers and B = x (K-major as stored), then G^T = (dsdf h1)^T m2 on fp16 wgmma with A = the h1^T accumulator
+// from registers (each row scaled by a power of two into fp16's range and split into hi + lo) and B = the exact 0/1 mask expanded
+// into a K-major tile.  The column sums c and gb2 run beside it.
 #include <mutex>
 
 #include "loss.cuh"
@@ -167,13 +168,6 @@ __device__ __forceinline__ void wgmma_n16(float (&d)[8], uint32_t a0, uint32_t a
         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1));
 }
 // D = A x B (scale-d = 0: the accumulator's previous contents are not read) and D += A x B, as used by k_wgrad_tc
-__device__ __forceinline__ void wgmma_n128_z(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
-        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31]), "=f"(d[32]), "=f"(d[33]), "=f"(d[34]), "=f"(d[35]), "=f"(d[36]), "=f"(d[37]), "=f"(d[38]), "=f"(d[39]), "=f"(d[40]), "=f"(d[41]), "=f"(d[42]), "=f"(d[43]), "=f"(d[44]), "=f"(d[45]), "=f"(d[46]), "=f"(d[47]), "=f"(d[48]), "=f"(d[49]), "=f"(d[50]), "=f"(d[51]), "=f"(d[52]), "=f"(d[53]), "=f"(d[54]), "=f"(d[55]), "=f"(d[56]), "=f"(d[57]), "=f"(d[58]), "=f"(d[59]), "=f"(d[60]), "=f"(d[61]), "=f"(d[62]), "=f"(d[63])
-        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(0));
-}
 __device__ __forceinline__ void wgmma_n64_z(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
@@ -186,6 +180,23 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint32_t a0, uint32_t 
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1));
+}
+
+// D (=, +=) A x B in fp16 (m64n128k16, fp32 accumulation), as used by k_wgrad_tc for G: A register i holds two adjacent K
+// columns (lower K in the lower half) of row g + 8 (i & 1), columns 2t + 8 (i >> 1); B K-major (imm-trans-b = 0)
+__device__ __forceinline__ void wgmma_f16_n128_z(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31]), "=f"(d[32]), "=f"(d[33]), "=f"(d[34]), "=f"(d[35]), "=f"(d[36]), "=f"(d[37]), "=f"(d[38]), "=f"(d[39]), "=f"(d[40]), "=f"(d[41]), "=f"(d[42]), "=f"(d[43]), "=f"(d[44]), "=f"(d[45]), "=f"(d[46]), "=f"(d[47]), "=f"(d[48]), "=f"(d[49]), "=f"(d[50]), "=f"(d[51]), "=f"(d[52]), "=f"(d[53]), "=f"(d[54]), "=f"(d[55]), "=f"(d[56]), "=f"(d[57]), "=f"(d[58]), "=f"(d[59]), "=f"(d[60]), "=f"(d[61]), "=f"(d[62]), "=f"(d[63])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(0));
+}
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1));
 }
 
@@ -229,6 +240,16 @@ __device__ __forceinline__ void split_finite(float v, uint32_t &hi, uint32_t &lo
     hi = tf32_rna_finite(v);
     lo = tf32_rna_finite(v - __uint_as_float(hi));
 }
+// v0, v1 as fp16 pairs hi + lo (v0 in the lower halves): hi = rn(v), lo = rn(v - hi); v - hi is exact in fp32
+__device__ __forceinline__ void split_f16x2(float v0, float v1, uint32_t &hi, uint32_t &lo) {
+    float h0, h1;
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(v1), "f"(v0));
+    asm("{\n\t.reg .f16 a, b;\n\tmov.b32 {a, b}, %2;\n\tcvt.f32.f16 %0, a;\n\tcvt.f32.f16 %1, b;\n\t}" : "=f"(h0), "=f"(h1) : "r"(hi));
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(v1 - h1), "f"(v0 - h0));
+}
+// s with mx 2^s in [2^14, 2^15) for mx >= 0 (s = 0 for mx = 0), at most 126 so that 2^s and 2^-s are normal floats
+__device__ __forceinline__ int f16_shift(float mx) { return mx == 0.f ? 0 : min(141 - (int)(__float_as_uint(mx) >> 23), 126); }
+__device__ __forceinline__ float exp2_int(int s) { return __uint_as_float((uint32_t)(127 + s) << 23); }
 
 // ------------------------------------------------------------------------------------------------
 // Weight panels: the exact shared-memory image (K-major, 128B swizzle, K permuted by kperm, tf32 hi then lo) of every
@@ -739,18 +760,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
 //   gW1 = diag(w2) G   gW2[j] = sum_k W1[j,k] G[j,k] + b1[j] c[j]   gb1 = w2 * c   gb2 = sum_s dsdf
 // (gW0 = dh1^T x and gb0 = sum_s dh1 are formed by the training kernel, where dh1 is.)
 // Grid = 4 tiles x nsplit (one CTA per SM), split-K over samples.  CTA (tile, split) owns the 128 x 128 tile (k0, j0) of G^T.
-// The reduction index is the sample, and wgmma's tf32 forms take
-// B only as K-major shared memory and A from registers or K-major shared memory, so G is formed transposed with K = samples,
-// G^T[k, j] = sum_s (dsdf * h1)^T[k, s] m2[s, j]: A comes from registers and B, the mask, is rebuilt per chunk as a K-major tile.
+// The reduction index is the sample, and wgmma takes A from registers or K-major shared memory and B from shared memory, so G is
+// formed transposed with K = samples, G^T[k, j] = sum_s (dsdf * h1)^T[k, s] m2[s, j]: A comes from registers and B, the mask, is
+// rebuilt per chunk as a K-major tile.
 // Warpgroup w owns rows k0 + 64 w .. +63 (wgmma M = 64) and all 128 columns j.  Per chunk of WG_KC = 64 samples it
 //   1. recomputes h1^T[k, s] = W0[k, :] x[s, :]^T (N = 64 samples, K = 16) with 3xTF32 wgmma, terms in the training kernel's
 //      order: A = the tf32 hi / lo parts of W0 that the training kernel multiplies (the layer-1 panel), held in 16 registers for
-//      the whole kernel; B = the chunk's x split into hi / lo tiles (x's own [s][e] rows are K-major);
-//   2. forms dsdf * relu(h1^T + b0) in the accumulator registers (b0 per row, dsdf per column) and splits it into hi / lo.  An
-//      accumulator fragment is the A fragment of the next GEMM once K is permuted inside every group of 8 (kperm), so the mask
-//      tile stores its samples in kperm order;
-//   3. accumulates G^T with 2 terms (the mask is exact in tf32): A from the registers of step 2, B = the mask expanded from its bits
-//      into a [128 j][64 s] tile of 0 / 1.0f (K-major, 128-byte swizzle, two K-blocks of 32 samples), shared by both warpgroups.
+//      the whole kernel; B = the chunk's x split into hi / lo tiles (x's own [s][e] rows are K-major).  This is the training
+//      kernel's z1, so both kernels agree on every relu'(h1);
+//   2. forms v = dsdf * relu(h1^T + b0) in the accumulator registers (b0 per row, dsdf per column), scales each row by the power
+//      of two 2^s that puts the row's largest |v| over the chunk in [2^14, 2^15), and splits it into fp16 hi = rn(v 2^s) and
+//      lo = rn(v 2^s - hi).  fp16 has tf32's 11 significant bits, so hi + lo is v 2^s to 2^-22 relative while lo is normal and to
+//      2^-25 absolute (2^-39 of the row's maximum) below; the scaling is exact, and it is what keeps the row inside fp16's range.
+//      Columns 16 kk .. 16 kk + 15 of the n64 accumulator fragment are, as they stand, the fp16 A fragment of k-step kk;
+//   3. accumulates G^T with 2 fp16 terms (hi m2 + lo m2; the mask is exact in fp16, and fp16 products are exact in the fp32
+//      accumulator): A from the registers of step 2, B = the mask expanded from its bits into a [128 j][64 s] tile of 0 / 1.0
+//      halves (K-major, 128-byte swizzle: one 128-byte row per j), shared by both warpgroups.  The chunk's rows are scaled back by
+//      2^-s as they are added into the running sums.
 // While the G wgmmas run, the warps form the column sums c (the k0 = 0 tiles) and gb2 (tile 0), and build the next chunk's x and
 // mask tiles into the other of two tile buffers.  x, the mask rows and dsdf stream through a WG_NS-slot shared-memory ring filled
 // by cp.async WG_NS - 1 chunks ahead; one __syncthreads per chunk publishes the next chunk's data and tiles.
@@ -765,11 +791,11 @@ constexpr int WG_KC = 64, WG_NS = 4;
 constexpr int WG_LDX = 20;     // x rows in the ring: fragment loads (row g, column t) hit 32 distinct banks
 constexpr int WG_OM = WG_KC * WG_LDX, WG_OD = WG_OM + WG_KC * 8;   // slot: x | mask rows | dsdf
 constexpr int WG_SLOT = WG_OD + WG_KC;                             // floats
-constexpr int WG_MT = (WG_KC / 32) * HALF;   // mask tile: K-blocks of 32 samples, 128 rows (j) x 128 B each
+constexpr int WG_MT = 128 * 128;             // mask tile: 128 rows (j) x 64 fp16 samples
 constexpr int WG_XT = WG_KC * 128;           // x tile (hi or lo): a 128-byte row per sample, the 16 features in its first 64 B
-constexpr int WG_SMEM = 2 * (WG_MT + 2 * WG_XT) + WG_NS * WG_SLOT * 4 + 1024;   // 126 KB: 2 tile buffers, ring, alignment slack
+constexpr int WG_SMEM = 2 * (WG_MT + 2 * WG_XT) + WG_NS * WG_SLOT * 4 + 1024;   // 94 KB: 2 tile buffers, ring, alignment slack
 static_assert(WG_OM % 4 == 0 && WG_OD % 4 == 0 && WG_SLOT % 4 == 0, "cp.async 16-byte destinations");
-static_assert(WG_KC == 64, "the loaders and the x-tile build assign one 16-byte piece of x per thread");
+static_assert(WG_KC == 64, "the loaders and the x-tile build assign one 16-byte piece of x per thread, a mask row is 128 bytes");
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
@@ -841,9 +867,9 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
-    // x hi / lo and mask tiles of the chunk in ring slot `sl` into tile buffer b.  Thread tid writes mask tile row bj for the
-    // samples of parity bh: positions 4 bh .. 4 bh + 3 of sample group q hold samples 8q + bh + 2i (kperm).  The k0 = 0 tiles also
-    // add those samples' dsdf into c[j0 + bj] here.
+    // x hi / lo and mask tiles of the chunk in ring slot `sl` into tile buffer b.  Thread tid writes mask tile row bj for samples
+    // 32 bh .. 32 bh + 31, in sample order (16-byte pieces 4 bh .. 4 bh + 3 of the row).  The k0 = 0 tiles also add those samples'
+    // dsdf into c[j0 + bj] here.
     const int bj = tid & 127, bh = tid >> 7, bw = m2_word(bj) + (j0 >> 7), bb = m2_bit(bj);
     auto build = [&](const float *sl, int b) {
         {
@@ -861,16 +887,16 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
         uint8_t *mt = tiles + b * WG_MT;
         float sc = 0.f;
 #pragma unroll
-        for (int q = 0; q < WG_KC / 8; ++q) {
+        for (int q = 4 * bh; q < 4 * bh + 4; ++q) {
             uint32_t f[4];
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                const int s = 8 * q + 2 * i + bh;
-                const bool on = (Ms[s * 8 + bw] >> bb) & 1u;
-                f[i] = on ? 0x3f800000u : 0u;
-                if (k0 == 0) sc += on ? Ds[s] : 0.f;
+                const int s = 8 * q + 2 * i;
+                const bool on0 = (Ms[s * 8 + bw] >> bb) & 1u, on1 = (Ms[(s + 1) * 8 + bw] >> bb) & 1u;
+                f[i] = (on0 ? 0x3C00u : 0u) | (on1 ? 0x3C000000u : 0u);
+                if (k0 == 0) { sc += on0 ? Ds[s] : 0.f; sc += on1 ? Ds[s + 1] : 0.f; }
             }
-            *reinterpret_cast<uint4 *>(mt + (q >> 2) * HALF + panel_off(bj, 2 * (q & 3) + bh)) = make_uint4(f[0], f[1], f[2], f[3]);
+            *reinterpret_cast<uint4 *>(mt + panel_off(bj, q)) = make_uint4(f[0], f[1], f[2], f[3]);
         }
         c_acc += sc;
     };
@@ -905,29 +931,47 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
         wg_commit_wait();
         wg_fence_acc(d1);
 
-        // ---- 2. A fragments of k-step kk (samples 8 kk .. +7; K position q <-> sample 8 kk + kperm(q)) of dsdf * relu(h1^T + b0) ----
-        uint32_t ah[WG_KC / 8][4], al[WG_KC / 8][4];
+        // ---- 2. fp16 A fragments of k-step kk (samples 16 kk .. +15) of 2^s dsdf * relu(h1^T + b0), s per row ----
+        uint32_t ah[WG_KC / 16][4], al[WG_KC / 16][4];
+        float inv_a, inv_b;   // 2^-s of rows kr, kr + 8
         {
             const float *Ds = sl + WG_OD;
+            float ma = 0.f, mb = 0.f;
 #pragma unroll
-            for (int kk = 0; kk < WG_KC / 8; ++kk) {
-                const float2 ds = *reinterpret_cast<const float2 *>(Ds + 8 * kk + 2 * t);
-                const float v0 = d1[4 * kk] + b0a, v1 = d1[4 * kk + 1] + b0a, v2 = d1[4 * kk + 2] + b0b, v3 = d1[4 * kk + 3] + b0b;
-                const float v[4] = {ds.x * (v0 > 0.f ? v0 : 0.f), ds.x * (v2 > 0.f ? v2 : 0.f), ds.y * (v1 > 0.f ? v1 : 0.f),
-                                    ds.y * (v3 > 0.f ? v3 : 0.f)};
-                split4(v, ah[kk], al[kk]);
+            for (int j = 0; j < WG_KC / 8; ++j) {   // d1[4 j + x]: row kr + 8 (x >> 1), sample 8 j + 2t + (x & 1)
+                const float2 ds = *reinterpret_cast<const float2 *>(Ds + 8 * j + 2 * t);
+                const float v0 = d1[4 * j] + b0a, v1 = d1[4 * j + 1] + b0a, v2 = d1[4 * j + 2] + b0b, v3 = d1[4 * j + 3] + b0b;
+                d1[4 * j] = ds.x * (v0 > 0.f ? v0 : 0.f);
+                d1[4 * j + 1] = ds.y * (v1 > 0.f ? v1 : 0.f);
+                d1[4 * j + 2] = ds.x * (v2 > 0.f ? v2 : 0.f);
+                d1[4 * j + 3] = ds.y * (v3 > 0.f ? v3 : 0.f);
+                ma = fmaxf(ma, fmaxf(fabsf(d1[4 * j]), fabsf(d1[4 * j + 1])));
+                mb = fmaxf(mb, fmaxf(fabsf(d1[4 * j + 2]), fabsf(d1[4 * j + 3])));
+            }
+            ma = fmaxf(ma, __shfl_xor_sync(0xffffffffu, ma, 1)); ma = fmaxf(ma, __shfl_xor_sync(0xffffffffu, ma, 2));
+            mb = fmaxf(mb, __shfl_xor_sync(0xffffffffu, mb, 1)); mb = fmaxf(mb, __shfl_xor_sync(0xffffffffu, mb, 2));
+            const int sa = f16_shift(ma), sb = f16_shift(mb);
+            const float ua = exp2_int(sa), ub = exp2_int(sb);
+            inv_a = exp2_int(-sa); inv_b = exp2_int(-sb);
+#pragma unroll
+            for (int kk = 0; kk < WG_KC / 16; ++kk) {
+                const float *v = d1 + 8 * kk;
+                split_f16x2(v[0] * ua, v[1] * ua, ah[kk][0], al[kk][0]);   // row kr, samples 16 kk + 2t, + 1
+                split_f16x2(v[2] * ub, v[3] * ub, ah[kk][1], al[kk][1]);   // row kr + 8
+                split_f16x2(v[4] * ua, v[5] * ua, ah[kk][2], al[kk][2]);   // row kr, samples 16 kk + 8 + 2t, + 1
+                split_f16x2(v[6] * ub, v[7] * ub, ah[kk][3], al[kk][3]);   // row kr + 8
             }
         }
 
-        // ---- 3. this chunk's G^T = (dsdf h1)^T m2, left running while the warps do the rest ----
+        // ---- 3. this chunk's 2^s G^T = (2^s dsdf h1)^T m2, left running while the warps do the rest ----
         float part[64];
         wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < WG_KC / 8; ++kk) {
-            const uint64_t bd = md + (kk >> 2) * (HALF >> 4) + 2 * (kk & 3);
-            if (kk == 0) wgmma_n128_z(part, ah[0][0], ah[0][1], ah[0][2], ah[0][3], bd);
-            else wgmma_n128(part, ah[kk][0], ah[kk][1], ah[kk][2], ah[kk][3], bd);
-            wgmma_n128(part, al[kk][0], al[kk][1], al[kk][2], al[kk][3], bd);
+        for (int kk = 0; kk < WG_KC / 16; ++kk) {
+            const uint64_t bd = md + 2 * kk;
+            if (kk == 0) wgmma_f16_n128_z(part, ah[0][0], ah[0][1], ah[0][2], ah[0][3], bd);
+            else wgmma_f16_n128(part, ah[kk][0], ah[kk][1], ah[kk][2], ah[kk][3], bd);
+            wgmma_f16_n128(part, al[kk][0], al[kk][1], al[kk][2], al[kk][3], bd);
         }
         asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 
@@ -939,7 +983,7 @@ __global__ void __launch_bounds__(256, 1) k_wgrad_tc(long long M_host, const int
         asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
         wg_fence_acc(part);
 #pragma unroll
-        for (int i = 0; i < 64; ++i) tot[i] += part[i];
+        for (int i = 0; i < 64; ++i) tot[i] = fmaf(part[i], (i & 2) ? inv_b : inv_a, tot[i]);   // the product is exact
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (split >= nch) return;
