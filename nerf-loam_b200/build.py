@@ -31,18 +31,22 @@ def _stale(target, deps):
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False):
-    os.makedirs(OBJ, exist_ok=True)
+def build(force=False, verbose=False, defines=(), out_dir=None):
+    """Compile into _obj/ and libnerfloam_b200.so beside this file, or, with out_dir, into out_dir/_obj and
+    out_dir/libnerfloam_b200.so (a variant built with extra -D defines, such as the phase stamps)."""
+    obj = os.path.join(out_dir, "_obj") if out_dir else OBJ
+    lib = os.path.join(out_dir, "libnerfloam_b200.so") if out_dir else LIB
+    os.makedirs(obj, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
     headers.append(os.path.join(os.path.dirname(HERE), "include", "nerfloam_b200.h"))
     objs = []
     procs = []
     for src in SOURCES:
         s = os.path.join(CSRC, src)
-        o = os.path.join(OBJ, os.path.splitext(src)[0] + ".o")
+        o = os.path.join(obj, os.path.splitext(src)[0] + ".o")
         objs.append(o)
         if force or _stale(o, [s] + headers):
-            cmd = [_nvcc()] + ARCH + FLAGS + ["-c", s, "-o", o]
+            cmd = [_nvcc()] + ARCH + FLAGS + ["-D" + d for d in defines] + ["-c", s, "-o", o]
             if verbose:
                 print(" ".join(cmd))
             procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
@@ -56,12 +60,12 @@ def build(force=False, verbose=False):
             sys.stdout.write(out.decode())
     if failed:
         raise RuntimeError("nvcc failed")
-    if force or procs or _stale(LIB, objs):
-        cmd = [_nvcc()] + ARCH + ["-shared", "-o", LIB] + objs + ["-cudart", "static"]
+    if force or procs or _stale(lib, objs):
+        cmd = [_nvcc()] + ARCH + ["-shared", "-o", lib] + objs + ["-cudart", "static"]
         if verbose:
             print(" ".join(cmd))
         subprocess.check_call(cmd)
-    return LIB
+    return lib
 
 
 SVO_LIB = os.path.join(HERE, "svo_b200.so")

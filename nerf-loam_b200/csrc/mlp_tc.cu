@@ -9,6 +9,8 @@
 //   * B operands (weights, pre-split into tf32 hi/lo and pre-swizzled into the 128B-swizzle K-major image wgmma reads,
 //     k_tc_prepare) stream from L2 through a 4-slot shared-memory ring: 1-D bulk copies (TMA) completing on mbarriers,
 //     issued by thread 0 up to 3 slots ahead; a slot is refilled once the wgmmas of all 8 warps that read it retired.
+//   * The K = 256 GEMMs are software-pipelined in commit groups of 2 k-steps (wgmma.wait_group 1): a warpgroup builds its next
+//     A fragments and waits for the ring while its previous group runs (gemm in k_mlp_wg).
 //   * Every N = 256 GEMM runs as two N = 128 halves, so the previous layer's activations (128 registers per thread) and
 //     one accumulator half (64) fit in the register file together.
 // Per 128-sample training tile the ring carries 42 items: layer 1 (2 halves), layer 2 (2 halves x 8 K-blocks of 32),
@@ -25,6 +27,7 @@
 // from registers (each row scaled by a power of two into fp16's range and split into hi + lo) and B = the exact 0/1 mask expanded
 // into a K-major tile.  The column sums c and gb2 run beside it.
 #include <mutex>
+#include <type_traits>
 
 #include "loss.cuh"
 #include "nl_cuda.cuh"
@@ -149,9 +152,13 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// every commit group of this warpgroup but the N committed last has completed
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void wg_commit_wait() {
-    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    wg_commit();
+    wg_wait<0>();
 }
 __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
     asm volatile(
@@ -319,6 +326,14 @@ __device__ __forceinline__ uint32_t m2_pack(uint32_t m) {
     return (m | (m >> 8)) & 0x0000FFFFu;
 }
 
+// Phase breakdown of k_mlp_wg (scripts/time_decoder_phases.py builds a copy of the library with -DNL_TC_STAMPS; without it the
+// stamps compile to nothing).  Thread 0 of each warpgroup adds the clock64() cycles since its previous stamp to the counter of the
+// phase the stamp closes, in shared memory beside the ring's mbarriers, and adds its counters into tc_stamps at kernel end.
+enum StampPhase { PH_RING, PH_ABUILD, PH_WAIT, PH_EPI1, PH_EPI2, PH_LOSS, PH_WGRAD, PH_REST, NPH };
+#ifdef NL_TC_STAMPS
+__device__ unsigned long long tc_stamps[2][NPH];
+#endif
+
 // ring item i of a tile -> panel stage and N half
 __device__ __forceinline__ void item_of(int i, int &stage, int &half) {
     if (i < 2) { stage = 0; half = i; }
@@ -365,7 +380,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
         for (int s = 0; s < NSLOT; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+#ifdef NL_TC_STAMPS
+    static_assert(16 * NSLOT + 2 * NPH * 8 <= 256, "the phase counters share the mbarriers' 256 bytes");
+    unsigned long long *st_acc = reinterpret_cast<unsigned long long *>(sm + SM_BAR + 16 * NSLOT) + NPH * (tid >> 7);
+    if ((tid & 127) == 0)
+        for (int i = 0; i < NPH; ++i) st_acc[i] = 0ull;
+#endif
     __syncthreads();
+#ifdef NL_TC_STAMPS
+    long long st_last = clock64();
+    auto stamp = [&](int ph) {
+        if ((tid & 127) == 0) { const long long now = clock64(); st_acc[ph] += (unsigned long long)(now - st_last); st_last = now; }
+    };
+#else
+    auto stamp = [](int) {};
+#endif
 
     // thread 0 feeds the ring: item n is always issued before anyone waits for it; items up to n + NSLOT - 1 are issued
     // when their slot is already free (non-blocking test), so the copies run ahead of the MMAs
@@ -381,7 +410,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
         bulk_g2s(ring + s * SLOT, src, bytes, FULL(s));
         bulk_g2s(ring + s * SLOT + HALF, src + PANEL_B, bytes, FULL(s));
     };
-    uint32_t n = 0;   // ring items consumed by this thread
+    uint32_t n = 0, nrel = 0;   // ring items acquired / released by this thread
     // wait for item n; returns the descriptors of its hi and lo halves.  The caller computes its A fragments first and then
     // issues wgmma.fence (registers written after the fence may not feed the wgmmas behind it)
     auto acquire = [&](uint64_t &bh, uint64_t &bl) {
@@ -396,12 +425,46 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
         mbar_wait(FULL(s), (n / NSLOT) & 1);
         bh = make_desc(ring + s * SLOT);
         bl = make_desc(ring + s * SLOT + HALF);
-    };
-    auto release = [&]() {
-        wg_commit_wait();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(EMPTY(n % NSLOT));
         ++n;
+    };
+    // the oldest acquired item's slot is free again: the caller has waited for every wgmma that read it
+    auto release = [&]() {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(EMPTY(nrel % NSLOT));
+        ++nrel;
+    };
+    // A GEMM of NG / 2 ring items (K-blocks of 4 k-steps), software-pipelined in NG commit groups of 2 k-steps: group q runs k-steps
+    // 2 (q & 1), + 1 of item q / 2 with the A fragments in set q & 1.  build(q) forms group q's fragments and mma(q, bh, bl) issues
+    // its wgmmas, in the order an unpipelined K-block would.  Once group q - 1 is committed, wgmma.wait_group 1 retires group q - 2,
+    // and group q is built into the registers q - 2 read while q - 1 runs, so a warpgroup keeps a group on the tensor pipe while it
+    // splits its next activations or waits for the ring.  An item is released when its second group has retired, one group after
+    // the next item was acquired.  That cannot deadlock the ring: when thread 0 acquires item n, its own warpgroup still holds only
+    // item n - 1 (its second group in flight) and has released n - 2 and everything before, while the one blocking wait in the feed
+    // is for item n's slot, last held by item n - NSLOT.  The other warpgroup needs nothing from thread 0 to release n - NSLOT: every
+    // item up to n - 1 was issued before thread 0 came here.  The last group is waited for (wait_group 0) before gemm returns, so
+    // the accumulators may be read after it.
+    auto gemm = [&](auto ng, auto &&build, auto &&mma) {
+        constexpr int NG = decltype(ng)::value;
+        static_assert(NG % 2 == 0, "two commit groups per ring item");
+        uint64_t bh = 0, bl = 0;
+#pragma unroll
+        for (int q = 0; q < NG; ++q) {
+            if (q >= 2) {
+                wg_wait<1>();
+                if (q & 1) release();
+                stamp(PH_WAIT);
+            }
+            build(q);
+            stamp(PH_ABUILD);
+            if (!(q & 1)) { acquire(bh, bl); stamp(PH_RING); }
+            wg_fence();
+            mma(q, bh, bl);
+            wg_commit();
+            stamp(PH_REST);
+        }
+        wg_wait<0>();
+        release();
+        stamp(PH_WAIT);
     };
 
     const float b2 = p.b2[0];
@@ -427,16 +490,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
 #pragma unroll
             for (int i = 0; i < 128; ++i) h[i] = 0.f;
             uint32_t ah[2][4], al[2][4];
+            stamp(PH_REST);
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks) frag3(xh, ks, ah[ks], al[ks]);
+            stamp(PH_ABUILD);
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
                 uint64_t bh, bl;
                 acquire(bh, bl);
+                stamp(PH_RING);
                 wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < 2; ++ks) mma3<64>(sub64(h, 64 * half), ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
+                stamp(PH_REST);
+                wg_commit_wait();
                 release();
+                stamp(PH_WAIT);
             }
         }
         // h1 = relu(D1 + b0), relu'(h1) bits: bit (4j + x) of the 128-bit mask, parked in shared memory until dh1
@@ -456,6 +525,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 for (int i = 0; i < 4; ++i) mask1s[i * NTHREADS + tid] = mask1[i];
             }
         }
+        stamp(PH_EPI1);
 
         // ---- layer 2 (two N halves) + output layer partial sums ----
         float ps0 = 0.f, ps1 = 0.f;
@@ -464,18 +534,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
             float d[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) d[i] = 0.f;
+            uint32_t ah[2][2][4], al[2][2][4];   // [set][k-step of the group]: 8 K-blocks of 4 k-steps, 16 groups
+            stamp(PH_REST);
+            gemm(
+                std::integral_constant<int, 16>{},
+                [&](int q) {
 #pragma unroll
-            for (int kb = 0; kb < 8; ++kb) {
-                uint32_t ah[4][4], al[4][4];
+                    for (int ks = 0; ks < 2; ++ks) frag3(h, 2 * q + ks, ah[q & 1][ks], al[q & 1][ks]);
+                },
+                [&](int q, uint64_t bh, uint64_t bl) {
 #pragma unroll
-                for (int ks = 0; ks < 4; ++ks) frag3(h, 4 * kb + ks, ah[ks], al[ks]);
-                uint64_t bh, bl;
-                acquire(bh, bl);
-                wg_fence();
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) mma3<64>(d, ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
-                release();
-            }
+                    for (int ks = 0; ks < 2; ++ks) {
+                        const int k = 2 * (q & 1) + ks;   // k-step inside the K-block
+                        mma3<64>(d, ah[q & 1][ks], al[q & 1][ks], bh + 2 * k, bl + 2 * k);
+                    }
+                });
             // relu'(h2) bits: bit (4j + x) of the 128-bit mask (j = 16 half + jj), words 2 half and 2 half + 1 of it
             uint32_t mask2[2] = {0u, 0u};
 #pragma unroll
@@ -494,6 +567,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                 mask2s[(2 * half) * NTHREADS + tid] = mask2[0];
                 mask2s[(2 * half + 1) * NTHREADS + tid] = mask2[1];
             }
+            stamp(PH_EPI2);
         }
         // the 4 threads of a quad hold the 4 column classes of the same two rows
         ps0 += __shfl_xor_sync(0xffffffffu, ps0, 1); ps0 += __shfl_xor_sync(0xffffffffu, ps0, 2);
@@ -542,6 +616,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
 #pragma unroll
                 for (int r = 0; r < 2; ++r) nl_seg_loss_add(p.stats, t == 0 ? seg_k[r] : -1, seg_fs[r], seg_sdf[r]);
             }
+            stamp(PH_LOSS);
             if constexpr (!TRAIN) continue;          // scoring: the tile ends with its loss
             // WGRAD: the activation buffer rows of this warpgroup leave through bulk copies from its staging area (dh1 quarter |
             // relu'(h2) words | dsdf).  The first warp's lanes issue them (two dh1 rows each, when dh1 is copied out at all); a staged
@@ -568,6 +643,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                     if (live0 && (m0 | 3) >= M) p.act_d[m0] = dsdf[0];
                     if (live1 && (m1 | 3) >= M) p.act_d[m1] = dsdf[1];
                 }
+                stamp(PH_WGRAD);
             }
             // stage dh1 columns 64 qq .. 64 qq + 63 (and with qq = 0 the relu'(h2) words, dsdf and the x tile) and start their copies
             auto stage_quarter = [&](int qq) {
@@ -670,29 +746,34 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
             // ---- backward layer 2: D3 = relu'(h2) . (diag(w2) W1).  The A operand is the 0/1 mask (exact in tf32: 2 terms) ----
 #pragma unroll
             for (int i = 0; i < 128; ++i) h[i] = 0.f;
+            // one pipeline over both N halves (groups 0..15: columns 0..127, 16..31: 128..255); K-block kb of a half holds k-steps
+            // 4 kb .. 4 kb + 3, whose mask bits are in word kb / 2
+            {
+                uint32_t a[2][2][4];   // [set][k-step of the group]
+                stamp(PH_REST);
+                gemm(
+                    std::integral_constant<int, 32>{},
+                    [&](int q) {
+                        const int kb = (q & 15) >> 1;
+                        const uint32_t wk = mask2s[(kb >> 1) * NTHREADS + tid];
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
+                        for (int ks = 0; ks < 2; ++ks) {
+                            const int j = 4 * kb + 2 * (q & 1) + ks;
+                            const uint32_t w = wk >> ((j & 7) * 4);
+                            uint32_t(&f)[4] = a[q & 1][ks];
+                            f[0] = (w & 1u) ? 0x3f800000u : 0u; f[1] = (w & 4u) ? 0x3f800000u : 0u;
+                            f[2] = (w & 2u) ? 0x3f800000u : 0u; f[3] = (w & 8u) ? 0x3f800000u : 0u;
+                        }
+                    },
+                    [&](int q, uint64_t bh, uint64_t bl) {
 #pragma unroll
-                for (int kb = 0; kb < 8; ++kb) {
-                    uint32_t a[4][4];
-                    const uint32_t wk = mask2s[(kb >> 1) * NTHREADS + tid];
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks) {
-                        const int j = 4 * kb + ks;
-                        const uint32_t w = wk >> ((j & 7) * 4);
-                        a[ks][0] = (w & 1u) ? 0x3f800000u : 0u; a[ks][1] = (w & 4u) ? 0x3f800000u : 0u;
-                        a[ks][2] = (w & 2u) ? 0x3f800000u : 0u; a[ks][3] = (w & 8u) ? 0x3f800000u : 0u;
-                    }
-                    uint64_t bh, bl;
-                    acquire(bh, bl);
-                    wg_fence();
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks) {
-                        wgmma_n128(sub64(h, 64 * half), a[ks][0], a[ks][1], a[ks][2], a[ks][3], bh + 2 * ks);
-                        wgmma_n128(sub64(h, 64 * half), a[ks][0], a[ks][1], a[ks][2], a[ks][3], bl + 2 * ks);
-                    }
-                    release();
-                }
+                        for (int ks = 0; ks < 2; ++ks) {
+                            const int k = 2 * (q & 1) + ks;
+                            const uint32_t(&f)[4] = a[q & 1][ks];
+                            wgmma_n128(sub64(h, 64 * (q >> 4)), f[0], f[1], f[2], f[3], bh + 2 * k);
+                            wgmma_n128(sub64(h, 64 * (q >> 4)), f[0], f[1], f[2], f[3], bl + 2 * k);
+                        }
+                    });
             }
             // dh1 = dsdf * D3 * relu'(h1)
 #pragma unroll
@@ -705,23 +786,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
                         h[4 * j + x] = ((m1w >> ((j & 7) * 4 + x)) & 1u) ? dsdf[x >> 1] * h[4 * j + x] : 0.f;
             }
             // ---- backward layer 1: d x = dh1 . W0 (N = 16); each dh1 quarter is staged (and copied out) before its two K-blocks,
-            // and its gW0 / gb0 terms run while the wgmmas of the first of them are in flight ----
+            // and its gW0 / gb0 terms run while the first commit group of the first of them is in flight ----
             float dx[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) dx[i] = 0.f;
+            {
+                uint32_t ah[2][2][4], al[2][2][4];   // [set][k-step of the group]: 8 K-blocks of 4 k-steps, 16 groups
+                stamp(PH_REST);
+                gemm(
+                    std::integral_constant<int, 16>{},
+                    [&](int q) {
+                        if (WGRAD && q % 4 == 0) { stage_quarter(q / 4); stamp(PH_WGRAD); }
 #pragma unroll
-            for (int kb = 0; kb < 8; ++kb) {
-                if (WGRAD && kb % 2 == 0) stage_quarter(kb / 2);
-                uint32_t ah[4][4], al[4][4];
+                        for (int ks = 0; ks < 2; ++ks) frag3(h, 2 * q + ks, ah[q & 1][ks], al[q & 1][ks]);
+                    },
+                    [&](int q, uint64_t bh, uint64_t bl) {
 #pragma unroll
-                for (int ks = 0; ks < 4; ++ks) frag3(h, 4 * kb + ks, ah[ks], al[ks]);
-                uint64_t bh, bl;
-                acquire(bh, bl);
-                wg_fence();
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) mma3<8>(dx, ah[ks], al[ks], bh + 2 * ks, bl + 2 * ks);
-                if (WGRAD && kb % 2 == 0) gw0_quarter(kb / 2);
-                release();
+                        for (int ks = 0; ks < 2; ++ks) {
+                            const int k = 2 * (q & 1) + ks;
+                            mma3<8>(dx, ah[q & 1][ks], al[q & 1][ks], bh + 2 * k, bl + 2 * k);
+                        }
+                        if (WGRAD && q % 4 == 0) { stamp(PH_REST); gw0_quarter(q / 4); stamp(PH_WGRAD); }
+                    });
             }
 #pragma unroll
             for (int jj = 0; jj < 2; ++jj) {
@@ -753,6 +839,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_mlp_wg(Params p) {
             if (loss_sdf != 0.0) atomicAdd(&p.stats->sdf_sum, loss_sdf);
         }
     }
+#ifdef NL_TC_STAMPS
+    stamp(PH_REST);
+    if ((tid & 127) == 0)
+        for (int i = 0; i < NPH; ++i) atomicAdd(&tc_stamps[tid >> 7][i], st_acc[i]);
+#endif
 }
 
 // The decoder weight gradients past layer 1 from x = feats, the relu'(h2) bits and dsdf; h1 is recomputed from x instead of stored.
@@ -1034,6 +1125,16 @@ int launch(const Params &p, cudaStream_t stream) {
 }
 
 }  // namespace tc
+
+#ifdef NL_TC_STAMPS
+// k_mlp_wg's phase counters (cycles summed over CTAs and launches), [2 warpgroups][tc::NPH] in StampPhase order, then zeroed
+extern "C" NL_API int nl_mlp_tc_stamps(unsigned long long *out) {
+    const unsigned long long zero[2 * tc::NPH] = {};
+    if (cudaMemcpyFromSymbol(out, tc::tc_stamps, sizeof(zero)) != cudaSuccess || cudaMemcpyToSymbol(tc::tc_stamps, zero, sizeof(zero)) != cudaSuccess)
+        return nl_set_error_code(NL_ERR_CUDA, "nl_mlp_tc_stamps");
+    return NL_OK;
+}
+#endif
 
 extern "C" int64_t nl_mlp_tc_panel_bytes(void) { return (int64_t)tc::STEPS_TRAIN * tc::STAGE_B; }
 
