@@ -75,10 +75,16 @@ def split(a):
 
 
 def trunc32(v):
-    """fp64 -> fp32 rounded toward zero."""
-    f = v.astype(np.float32)
-    over = np.abs(f.astype(np.float64)) > np.abs(v)
-    f[over] = np.nextafter(f[over], np.float32(0))
+    """fp64 -> fp32 rounded toward zero.  Where the result is a normal fp32, clearing the 29 low significand bits of the fp64
+    truncates it exactly; zeros, subnormals, overflow and NaN take the rounding route (round, then step back toward zero)."""
+    f = (np.ascontiguousarray(v, np.float64).view(np.uint64) & np.uint64(0xFFFFFFFFE0000000)).view(np.float64).astype(np.float32)
+    a = np.abs(v)
+    odd = ~((a >= 2.0 ** -126) & (a < 2.0 ** 128)) & (v != 0)
+    if odd.any():
+        r = v[odd].astype(np.float32)
+        over = np.abs(r.astype(np.float64)) > np.abs(v[odd])
+        r[over] = np.nextafter(r[over], np.float32(0))
+        f[odd] = r
     return f
 
 

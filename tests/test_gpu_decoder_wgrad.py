@@ -10,6 +10,7 @@ import ctypes as C
 import pytest
 import torch
 
+import decoder_wgrad_ref as W
 from util import golden, load_decoder
 
 pytestmark = pytest.mark.gpu
@@ -53,22 +54,12 @@ def _params64(dec):
 
 
 def fp64_grads(dec, x, g):
-    W0, b0, W1, b1, w2, b2 = _params64(dec)
-    out = [torch.zeros_like(p) for p in (W0, b0, W1, b1, w2, b2)]
+    """decoder_wgrad_ref.grads64 over chunks of samples, on the device."""
+    p = _params64(dec)
+    out = [torch.zeros_like(q) for q in p]
     for s in range(0, x.shape[0], 1 << 17):
-        xs, gs = x[s:s + (1 << 17)].double(), g[s:s + (1 << 17)].double()
-        z1 = xs @ W0.T + b0
-        h1 = z1.clamp_min(0)
-        z2 = h1 @ W1.T + b1
-        h2 = z2.clamp_min(0)
-        dz2 = gs[:, None] * w2[0] * (z2 > 0)
-        dz1 = (dz2 @ W1) * (z1 > 0)
-        out[0] += dz1.T @ xs
-        out[1] += dz1.sum(0)
-        out[2] += dz2.T @ h1
-        out[3] += dz2.sum(0)
-        out[4] += (gs[:, None] * h2).sum(0, keepdim=True)
-        out[5] += gs.sum().reshape(1)
+        for o, d in zip(out, W.grads64(x[s:s + (1 << 17)].double(), p, g[s:s + (1 << 17)].double())):
+            o += d
     return out
 
 
